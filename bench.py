@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Benchmark of the UniVL data-parallel training hot path on B200 (BASELINE.json metric: video-text samples/sec).
+"""Benchmark of the UniVL data-parallel training hot path on H100 (BASELINE.json metric: video-text samples/sec).
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path (N>1: launched under torchrun)
     python bench.py --impl reference --gpus N --steps K ...  # the reference algorithm on the host CPU cores
@@ -12,8 +12,14 @@ weights, dropout 0.1 active, random-init weights, synthetic (token-id, 1024-d S3
 
 One JSON line on stdout (rank 0).  `value` = whole-job samples/s with inputs resident in HBM; `e2e` = the same step
 driven from pinned HOST buffers (H2D of every input and D2H of the loss inside the timed region); `roofline` = the
-tcgen05 GEMM kernel's achieved TFLOP/s (CUDA events around its launches) against the measured bf16 peak;
+wgmma GEMM kernel's achieved TFLOP/s (CUDA events around its launches) against the bf16 peak;
 `cpu_baseline` = the CPU oracle (port of the reference algorithm) timed on this box's host cores on a bounded sample.
+
+`--dump-outputs DIR` (rank 0) writes what the last timed step computed as .npy files: `loss.npy`, and a fixed, seeded
+sample of the updated fp32 master weights (`params_sample.npy`) and of rank 0's fp32 gradients from that step's backward
+(`grads_sample.npy`; with one GPU these are the gradients the optimizer applied, with N > 1 the rank's local gradients
+before the all-reduce), with `sample_index.npy` (float64) giving the positions in the flat parameter vector.  Inputs,
+weights and dropout streams are seeded, so two builds run with the same arguments can be compared output for output.
 
 N > 1: the gradients travel as a bf16 payload that the optimizer reads directly; for more than 2 GPUs the backward is cut at
 text layer 6 (`--overlap_cuts`) so the all-reduce of the finished 61 % of the bytes runs under the rest of the backward
@@ -31,9 +37,9 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 
-# Measured (profiles/r02_overlap_sweep.md): cutting the backward at text layer 6 and all-reducing the finished 61 % of the
-# gradient bytes under the remaining backward gains 3.5 % at N=8 (NVLS all-reduce); at N=2 (ring all-reduce, SM copies)
-# the collective slows the backward by what it hides, so the cut is only taken for world > 2.
+# Cutting the backward at text layer 6 lets the all-reduce of the finished 61 % of the gradient bytes run under the
+# remaining backward; with two GPUs the collective slows the backward by what it hides, so the cut is only taken for
+# world > 2.
 AUTO_CUTS = "6"
 
 
@@ -63,6 +69,9 @@ def parse():
                     "the reservation the persistent kernels of the overlapped phases size their grids for")
     ap.add_argument("--graph", type=int, default=1, help="1: replay the step as one CUDA graph (falls back to eager "
                     "launches if capture fails), 0: eager")
+    ap.add_argument("--dump-outputs", dest="dump_outputs", default=None, metavar="DIR",
+                    help="write the loss and a seeded sample of the updated weights and gradients of the last timed "
+                    "step to DIR/<name>.npy (float32)")
     return ap.parse_args()
 
 
@@ -79,7 +88,7 @@ def peaks():
         with open(path) as fh:
             d = json.load(fh)
         return float(d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1400.0))), "measured (MEASURED_PEAKS.json, sustained)"
-    return 1400.0, "fallback (B200_PROFILING.md sustained bf16)"
+    return 989.0, "H100 SXM data sheet, dense bf16 at 700 W (not reached by any measured kernel)"
 
 
 class ClockSampler(threading.Thread):
@@ -261,6 +270,26 @@ def run_reference_arm(a, budget_s=270.0):
 
 
 # ---------------------------------------------------------------------------------------------------------
+DUMP_SAMPLE = 1 << 21   # elements of the weight / gradient samples: 2 x 8 MB of float32 plus a 16 MB index
+
+
+def dump_outputs(out_dir, loss, flat_params, flat_grads):
+    """the last timed step's loss and a fixed, seeded sample of the flat fp32 weights and gradients -> out_dir/*.npy"""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    n = flat_params.numel()
+    g = torch.Generator().manual_seed(20240)
+    idx = torch.randint(0, n, (DUMP_SAMPLE,), generator=g).sort().values
+    idx_dev = idx.to(flat_params.device)
+    arrays = {"loss": loss.detach().float().reshape(1).cpu(),
+              "params_sample": flat_params.index_select(0, idx_dev).float().cpu(),
+              "grads_sample": flat_grads.index_select(0, idx_dev).float().cpu(),
+              "sample_index": idx.double()}
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.numpy())
+
+
 def main():
     a = parse()
     if a.impl == "reference":
@@ -477,6 +506,8 @@ def main():
     ms = e0.elapsed_time(e1) / a.steps
     launches = (launches_per_step * a.steps) if graphed else (rt.launch_count() - launches0)
     loss_val = float(loss.detach())
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, loss, opt.p, opt.g)
 
     # where a multi-GPU step goes (rank 0's device clock, 5 extra steps outside the timed region)
     breakdown = None
@@ -545,11 +576,10 @@ def main():
         sampler.stop_flag = True
         sampler.join(timeout=3)
 
-    # ---- roofline of the dominant kernel: CUDA events around every tcgen05 GEMM launch on the launching stream ----
-    # The dominant kernel is the CTA-pair GEMM (gemm_tcgen05_2cta_kernel, ~49% of the step in profiles/); the library
-    # reports which variant each call launched, so its launches are separated from the single-CTA persistent ones.
+    # ---- roofline of the dominant kernel: CUDA events around every wgmma GEMM launch on the launching stream ----
+    # univl_gemm_plan reports which kernel each call launches (today always 1, the persistent wgmma kernel).
     from univl_b200 import lib as _lib
-    prof = {2: {"flops": 0.0, "events": []}, 1: {"flops": 0.0, "events": []}, 0: {"flops": 0.0, "events": []}}
+    prof = {1: {"flops": 0.0, "events": []}}
     orig_gemm = ops.gemm
 
     def timed_gemm(a_, b_, M, N, K, out, *args, **kw):
@@ -615,23 +645,9 @@ def main():
         ms_k = sum(s.elapsed_time(e) for s, e in v["events"])
         per[k] = {"ms": ms_k, "n": len(v["events"]), "flops": v["flops"],
                   "tflops": v["flops"] / (ms_k * 1e-3) / 1e12 if ms_k > 0 else 0.0}
-    dom = per[2] if per[2]["n"] else per[1]
+    dom = per[1]
     gemm_ms, n_gemm, achieved = dom["ms"], dom["n"], dom["tflops"]
-    all_ms = sum(v["ms"] for v in per.values())
-    all_flops = sum(v["flops"] for v in per.values())
     peak, peak_src = peaks()
-    traffic, pipe_util = None, None
-    try:
-        with open(os.path.join(ROOT, "profiles", "r01_roofline_traffic.json")) as f:
-            captured = json.load(f)
-        traffic = captured.get("traffic_bytes_per_launch")
-        pipe_util = captured.get("tensor_pipe_util_pct")  # BASELINE's second metric: ncu figures, not timed here
-        r02 = os.path.join(ROOT, "profiles", "r02_fused_attn_pipe.json")
-        if os.path.exists(r02):
-            with open(r02) as f:
-                pipe_util = json.load(f)
-    except (OSError, ValueError):
-        pass
 
     # max over ranks
     t = torch.tensor([ms, ms_e2e if not a.no_e2e else 0.0], device=dev, dtype=torch.float64)
@@ -654,30 +670,17 @@ def main():
                        a.grad_payload, "after backward" if phased is None or not graphed else
                        "overlapped with backward: %d phases cut at text layers %s" % (phased.n_phases, phased.cuts))),
                    "launch": "cuda-graph replay" if graphed else "eager",
-                   "l2": "per-step working set (~6 GB of activations at FT-Align b=32) exceeds the 126 MB L2"},
+                   "l2": "per-step working set (~6 GB of activations at FT-Align b=32) exceeds the 50 MB L2"},
         "gpu_launches": launches, "loss": loss_val,
         **({"step_breakdown_ms": breakdown} if breakdown else {}),
         "roofline": {"bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TFLOP/s",
-                     "frac": achieved / peak if peak else None, "traffic": traffic,
-                     "kernel": "gemm_tcgen05_2cta_kernel" if per[2]["n"] else "gemm_tcgen05_persistent_kernel",
+                     "frac": achieved / peak if peak else None,
+                     "kernel": "gemm_wgmma_kernel",
                      "launches_per_step": n_gemm / max(1, a.profile_steps),
                      "gemm_ms_per_step": gemm_ms / max(1, a.profile_steps), "peak_source": peak_src,
-                     "algorithmic_flops_per_step": dom["flops"] / max(1, a.profile_steps),
-                     "traffic_source": "ncu --set full capture summarised in profiles/r01_ncu_full_gemm_cross.txt"
-                                       " (mean dram read+write bytes per launch of the cross-encoder launches)",
-                     "all_gemm_kernels": {"tflops": all_flops / (all_ms * 1e-3) / 1e12 if all_ms > 0 else 0.0,
-                                          "ms_per_step": all_ms / max(1, a.profile_steps),
-                                          "launches_per_step": sum(v["n"] for v in per.values())
-                                          / max(1, a.profile_steps)},
-                     "persistent_kernel": {"tflops": per[1]["tflops"],
-                                           "ms_per_step": per[1]["ms"] / max(1, a.profile_steps),
-                                           "launches_per_step": per[1]["n"] / max(1, a.profile_steps)},
-                     "note": "256x256 CTA-pair tiles move 32 KB of operands per CTA per 64-deep k-block (128 flop/B): "
-                             "L2->SM delivery (~12 TB/s) caps them near 1.5 PFLOP/s, the same regime as the cuBLAS "
-                             "peak used here"},
+                     "algorithmic_flops_per_step": dom["flops"] / max(1, a.profile_steps)},
         "clocks": sampler.summary() if sampler else None,
         "fused_attention": fa_out,
-        "tensor_pipe_util_pct": pipe_util,
     }
     if not a.no_e2e:
         line["e2e"] = {"value": samples / (ms_e2e_max * 1e-3), "unit": "samples/s", "h2d_bytes_per_step": h2d_bytes,

@@ -1,4 +1,4 @@
-/* univl_b200 — C ABI of the B200-native UniVL hot path (libunivl_b200.so, sm_100a).
+/* univl_b200 — C ABI of the H100-native UniVL hot path (libunivl_b200.so, sm_90a).
  *
  * The reference (microsoft/UniVL) has no FFI: its "plugin API" is the Python class surface of
  * modules/modeling.py (UniVL.forward :188-271 etc.), which univl_b200/modules/ mirrors.  This header is the new
@@ -23,12 +23,12 @@ extern "C" {
 const char* univl_last_error_string(void);
 int univl_abi_version(void);
 /* Number of SMs a concurrent collective kernel (NCCL all-reduce on another stream) occupies while the kernels enqueued
- * from now on run; persistent grids (GEMM, fused attention) are sized to the remaining SMs / SM pairs.  0 = none
+ * from now on run; persistent grids (GEMM, fused attention) are sized to the remaining SMs.  0 = none
  * (default).  Process-wide; read at enqueue time (captured graphs keep their grids).
  * No reference counterpart: DDP's overlapped bucket all-reduce (main_task_retrieval.py:197) leaves this to cuBLAS. */
 int univl_set_reserved_sms(int n);
 
-/* ---- GEMM (tcgen05 / TMEM / TMA) -------------------------------------------------------------------------
+/* ---- GEMM (wgmma / TMA) ---------------------------------------------------------------------------------
  * D[M,N] = epilogue(sum_k A(m,k) B(n,k)), bf16 operands, fp32 accumulation.
  * A is [M,Kc] row-major (a_mn_major=0) or [Kc,M] row-major (a_mn_major=1); likewise B with N.
  * Replaces every nn.Linear forward / dgrad / wgrad of the hot path:
@@ -37,13 +37,13 @@ int univl_set_reserved_sms(int n);
  *   module_visual.py:308-311 (MFM projection), modeling.py:285 (MFM logits), module_cross.py:284 (pooler).
  * epilogue: 0 out(bf16)=alpha*acc+bias | 1 aux_out(bf16)=acc+bias, out(bf16)=gelu_erf(.) (until_module.py:28-33)
  *           2 out(bf16)=acc*gelu'(aux_in) | 3 out(bf16)=alpha*acc+aux_in | 4 out(f32)=alpha*acc+bias
- *           5 out(f32)+=alpha*acc (atomic; split-K and gradient accumulation)
+ *           5 out(f32)+=alpha*acc (gradient accumulation; split-K partials are summed in split order)
  * block_n: 0 = auto | 64 | 128 | 256.  split_k: 0 = auto (epilogue 5 only). */
 int univl_gemm_bf16(const void* A, long long lda, int a_mn_major, const void* B, long long ldb, int b_mn_major,
                     int M, int N, int Kc, void* out, long long ldo, int epilogue, const float* bias,
                     const void* aux_in, long long ld_aux_in, void* aux_out, long long ld_aux_out, float alpha,
                     int block_n, int split_k, void* stream);
-/* kernel variant univl_gemm_bf16 launches for this problem: 2 CTA-pair, 1 single-CTA persistent, 0 bring-up; a pure
+/* kernel variant univl_gemm_bf16 launches for this problem: 1 = the persistent wgmma kernel (the only one); a pure
  * function of its arguments (measurement aid: bench.py attributes launch times to the dominant kernel with it) */
 int univl_gemm_plan(int M, int N, int Kc, int epilogue, int block_n, int split_k);
 
@@ -99,7 +99,7 @@ int univl_attention_bwd(const void* q, long long ldq, const void* k, long long l
                         const long long* mask_b, int Wa, int Fb, int Nb, int all_pairs, int n_seq, int heads, int Sq,
                         int Sk, int causal, float scale, float p_drop, const unsigned long long* rng_state,
                         unsigned long long stream_id, int rng_layout, float* dbq, float* dbk, float* dbv, void* stream);
-/* ---- fused QKV projection + self-attention, forward (tcgen05 / TMEM / TMA; module_bert.py:171-197 as ONE kernel) ----
+/* ---- fused QKV projection + self-attention, forward (wgmma / TMA; module_bert.py:171-197 as ONE kernel) --------------
  * ctx[T,H] = merge_heads(dropout(softmax((x Wq^T + bq)(x Wk^T + bk)^T * scale + mask)) (x Wv^T + bv)), T = n_seq * S,
  * H = heads * 64 = 768.  wqkv: bf16 [3H, H] (query | key | value rows), bias fp32 [3H].  The [T,3H] projections and the
  * score matrices stay on chip; qkv_out (nullable) additionally receives bf16 q | k | v for the backward pass.  Supported
@@ -111,7 +111,7 @@ int univl_fused_qkv_attention_fwd(const void* x, long long ldx, const void* wqkv
                                   const long long* mask_a, const long long* mask_b, int Wa, int Fb, int Nb,
                                   int all_pairs, int n_seq, int heads, int S, int causal, float scale, float p_drop,
                                   const unsigned long long* rng_state, unsigned long long stream_id, void* stream);
-/* backward of the attention core for the same shapes, on tcgen05 (S, dP, dS, P in TMEM / shared memory only):
+/* backward of the attention core for the same shapes, on wgmma (S, dP, dS, P in registers / shared memory only):
  * dqkv[T,3H] = d(q | k | v) from the saved qkv, the context o, d_o and lse; dbias (nullable, fp32 [3H]) accumulates the
  * projection-bias gradients (column sums).  Masks / dropout as the fused forward (row-major dropout layout). */
 int univl_fused_attention_bwd(const void* qkv, long long ld_qkv, const void* o, long long ldo, const float* lse,

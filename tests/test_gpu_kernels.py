@@ -44,7 +44,7 @@ def test_gemm_all_operand_majors(a_mn, b_mn, shape):
 
 def test_reserved_sms_shrink_persistent_grids_not_results():
     """univl_set_reserved_sms: persistent kernels launched while a collective holds SMs use fewer CTAs (each walks more
-    tiles); every output is unchanged — GEMM (1-CTA and CTA-pair tiles) and the fused attention forward / backward."""
+    tiles); every output is unchanged — GEMM (several tile widths) and the fused attention forward / backward."""
     g = torch.Generator(device=DEV).manual_seed(4)
     cases = [(1536, 768, 768), (2560, 3072, 768), (300, 200, 136)]
     mats = [(_bf(torch.randn(M, K, device=DEV, generator=g) * 0.5), _bf(torch.randn(N, K, device=DEV, generator=g) * 0.5))
@@ -284,7 +284,7 @@ def _fused_inputs(n_seq, S, seed):
                                             (9, 16, True), (4, 32, False), (3, 64, False), (2, 80, False), (1, 112, False),
                                             (40, 96, False), (301, 48, False)])
 def test_fused_qkv_attention_fwd_matches_unfused_and_fp32(n_seq, S, causal):
-    """ONE tcgen05 kernel (projection + softmax(QK^T)V) against (a) fp32 PyTorch on the same bf16 inputs and (b) the
+    """ONE wgmma kernel (projection + softmax(QK^T)V) against (a) fp32 PyTorch on the same bf16 inputs and (b) the
     QKV-GEMM + attention-core pair; packed sequences (S = 16 ... 64), partial last row block, several items per CTA."""
     H, h = 768, 12
     assert ops.fused_attention_supported(n_seq, S, H)
@@ -322,7 +322,7 @@ def test_fused_qkv_attention_fwd_matches_unfused_and_fp32(n_seq, S, causal):
                                               (40, 96, False, 0.0), (3, 48, False, 0.25), (2, 128, False, 0.25),
                                               (301, 48, False, 0.1)])
 def test_fused_attention_bwd_matches_fp32_and_unfused_backward(n_seq, S, causal, p):
-    """tcgen05 attention backward: (p = 0) against fp32 autograd of the same op, and (any p) against the mma.sync
+    """wgmma attention backward: (p = 0) against fp32 autograd of the same op, and (any p) against the mma.sync
     backward kernel regenerating the same row-major dropout mask; bias-gradient column sums included."""
     H, h = 768, 12
     x, w, b, mask = _fused_inputs(n_seq, S, 100 + S + n_seq)

@@ -1,4 +1,4 @@
-"""Build libunivl_b200.so (sm_100a) in-tree with nvcc.
+"""Build libunivl_b200.so (sm_90a) in-tree with nvcc.
 
 The shared library is the C-ABI boundary (include/univl_b200.h); it links cudart statically and does
 not link libcuda, so it loads on a GPU-less host (the CPU test-suite checks its exported symbols).
@@ -15,7 +15,7 @@ LIB = os.path.join(HERE, "libunivl_b200.so")
 STAMP = os.path.join(HERE, "csrc", ".build_stamp")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "--use_fast_math",
     "-Xcompiler", "-fPIC",
@@ -66,7 +66,7 @@ def build(force=False, verbose=False):
             sys.stderr.write(out)
     if failed:
         raise RuntimeError("univl_b200: nvcc compilation failed")
-    link = [nvcc, "-shared", "-cudart", "static", "-gencode", "arch=compute_100a,code=sm_100a",
+    link = [nvcc, "-shared", "-cudart", "static", "-gencode", "arch=compute_90a,code=sm_90a",
             "-o", LIB, *objs]
     subprocess.check_call(link)
     with open(STAMP, "w") as fh:

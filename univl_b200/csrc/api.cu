@@ -31,23 +31,62 @@ bool pdl_enabled() {
 // of every persistent kernel under the collective.  Read at enqueue time, so it is baked into captured graphs.
 static int g_reserved_sms = 0;
 
-int usable_sms() {
+int device_sms() {
   static int sms = 0;
   if (sms == 0) {
-    int dev = 0, n = 148;
+    int dev = 0, n = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
     sms = n;
   }
-  const int n = sms - g_reserved_sms;
+  return sms;
+}
+
+int usable_sms() {
+  const int n = device_sms() - g_reserved_sms;
   return n < 8 ? 8 : n;
 }
 
-// CTA pairs need both SMs of a TPC: every reserved SM may sit in a different TPC
-int usable_sm_pairs() {
-  const int all = (usable_sms() + g_reserved_sms) / 2;
-  const int n = all - g_reserved_sms;
-  return n < 4 ? 4 : n;
+int scratch_alloc(void** p, size_t bytes, cudaStream_t st) {
+  static bool pool_ready[64] = {};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev < 64 && !pool_ready[dev]) {
+    // keep freed scratch in the device's default pool instead of returning it at every synchronisation
+    cudaMemPool_t pool;
+    if (cudaDeviceGetDefaultMemPool(&pool, dev) == cudaSuccess) {
+      uint64_t keep = ~0ull;
+      cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
+    }
+    pool_ready[dev] = true;
+  }
+  const cudaError_t e = cudaMallocAsync(p, bytes < 16 ? 16 : bytes, st);
+  if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "scratch allocation of %zu bytes: %s", bytes, cudaGetErrorString(e));
+  return UNIVL_OK;
+}
+
+__global__ void __launch_bounds__(256)
+partials_reduce_kernel(const float* __restrict__ part, int nparts, long long rows, long long cols, float* __restrict__ dst,
+                       long long ld) {
+  const long long n = rows * cols;
+  for (long long i = blockIdx.x * 256LL + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+    float t = 0.f;
+    for (int k = 0; k < nparts; ++k) t += part[(long long)k * n + i];
+    const long long r = i / cols, c = i - r * cols;
+    dst[r * ld + c] += t;
+  }
+}
+
+int partials_reduce(float* part, int nparts, long long rows, long long cols, float* dst, long long ld, cudaStream_t st) {
+  const long long n = rows * cols;
+  long long blocks = (n + 255) / 256;
+  if (blocks > device_sms() * 8LL) blocks = device_sms() * 8LL;
+  if (blocks < 1) blocks = 1;
+  partials_reduce_kernel<<<(int)blocks, 256, 0, st>>>(part, nparts, rows, cols, dst, ld);
+  const cudaError_t e = cudaGetLastError();
+  cudaFreeAsync(part, st);
+  if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "partials_reduce launch: %s", cudaGetErrorString(e));
+  return UNIVL_OK;
 }
 
 }  // namespace univl

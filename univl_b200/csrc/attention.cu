@@ -8,7 +8,7 @@
 // d = 64, whole K/V of one (sequence, head) live in shared memory, so softmax is exact two-pass (max+sum, then
 // normalised P) and nothing of the [B, h, S, S] score tensor ever reaches HBM.  Tensor work uses warp-level
 // mma.sync m16n8k16 bf16 (the S x S x 64 products are ~4 % of a layer's FLOPs; the projections around them run on
-// tcgen05 — see gemm_tcgen05.cu).  One CTA per (sequence, head); each warp owns 16 query rows (or 16 key rows in the
+// wgmma — see gemm_wgmma.cu).  One CTA per (sequence, head); each warp owns 16 query rows (or 16 key rows in the
 // dK/dV pass of backward) at a time.  Backward recomputes P from Q, K and the saved log-sum-exp, flash-style, with
 // no atomics: dQ is produced by query-row tasks, dK/dV by key-row tasks that recompute the transposed tiles.
 // Dropout masks are Philox(seed, stream, element) and regenerated identically in every pass.
@@ -727,7 +727,7 @@ attention_bwd_kernel(const AttnParams p_in) {
       float v = 0.f;
       for (int k = 0; k < n; ++k) v += src[k * 64];
       float* dst = kind == 0 ? p.dbq : kind == 1 ? p.dbk : p.dbv;
-      if (v != 0.f) atomicAdd(dst + h * HD + col, v);
+      dst[(long long)seq * p.heads * HD + h * HD + col] = v;  // this sequence's partial row
     }
   }
 }
@@ -824,7 +824,6 @@ extern "C" int univl_attention_bwd(const void* q, long long ldq, const void* k, 
   p.lddq = lddq; p.lddk = lddk; p.lddv = lddv;
   UNIVL_CHECK_ARG((dbq == nullptr) == (dbk == nullptr) && (dbq == nullptr) == (dbv == nullptr),
                   "attention_bwd: bias-gradient pointers must be all set or all null");
-  p.dbq = dbq; p.dbk = dbk; p.dbv = dbv;
   const int Sq16 = (Sq + 15) & ~15, Sk16 = (Sk + 15) & ~15;
   size_t smem = (size_t)(2 * Sq16 + 2 * Sk16) * LDS * 2 + (size_t)(Sk16 + 2 * Sq16 + (Sq16 / 16 + 2 * (Sk16 / 16)) * 64) * 4;
   p.share_tiles = (Sq16 <= 128 && Sk16 <= 128) ? 1 : 0;
@@ -840,7 +839,19 @@ extern "C" int univl_attention_bwd(const void* q, long long ldq, const void* k, 
   int tasks = Sq16 / 16 + Sk16 / 16;
   if (p.share_tiles) tasks = Sq16 / 16 > Sk16 / 16 ? Sq16 / 16 : Sk16 / 16;  // the two passes run one after the other
   const int bwd_warps = tasks < ATT_BWD_WARPS ? tasks : ATT_BWD_WARPS;
-  launch_kernel(attention_bwd_kernel, dim3(n_seq * heads), dim3(bwd_warps * 32), smem, (cudaStream_t)stream, p);
+  // bias gradients: one partial row per sequence, summed in sequence order after the kernel
+  cudaStream_t st = (cudaStream_t)stream;
+  float* outs[3] = {dbq, dbk, dbv};
+  float* parts[3] = {nullptr, nullptr, nullptr};
+  if (dbq != nullptr)
+    for (int w = 0; w < 3; ++w)
+      if (int rc = scratch_alloc((void**)&parts[w], (size_t)n_seq * heads * HD * sizeof(float), st)) return rc;
+  p.dbq = parts[0]; p.dbk = parts[1]; p.dbv = parts[2];
+  launch_kernel(attention_bwd_kernel, dim3(n_seq * heads), dim3(bwd_warps * 32), smem, st, p);
   UNIVL_CHECK_LAUNCH("attention_bwd");
+  if (dbq != nullptr)
+    for (int w = 0; w < 3; ++w)
+      if (int rc = partials_reduce(parts[w], n_seq, 1, (long long)heads * HD, outs[w], (long long)heads * HD, st))
+        return rc;
   return UNIVL_OK;
 }

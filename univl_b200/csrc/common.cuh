@@ -1,7 +1,7 @@
-// univl_b200 — shared device helpers for the sm_100a kernels.
+// univl_b200 — shared device helpers for the sm_90a kernels.
 //
-// Thin inline-PTX wrappers for the Blackwell primitives the kernels use
-// (mbarrier, TMA bulk-tensor copies, tcgen05 MMA / TMEM), plus small math and
+// Thin inline-PTX wrappers for the Hopper primitives the kernels use
+// (mbarrier, TMA bulk-tensor copies, wgmma), plus small math and
 // packing helpers.  Everything here is header-only and device-side except the
 // error-string plumbing at the bottom.
 #pragma once
@@ -20,8 +20,14 @@ typedef __nv_bfloat16 bf16;
 // error plumbing shared by all translation units (defined in api.cu)
 // ----------------------------------------------------------------------------
 int set_error(int code, const char* fmt, ...);
+int device_sms();        // SM count of the current device (api.cu)
 int usable_sms();        // SM count minus univl_set_reserved_sms (api.cu)
-int usable_sm_pairs();  // TPCs with both SMs free under the same reservation
+// Deterministic cross-CTA sums: a kernel writes one partial row per contributor into stream-ordered scratch memory
+// (cudaMallocAsync, capturable in CUDA graphs) instead of adding atomically; partials_reduce adds the rows to dst in
+// contributor order and frees the scratch, so every run sums in the same order.  (api.cu)
+int scratch_alloc(void** p, size_t bytes, cudaStream_t st);
+// dst[r * ld + c] += sum over k in [0, nparts) of part[k * rows * cols + r * cols + c], k ascending; frees part
+int partials_reduce(float* part, int nparts, long long rows, long long cols, float* dst, long long ld, cudaStream_t st);
 #define UNIVL_OK 0
 #define UNIVL_ERR_ARG -1
 #define UNIVL_ERR_CUDA -2
@@ -52,35 +58,23 @@ __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.lau
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
 template <typename... KArgs, typename... Args>
-static inline cudaError_t launch_kernel_cluster(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem,
-                                                cudaStream_t st, int cluster_x, Args... args) {
+static inline cudaError_t launch_kernel(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
+                                        Args... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
-  cudaLaunchAttribute attr[2];
+  cudaLaunchAttribute attr[1];
   int n = 0;
   if (pdl_enabled()) {
     attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[n].val.programmaticStreamSerializationAllowed = 1;
     ++n;
   }
-  if (cluster_x > 1) {
-    attr[n].id = cudaLaunchAttributeClusterDimension;
-    attr[n].val.clusterDim.x = (unsigned)cluster_x;
-    attr[n].val.clusterDim.y = 1;
-    attr[n].val.clusterDim.z = 1;
-    ++n;
-  }
   cfg.attrs = attr;
   cfg.numAttrs = n;
   return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
-}
-template <typename... KArgs, typename... Args>
-static inline cudaError_t launch_kernel(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
-                                        Args... args) {
-  return launch_kernel_cluster(kern, grid, block, smem, st, 1, args...);
 }
 
 // ----------------------------------------------------------------------------
@@ -235,30 +229,14 @@ __device__ __forceinline__ uint32_t mbar_try_wait(uint64_t* bar, uint32_t parity
       : "memory");
   return ok;
 }
-// non-suspending probe (mbarrier.try_wait may put the thread to sleep for a system-dependent time when the phase is not
-// complete: fine for a blocking wait, wrong for a scheduler that polls several barriers)
-__device__ __forceinline__ uint32_t mbar_test_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.b32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok;
-}
 // Bounded wait: a pipeline bug must surface as a trap (launch failure), never as
 // a hung GPU.  try_wait already suspends in hardware, so the spin count stays low
-// in healthy runs; 1<<26 polls is many seconds.
+// in healthy runs; 1<<26 polls is many seconds.  No printf here: a function call inside the wgmma consumer loops makes
+// ptxas serialise every wgmma (C7510), so the timeout is reported by the trap alone.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if (++spins > (1u << 26)) {
-      printf("univl: mbarrier wait timed out (block %d,%d,%d thread %d)\n", blockIdx.x, blockIdx.y,
-             blockIdx.z, threadIdx.x);
-      __trap();
-    }
+    if (++spins > (1u << 26)) __trap();
   }
 }
 
@@ -276,36 +254,11 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
-// multicast variant: the box lands at the same shared-memory offset of every CTA in cta_mask (bit i = cluster rank i) and
-// completes tx bytes on the mbarrier at the same offset in each of them
-__device__ __forceinline__ void tma_load_2d_mc(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                               uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%2, %3}], [%4], %5;"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1), "r"(smem_u32(bar)), "h"(cta_mask)
-      : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_rank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_barrier() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
 
 // ---- TMA stores (shared -> global) -----------------------------------------------------------------------------
 // bulk tensor store / reduce of one staging box; coordinates {inner (column), outer (row)}
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src, int c0, int c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.tile.bulk_group [%0, {%1, %2}], [%3];" ::"l"(
-                   reinterpret_cast<uint64_t>(m)),
-               "r"(c0), "r"(c1), "r"(smem_u32(smem_src))
-               : "memory");
-}
-__device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* m, const void* smem_src, int c0, int c1) {
-  asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%1, %2}], [%3];" ::"l"(
                    reinterpret_cast<uint64_t>(m)),
                "r"(c0), "r"(c1), "r"(smem_u32(smem_src))
                : "memory");
@@ -319,18 +272,9 @@ __device__ __forceinline__ void bulk_wait_read() {
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // ----------------------------------------------------------------------------
-// tcgen05 / TMEM
+// Hopper warpgroup MMA (wgmma) plumbing
 // ----------------------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before_sync() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after_sync() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// One lane of a fully converged warp (elect.sync).  The MMA-issuing warp runs its loop with ALL lanes (warp-uniform
-// control flow keeps addresses / descriptors in uniform registers) and wraps only the tcgen05.mma / commit instructions
-// in `if (elect_one())`; an `if (lane == 0)` region around the whole loop makes the compiler re-broadcast every operand
-// (ELECT + R2UR per instruction), which measurably throttles the single issuing thread.
+// One lane of a fully converged warp (elect.sync), for the single-thread TMA issue of a producer warp.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(
@@ -340,71 +284,41 @@ __device__ __forceinline__ bool elect_one() {
       : "=r"(pred));
   return pred != 0;
 }
-// whole warp; writes the TMEM base address to *smem_slot
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_slot, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_slot)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
+// keeps the compiler from moving reads / writes of an accumulator across the asynchronous MMA region
+template <int R>
+__device__ __forceinline__ void fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// D[tmem] (+)= A[smem desc] * B[smem desc]; single thread issues
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
+// register budget of a warpgroup (producer warpgroups give theirs to the MMA warpgroups)
+template <int N>
+__device__ __forceinline__ void regs_dealloc() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
 }
-// arrive on an mbarrier once all previously issued MMAs of this thread retire
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+template <int N>
+__device__ __forceinline__ void regs_alloc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
 }
-// same, arriving on the barrier at this shared-memory offset in every CTA of cta_mask (cluster ranks)
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(smem_u32(bar)), "h"(cta_mask)
-      : "memory");
-}
-// 32 lanes x 16 consecutive fp32 columns: thread t of the warp reads TMEM lane (base_lane + t)
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// Instruction descriptor, kind::f16, bf16 x bf16 -> fp32 (bit layout: CUTLASS
-// cute/arch/mma_sm100_desc.hpp UMMA::InstrDescriptor).
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, bool a_mn_major, bool b_mn_major) {
-  return (1u << 4)                          // c_format = F32
-         | (1u << 7)                        // a_format = BF16
-         | (1u << 10)                       // b_format = BF16
-         | ((a_mn_major ? 1u : 0u) << 15)   // a_major
-         | ((b_mn_major ? 1u : 0u) << 16)   // b_major
-         | ((uint32_t)(N >> 3) << 17)       // n_dim
-         | ((uint32_t)(M >> 4) << 24);      // m_dim
+// named barrier over `count` threads (ids 1..15; 0 is __syncthreads)
+__device__ __forceinline__ void named_bar(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
-// Shared-memory matrix descriptor, SWIZZLE_128B (UMMA::SmemDescriptor): start
-// address, leading/stride byte offsets all in 16-byte units, version=1 (sm_100).
-__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes,
-                                                         uint32_t sbo_bytes) {
+// Shared-memory matrix descriptor of a 128B-swizzled operand (sm_90 GmmaDescriptor): start address, leading / stride
+// byte offsets in 16-byte units, layout type 1 = SWIZZLE_128B.  K-major: SBO = 1024 (8 rows of 128 B), LBO unused.
+// MN-major: LBO = distance between 64-element MN blocks, SBO = 1024 (8 k-rows of 128 B).
+__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFFu);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;  // version
-  d |= (uint64_t)2 << 61;  // layout_type = SWIZZLE_128B
+  d |= (uint64_t)1 << 62;  // layout_type = SWIZZLE_128B
   return d;
 }
 

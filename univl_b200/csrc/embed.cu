@@ -8,8 +8,9 @@
 //             modules/modeling.py:315-325; in all-pairs mode sequence p = (i, j) = (p / Nb, p % Nb) reads text i and
 //             video j in place — the `repeat`ed [B*B, W+F, H] input of modeling.py:358-367 is never materialised.
 // The tables are the fp32 master parameters (no bf16 copy is needed for a gather).  Backward recomputes the pre-LN
-// row, runs the LayerNorm backward and scatters: atomics into the fp32 table gradients, direct bf16 writes (summed in
-// registers over the pairs that share a source row) into the activation gradients.
+// row and runs the LayerNorm backward: each row's table gradient goes to scratch memory and is summed per table row in
+// row order (keyed_rows_sum_kernel); the activation gradients are direct bf16 writes (summed in registers over the
+// pairs that share a source row).
 #include "common.cuh"
 
 namespace univl {
@@ -149,43 +150,38 @@ __device__ __forceinline__ void flush_colsums(float (&acc)[EMB_VEC][8], float* d
       float t = 0.f;
 #pragma unroll
       for (int w = 0; w < EMB_WARPS; ++w) t += red[w][e];
-      if (t != 0.f) atomicAdd(dst + i * 256 + e, t);
+      dst[((long long)blockIdx.y * gridDim.x + blockIdx.x) * EMB_H + i * 256 + e] = t;  // this CTA's partial row
     }
   }
 }
 
-// Table-gradient accumulation.  Hundreds of token rows share one position row and practically all share one type row,
-// so per-element atomics serialise in L2 (measured: the two embedding backward kernels spent most of their 0.5 ms
-// there).  Each warp instead walks rows whose position index is constant (the row stride is a multiple of the sequence
-// length), keeps the position / type sums in registers and flushes when the key changes or at the end.
-struct KeyedAcc {
-  float v[EMB_VEC][8];
-  int key;
-};
-__device__ __forceinline__ void keyed_init(KeyedAcc& a) {
-  a.key = -1;
-#pragma unroll
-  for (int i = 0; i < EMB_VEC; ++i)
-#pragma unroll
-    for (int j = 0; j < 8; ++j) a.v[i][j] = 0.f;
+// Table gradients (word / position / type rows): every row's gradient dz and its table keys go to scratch memory and
+// keyed_rows_sum_kernel adds, per key, the rows in row order — the same sums in the same order on every run.
+__device__ __forceinline__ void st8f(float* p, const float (&v)[8]) {
+  *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]);
+  *reinterpret_cast<float4*>(p + 4) = make_float4(v[4], v[5], v[6], v[7]);
 }
-__device__ __forceinline__ void keyed_flush(KeyedAcc& a, float* table, int lane) {
-  if (a.key < 0) return;
-#pragma unroll
-  for (int i = 0; i < EMB_VEC; ++i) {
-    float* dst = table + (long long)a.key * EMB_H + (i * 32 + lane) * 8;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      atomicAdd(dst + j, a.v[i][j]);
-      a.v[i][j] = 0.f;
+// dst[key * H + c] += sum of src[r * H + c] over the rows r whose key is `key` (ascending r); key < 0: no table row
+__global__ void __launch_bounds__(256)
+keyed_rows_sum_kernel(const float* __restrict__ src, const int* __restrict__ key, long long rows, float* __restrict__ dst) {
+  for (long long r = blockIdx.x; r < rows; r += gridDim.x) {
+    const int k = key[r];
+    if (k < 0) continue;
+    bool earlier = false;  // the first row with key k owns the sum; the block stops at the first chunk that shows one
+    for (long long q0 = 0; q0 < r && !earlier; q0 += blockDim.x) {
+      const long long q = q0 + threadIdx.x;
+      earlier = __syncthreads_or(q < r && key[q] == k) != 0;
+    }
+    if (earlier) continue;
+    for (int c = threadIdx.x; c < EMB_H; c += blockDim.x) {
+      float t = 0.f;
+      for (long long q = r; q < rows; ++q)
+        if (key[q] == k) t += src[q * EMB_H + c];
+      dst[(long long)k * EMB_H + c] += t;
     }
   }
 }
-__device__ __forceinline__ void keyed_add(KeyedAcc& a, int key, const float (&dz)[8], int i) {
-#pragma unroll
-  for (int j = 0; j < 8; ++j) a.v[i][j] += dz[j];
-  a.key = key;
-}
+
 // rows [0, n_rows) are walked as  first + k * stride  with stride = the largest multiple of `period` that the launched
 // warps cover, so a warp's position index (row % period) never changes; surplus warps idle
 __device__ __forceinline__ long long period_stride(long long launched_warps, int period) {
@@ -233,9 +229,9 @@ __global__ void __launch_bounds__(EMB_WARPS * 32)
 embed_text_bwd_kernel(const bf16* __restrict__ dy, const long long* __restrict__ ids,
                       const long long* __restrict__ type_ids, const float* __restrict__ word,
                       const float* __restrict__ pos, const float* __restrict__ type, const float* __restrict__ gamma,
-                      const float* __restrict__ mean_in, const float* __restrict__ rstd_in, float* __restrict__ dword,
-                      float* __restrict__ dpos, float* __restrict__ dtype, float* __restrict__ dgamma,
-                      float* __restrict__ dbeta, int n_seq, int S, int vocab, EmbDrop drop_in) {
+                      const float* __restrict__ mean_in, const float* __restrict__ rstd_in, float* __restrict__ zrows,
+                      int* __restrict__ keys, int want_type, float* __restrict__ dgamma, float* __restrict__ dbeta,
+                      int n_seq, int S, int vocab, EmbDrop drop_in) {
   const EmbDrop drop = resolve_emb_drop(drop_in);
   __shared__ float red[EMB_WARPS][257];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -245,9 +241,6 @@ embed_text_bwd_kernel(const bf16* __restrict__ dy, const long long* __restrict__
   for (int i = 0; i < EMB_VEC; ++i)
 #pragma unroll
     for (int j = 0; j < 8; ++j) acc_g[i][j] = acc_b[i][j] = 0.f;
-  KeyedAcc acc_p, acc_t;
-  keyed_init(acc_p);
-  keyed_init(acc_t);
   const long long stride = period_stride((long long)gridDim.x * EMB_WARPS, S);
   long long row = (long long)blockIdx.x * EMB_WARPS + warp;
   if (row >= stride) row = rows;
@@ -273,27 +266,12 @@ embed_text_bwd_kernel(const bf16* __restrict__ dy, const long long* __restrict__
       }
     }
     ln_row_bwd(z, dy + row * EMB_H, gamma, mean_in[row], rstd_in[row], row, drop, lane, dz, acc_g, acc_b);
-    if (acc_p.key != s) keyed_flush(acc_p, dpos, lane);
-    if (dtype != nullptr && acc_t.key != (int)t) keyed_flush(acc_t, dtype, lane);
 #pragma unroll
-    for (int i = 0; i < EMB_VEC; ++i) {
-      const int c = (i * 32 + lane) * 8;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) atomicAdd(dword + id * EMB_H + c + j, dz[i][j]);
-      keyed_add(acc_p, s, dz[i], i);
-      if (dtype != nullptr) keyed_add(acc_t, (int)t, dz[i], i);
-    }
-  }
-  keyed_flush(acc_p, dpos, lane);
-  if (dtype != nullptr) {
-    // type sums: reduce over the CTA's warps first (one atomic per column per CTA and type row)
-    for (int tt = 0; tt < 2; ++tt) {
-      float part[EMB_VEC][8];
-#pragma unroll
-      for (int i = 0; i < EMB_VEC; ++i)
-#pragma unroll
-        for (int j = 0; j < 8; ++j) part[i][j] = acc_t.key == tt ? acc_t.v[i][j] : 0.f;
-      flush_colsums(part, dtype + tt * EMB_H, red, warp, lane);
+    for (int i = 0; i < EMB_VEC; ++i) st8f(zrows + row * EMB_H + (i * 32 + lane) * 8, dz[i]);
+    if (lane == 0) {  // table rows this token's gradient belongs to: word id, position, type
+      keys[row] = (int)id;
+      keys[rows + row] = s;
+      keys[2 * rows + row] = want_type ? (int)t : -1;
     }
   }
   flush_colsums(acc_g, dgamma, red, warp, lane);
@@ -416,7 +394,7 @@ __global__ void __launch_bounds__(EMB_WARPS * 32)
 embed_src_bwd_kernel(const bf16* __restrict__ dy, SrcCfg src, const float* __restrict__ pos,
                      const float* __restrict__ type, const float* __restrict__ gamma,
                      const float* __restrict__ mean_in, const float* __restrict__ rstd_in, bf16* __restrict__ da,
-                     bf16* __restrict__ db, float* __restrict__ dpos, float* __restrict__ dtype,
+                     bf16* __restrict__ db, float* __restrict__ zrows, int* __restrict__ keys, int want_type,
                      float* __restrict__ dgamma, float* __restrict__ dbeta, EmbDrop drop_in) {
   const EmbDrop drop = resolve_emb_drop(drop_in);
   __shared__ float red[EMB_WARPS][257];
@@ -428,13 +406,8 @@ embed_src_bwd_kernel(const bf16* __restrict__ dy, SrcCfg src, const float* __res
   for (int i = 0; i < EMB_VEC; ++i)
 #pragma unroll
     for (int j = 0; j < 8; ++j) acc_g[i][j] = acc_b[i][j] = 0.f;
-  KeyedAcc acc_p;
-  keyed_init(acc_p);
-  float acc_t[EMB_VEC][8];
-#pragma unroll
-  for (int i = 0; i < EMB_VEC; ++i)
-#pragma unroll
-    for (int j = 0; j < 8; ++j) acc_t[i][j] = 0.f;
+  const long long rows_a = (long long)src.Na * src.Wa;
+  const long long n_rows = rows_a + (src.Fb > 0 ? (long long)src.Nb * src.Fb : 0);
   const long long stride = period_stride((long long)gridDim.x * EMB_WARPS, which == 0 ? src.Wa : src.Fb);
   long long sr = (long long)blockIdx.x * EMB_WARPS + warp;
   if (sr >= stride) sr = n_src_rows;
@@ -504,7 +477,7 @@ embed_src_bwd_kernel(const bf16* __restrict__ dy, SrcCfg src, const float* __res
     s1 = warp_sum(s1) * (1.0f / EMB_H);
     s2 = warp_sum(s2) * (1.0f / EMB_H);
     bf16* dst = (which == 0 ? da : db);
-    if (acc_p.key != r.s) keyed_flush(acc_p, dpos, lane);
+    const long long zr = (which == 0 ? 0 : rows_a) + sr;  // row of the table-gradient scratch
 #pragma unroll
     for (int i = 0; i < EMB_VEC; ++i) {
       const int col = (i * 32 + lane) * 8;
@@ -512,15 +485,37 @@ embed_src_bwd_kernel(const bf16* __restrict__ dy, SrcCfg src, const float* __res
 #pragma unroll
       for (int j = 0; j < 8; ++j) dz[j] = rstd * (D[i][j] - s1 - z[i][j] * s2);
       if (dst != nullptr) st8h(dst + sr * EMB_H + col, dz);
-      keyed_add(acc_p, r.s, dz, i);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) acc_t[i][j] += dz[j];
+      st8f(zrows + zr * EMB_H + col, dz);
+    }
+    if (lane == 0) {  // table rows: position r.s, type = which source
+      keys[zr] = r.s;
+      keys[n_rows + zr] = want_type ? which : -1;
     }
   }
-  keyed_flush(acc_p, dpos, lane);
-  if (dtype != nullptr) flush_colsums(acc_t, dtype + (which == 0 ? 0 : EMB_H), red, warp, lane);
   flush_colsums(acc_g, dgamma, red, warp, lane);
   flush_colsums(acc_b, dbeta, red, warp, lane);
+}
+
+struct EmbTables {
+  float* t[3];  // word, position, type gradients (each nullable); keys holds one slot of `rows` keys per non-null table
+};
+// table gradients from the per-row scratch (keyed, in row order) and LayerNorm gamma / beta from the per-CTA partials;
+// frees the scratch
+static int emb_table_grads(float* zrows, int* keys, long long rows, EmbTables tabs, float* pg, float* pb, int parts,
+                           float* dgamma, float* dbeta, cudaStream_t st) {
+  long long blocks = rows < device_sms() * 8LL ? rows : device_sms() * 8LL;
+  int k_used = 0;
+  for (int k = 0; k < 3; ++k) {
+    if (tabs.t[k] == nullptr) continue;
+    keyed_rows_sum_kernel<<<(int)(blocks < 1 ? 1 : blocks), 256, 0, st>>>(zrows, keys + (long long)k_used * rows, rows,
+                                                                           tabs.t[k]);
+    ++k_used;
+  }
+  UNIVL_CHECK_LAUNCH("embed table gradients");
+  cudaFreeAsync(zrows, st);
+  cudaFreeAsync(keys, st);
+  if (int rc = partials_reduce(pg, parts, 1, EMB_H, dgamma, EMB_H, st)) return rc;
+  return partials_reduce(pb, parts, 1, EMB_H, dbeta, EMB_H, st);
 }
 
 static EmbDrop make_emb_drop(float p, const unsigned long long* rng, unsigned long long stream) {
@@ -537,12 +532,12 @@ static EmbDrop make_emb_drop(float p, const unsigned long long* rng, unsigned lo
 // all-pairs source kernel with 5 warps per SM: 127 us, latency-bound)
 static int emb_bwd_grid(long long rows) {
   long long blocks = (rows + EMB_WARPS * 2 - 1) / (EMB_WARPS * 2);
-  const long long cap = 148LL * 4;
+  const long long cap = (long long)device_sms() * 4;
   return (int)(blocks < 1 ? 1 : (blocks > cap ? cap : blocks));
 }
 static int emb_grid(long long rows) {
   long long blocks = (rows + EMB_WARPS - 1) / EMB_WARPS;
-  const long long cap = 148LL * 8;
+  const long long cap = (long long)device_sms() * 8;
   return (int)(blocks < 1 ? 1 : (blocks > cap ? cap : blocks));
 }
 
@@ -575,11 +570,20 @@ extern "C" int univl_embed_text_bwd(const void* dy, const long long* ids, const 
   UNIVL_CHECK_ARG(dy && ids && word && pos && gamma && mean && rstd && dword && dpos && dgamma && dbeta,
                   "embed_text_bwd: null pointer");
   if (n_seq == 0) return UNIVL_OK;
-  embed_text_bwd_kernel<<<emb_bwd_grid((long long)n_seq * S), EMB_WARPS * 32, 0, (cudaStream_t)stream>>>(
-      (const bf16*)dy, ids, type_ids, word, pos, type, gamma, mean, rstd, dword, dpos, dtype, dgamma, dbeta, n_seq, S,
-      vocab, make_emb_drop(p_drop, rng_state, stream_id));
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long rows = (long long)n_seq * S;
+  const int grid = emb_bwd_grid(rows);
+  float *zrows, *pg, *pb;
+  int* keys;
+  if (int rc = scratch_alloc((void**)&zrows, (size_t)rows * EMB_H * sizeof(float), st)) return rc;
+  if (int rc = scratch_alloc((void**)&keys, (size_t)3 * rows * sizeof(int), st)) return rc;
+  if (int rc = scratch_alloc((void**)&pg, (size_t)grid * EMB_H * sizeof(float), st)) return rc;
+  if (int rc = scratch_alloc((void**)&pb, (size_t)grid * EMB_H * sizeof(float), st)) return rc;
+  embed_text_bwd_kernel<<<grid, EMB_WARPS * 32, 0, st>>>(
+      (const bf16*)dy, ids, type_ids, word, pos, type, gamma, mean, rstd, zrows, keys, dtype != nullptr ? 1 : 0, pg, pb,
+      n_seq, S, vocab, make_emb_drop(p_drop, rng_state, stream_id));
   UNIVL_CHECK_LAUNCH("embed_text_bwd");
-  return UNIVL_OK;
+  return emb_table_grads(zrows, keys, rows, {dword, dpos, dtype}, pg, pb, grid, dgamma, dbeta, st);
 }
 
 extern "C" int univl_embed_src_fwd(const void* a, const void* b, const float* pos, const float* type,
@@ -613,9 +617,18 @@ extern "C" int univl_embed_src_bwd(const void* dy, const void* a, const void* b,
   if (Na == 0) return UNIVL_OK;
   const long long rows_a = (long long)Na * Wa, rows_b = (long long)(Fb == 0 ? 0 : Nb) * Fb;
   dim3 grid(emb_bwd_grid(rows_a > rows_b ? rows_a : rows_b), Fb == 0 ? 1 : 2);
-  embed_src_bwd_kernel<<<grid, EMB_WARPS * 32, 0, (cudaStream_t)stream>>>(
-      (const bf16*)dy, src, pos, type, gamma, mean, rstd, (bf16*)da, (bf16*)db, dpos, dtype, dgamma, dbeta,
-      make_emb_drop(p_drop, rng_state, stream_id));
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long rows = rows_a + rows_b;
+  const int parts = (int)(grid.x * grid.y);
+  float *zrows, *pg, *pb;
+  int* keys;
+  if (int rc = scratch_alloc((void**)&zrows, (size_t)rows * EMB_H * sizeof(float), st)) return rc;
+  if (int rc = scratch_alloc((void**)&keys, (size_t)2 * rows * sizeof(int), st)) return rc;
+  if (int rc = scratch_alloc((void**)&pg, (size_t)parts * EMB_H * sizeof(float), st)) return rc;
+  if (int rc = scratch_alloc((void**)&pb, (size_t)parts * EMB_H * sizeof(float), st)) return rc;
+  embed_src_bwd_kernel<<<grid, EMB_WARPS * 32, 0, st>>>(
+      (const bf16*)dy, src, pos, type, gamma, mean, rstd, (bf16*)da, (bf16*)db, zrows, keys, dtype != nullptr ? 1 : 0,
+      pg, pb, make_emb_drop(p_drop, rng_state, stream_id));
   UNIVL_CHECK_LAUNCH("embed_src_bwd");
-  return UNIVL_OK;
+  return emb_table_grads(zrows, keys, rows, {nullptr, dpos, dtype}, pg, pb, parts, dgamma, dbeta, st);
 }

@@ -1,4 +1,4 @@
-// univl_b200 — fused QKV-projection + multi-head self-attention, forward, on tcgen05 / TMEM / TMA (sm_100a).
+// univl_b200 — fused QKV-projection + multi-head self-attention on wgmma / TMA (sm_90a), forward and backward.
 //
 // Reference op sequence replaced (modules/module_bert.py:171-197 = module_visual.py:155-181 = module_cross.py:162-188;
 // decoder self-attention module_decoder.py:220-247 with the causal mask of :385-396):
@@ -9,33 +9,27 @@
 //
 // Work item = (row block, head).  A row block is G = floor(128 / S) whole sequences = RB = G*S <= 128 consecutive
 // token rows (S = 48 -> 96 rows, S = 96 -> 96, S = 128 -> 128); a CTA walks a contiguous range of items, heads
-// fastest, so its x rows stay in L2 for the 12 heads.  Per item:
-//   1. projection   acc[128, 192] = x[128 rows, 768] . Wqkv_h[192, 768]^T      12 k-blocks x 4 tcgen05.mma (M128 N192 K16),
-//                   x and the three 64-row weight slices arrive by TMA into a 3-stage mbarrier ring
-//   2. drain        TMEM -> registers (+bias) -> bf16 -> Q, K, V shared-memory tiles in the 128B-swizzled UMMA operand
-//                   layout (one physical layout serves Q as K-major A, K as K-major B, V as MN-major B)
-//   3. S = Q K^T    4 tcgen05.mma (M128, N = RB, K16) into TMEM
-//   4. softmax      one thread per query row: tcgen05.ld, scale + additive mask (-10000 padding / causal, block-diagonal
-//                   across the packed sequences), exact online max/sum, Philox dropout, P (bf16) -> shared memory as
-//                   the K-major A operand, log-sum-exp -> HBM
-//   5. O = P V      RB/16 tcgen05.mma (M128 N64 K16) into TMEM, drained to the merged-head context rows in HBM.
-// TMEM (512 columns) is split in two halves that alternate between consecutive items: while the CUDA cores drain /
-// softmax item j in one half, the tensor pipe runs the projection of item j+1 in the other; the short S / PV products of
-// item j are issued by their own warp as soon as their operands are ready, so they slot in between projection k-blocks
-// and the projection issuer's loop stays as lean as a plain GEMM's.
-//
-// Warp roles (480 threads): warp 0 TMA producer, warp 1 projection-MMA issuer, warps 2-5 drain (TMEM lane quarter =
-// warp & 3), warps 6-13 softmax (two per quarter, alternating 16-key chunks), warp 14 issuer of the S / PV products.  All synchronisation is mbarrier-based (tcgen05.commit on the MMA side).
+// fastest, so its x rows stay in L2 for the 12 heads.  RB is a template parameter (80, 96, 112 or 128), so every
+// product below has its exact width.  Warp roles (384 threads): warpgroup 0 is the TMA producer, warpgroups 1 and 2
+// each own 64 query rows of the block.  Per item:
+//   1. projection   acc[64, 192] = x[64 rows, 768] . Wqkv_h[192, 768]^T   12 k-blocks x 4 wgmma m64n192k16 per
+//                   warpgroup; x and the three 64-row weight slices arrive by TMA into a 4-stage mbarrier ring
+//   2. drain        registers (+bias) -> bf16 -> Q, K, V shared-memory tiles in the 128B-swizzled operand layout (one
+//                   physical layout serves Q as K-major A, K as K-major B, V as MN-major B)
+//   3. S = Q K^T    4 wgmma (m64, N = RB, k16) into registers
+//   4. softmax      in registers, one quad of lanes per query row: scale + additive mask (-10000 padding / causal,
+//                   block-diagonal across the packed sequences), exact max / sum, Philox dropout, log-sum-exp -> HBM
+//   5. O = P V      P stays in registers as the A operand (RB / 16 wgmma m64n64k16), O -> merged-head context rows.
 #include <stdlib.h>
 
 #include "common.cuh"
 #include "tmap.cuh"
+#include "wgmma.cuh"
 
 namespace univl {
 
-constexpr int FA_THREADS = 480;   // forward: TMA + projection MMA + 4 drain + 8 softmax warps + core (S / PV) MMA warp
-constexpr int FB_THREADS = 320;   // backward: TMA + MMA + 8 compute warps
-constexpr int FA_STAGES = 3;
+constexpr int FA_THREADS = 384;                 // TMA producer warpgroup + two consumer warpgroups
+constexpr int FA_STAGES = 4;
 constexpr int FA_KB = 12;                       // 768 / 64 k-blocks
 constexpr int FA_X_BYTES = 128 * 64 * 2;        // 16 KB: x rows of one k-block
 constexpr int FA_W_BYTES = 192 * 64 * 2;        // 24 KB: q/k/v weight rows of one head, one k-block
@@ -44,16 +38,10 @@ constexpr int FA_TILE_BYTES = 128 * 128;        // one [128 rows][64 bf16] opera
 constexpr int FA_OFF_Q = FA_STAGES * FA_STAGE_BYTES;
 constexpr int FA_OFF_K = FA_OFF_Q + FA_TILE_BYTES;
 constexpr int FA_OFF_V = FA_OFF_K + FA_TILE_BYTES;
-constexpr int FA_OFF_P = FA_OFF_V + FA_TILE_BYTES;            // two 64-key atoms
-constexpr int FA_OFF_V2 = FA_OFF_P + 2 * FA_TILE_BYTES;       // V tile of odd items (V is double-buffered, see the drain warps)
-constexpr int FA_OFF_MADD = FA_OFF_V2 + FA_TILE_BYTES;        // 128 floats
-constexpr int FA_OFF_XCH = FA_OFF_MADD + 512;                 // softmax pair exchange: max[2][128], sum[2][128] floats
-constexpr int FA_OFF_BAR = FA_OFF_XCH + 2048;
-// full[3] empty[3] acc_full[2] s_full[2] p_ready[2] pv_done[2] half_free[2] qkv_ready[1]
-constexpr int FA_NUM_BARS = 2 * FA_STAGES + 11;
-constexpr int FA_SMEM_BYTES = FA_OFF_BAR + FA_NUM_BARS * 8 + 16 + 1024;
-constexpr int FA_HALF_COLS = 256;
-constexpr int FA_O_COL = 128;                   // O accumulator columns inside a half
+constexpr int FA_OFF_MADD = FA_OFF_V + FA_TILE_BYTES;         // 128 floats
+constexpr int FA_OFF_BAR = FA_OFF_MADD + 512;                 // full[FA_STAGES] empty[FA_STAGES]
+constexpr int FA_SMEM_BYTES = FA_OFF_BAR + 2 * FA_STAGES * 8 + 1024;
+static_assert(FA_SMEM_BYTES <= 227 * 1024, "shared memory per block");
 
 struct FusedAttnParams {
   int T, S, G, RB, n_seq, heads, n_blocks;
@@ -71,22 +59,8 @@ struct FusedAttnParams {
   const unsigned long long* rng;
   uint64_t stream;
   int store_qkv;
-  int item_order;
   int x_box_rows;   // rows of the x TMA box: RB when RB % 32 == 0 (see the launcher), else 128
-  long long* trace; // bring-up only: per-phase clock64 stamps of CTA 0 (tests/gpu_checks/trace_fused_attn.py), else null
 };
-
-// bring-up instrumentation: event e of item j of CTA 0 (first 16 items)
-#define FA_TRACE(e, j)                                                                          \
-  do {                                                                                          \
-    if (p.trace != nullptr && blockIdx.x == 0 && (j) < 16 && lane == 0) p.trace[(j) * 16 + (e)] = clock64(); \
-  } while (0)
-
-__device__ __forceinline__ bool mbar_poll(uint64_t* bar, uint32_t parity, bool blocking) {
-  if (!blocking) return mbar_test_wait(bar, parity) != 0;
-  mbar_wait(bar, parity);
-  return true;
-}
 
 // items [begin, end) of this CTA: contiguous ranges, the first (total % grid) CTAs take one more
 __device__ __forceinline__ void fa_item_range(int total, int& begin, int& end) {
@@ -96,107 +70,85 @@ __device__ __forceinline__ void fa_item_range(int total, int& begin, int& end) {
   end = begin + per + (b < rem ? 1 : 0);
 }
 
-// Item j of this CTA -> (row block, head).  order 0: a contiguous range of (block, head) items, heads fastest.  order 1
-// ("synchronised heads"): CTA c owns row blocks c, c + grid, c + 2 grid, ... and walks the 12 heads of each, so at any
-// moment all CTAs stream the SAME head's weight slices (requests for one L2 line arrive together) while each re-reads
-// only its own activation rows.
-struct FaItems {
-  int order, begin, count, heads, unit, n_units;
-  // unit / n_units: index and number of the workers that walk items (CTAs, or 2-CTA clusters whose "row block" is a pair)
-  __device__ __forceinline__ void init(int order_, int n_blocks, int heads_, int unit_, int n_units_) {
-    order = order_; heads = heads_; unit = unit_; n_units = n_units_;
-    if (order == 0) {
-      const int total = n_blocks * heads;
-      const int per = total / n_units, rem = total % n_units;
-      begin = unit * per + min(unit, rem);
-      count = per + (unit < rem ? 1 : 0);
-    } else {
-      begin = 0;
-      const int mine = (unit < n_blocks) ? (n_blocks - 1 - unit) / n_units + 1 : 0;
-      count = mine * heads;
-    }
+// additive key mask of row block rb (log2 domain) for key column `kcol` of the block: 0 / -10000; shared by the heads
+__device__ __forceinline__ float fa_key_mask(const long long* mask_a, const long long* mask_b, int Wa, int Fb, int Nb,
+                                             int all_pairs, int S, int G, int n_seq, int NK, int rb, int kcol) {
+  if (kcol >= NK) return 0.f;
+  const int g = kcol / S, kpos = kcol - g * S;
+  const long long seq = (long long)rb * G + g;
+  long long mv = 1;
+  if (mask_a != nullptr && seq < n_seq) {
+    const long long mi = all_pairs ? seq / Nb : seq, mj = all_pairs ? seq % Nb : seq;
+    if (kpos < Wa) mv = mask_a[mi * Wa + kpos];
+    else if (mask_b != nullptr) mv = mask_b[mj * Fb + (kpos - Wa)];
   }
-  __device__ __forceinline__ void decode(int j, int& rb, int& h) const {
-    if (order == 0) {
-      const int w = begin + j;
-      rb = w / heads;
-      h = w - rb * heads;
-    } else {
-      const int r = j / heads;
-      h = j - r * heads;
-      rb = unit + r * n_units;
-    }
-  }
-};
+  return mv != 0 ? 0.f : -10000.0f * 1.44269504088896340736f;
+}
 
-// MC = true: launched as clusters of two CTAs that walk the same (row-block pair, head) items, CTA r on row block
-// 2 * pair + r.  Both need the same 24 KB weight slice per k-block: each CTA issues HALF of its TMA boxes with
-// .multicast::cluster, so the slice leaves L2 once per pair (the kernel is bound by L2 -> SM operand delivery: 491 KB per
-// item without sharing, 343 KB with it).  A stage slot is free when BOTH CTAs' MMAs have consumed it (the peer writes
-// into it too): tcgen05.commit multicasts the "slot free" arrival to both CTAs' barriers.
-template <bool MC>
+// Dropout keep bits of one query row, NK keys.  Layout (row-major, matched by univl_attention_bwd rng_layout 1): element
+// (bh, query, key) is 16-bit word (key & 7) of Philox(seed, stream, (bh * S + query) * (S / 8) + key / 8).  In the wgmma
+// fragment the four lanes of a quad share a row and lane q holds keys 8 j + 2 q + {0, 1}, i.e. 32-bit word q of group
+// j's Philox output: each lane computes every fourth group and a 4 x 4 transpose over the quad hands out the words, so
+// one Philox call still decides 8 elements.  Bit 2 j + e of keep[j / 16] = key 8 j + 2 q + e kept.
+template <int NK>
+__device__ __forceinline__ void fa_keep_bits(uint64_t seed, uint64_t stream, uint64_t base, int c0_groups,
+                                             uint32_t thr, int quad, uint32_t (&keep)[(NK / 8 + 15) / 16]) {
+#pragma unroll
+  for (int i = 0; i < (NK / 8 + 15) / 16; ++i) keep[i] = 0;
+#pragma unroll
+  for (int j4 = 0; j4 < (NK / 8 + 3) / 4; ++j4) {
+    const int mine = 4 * j4 + quad;  // group this lane draws
+    const uint4 r = philox4x32(seed, stream, base + (uint64_t)(int64_t)(mine - c0_groups));
+    const uint32_t wv[4] = {r.x, r.y, r.z, r.w};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int src = quad ^ k;
+      const uint32_t send = wv[src];  // word `src` is what lane (quad ^ k) needs
+      const uint32_t got = k == 0 ? send : __shfl_xor_sync(0xffffffffu, send, k);
+      const int gj = 4 * j4 + src;    // group whose word quad lane `quad` received
+      if (gj < NK / 8) {
+        const uint32_t bits = ((got & 0xFFFFu) < thr ? 1u : 0u) | ((got >> 16) < thr ? 2u : 0u);
+        keep[gj >> 4] |= bits << (2 * (gj & 15));
+      }
+    }
+  }
+}
+
+template <int NK>
 __global__ void __launch_bounds__(FA_THREADS, 1)
 fused_qkv_attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
-                               const __grid_constant__ CUtensorMap tmap_qkv, const FusedAttnParams p_in) {
+                               const __grid_constant__ CUtensorMap tmap_qkv, const FusedAttnParams p) {
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + FA_OFF_BAR);
   uint64_t* empty_bar = full_bar + FA_STAGES;
-  uint64_t* acc_full = empty_bar + FA_STAGES;   // [2] projection accumulators complete      (MMA commit -> drain)
-  uint64_t* s_full = acc_full + 2;              // [2] S = Q K^T complete                    (MMA commit -> softmax)
-  uint64_t* p_ready = s_full + 2;               // [2] P in shared memory, S reads finished   (softmax -> MMA)
-  uint64_t* pv_done = p_ready + 2;              // [2] O complete; Q/K/V/P tiles free         (MMA commit -> drain)
-  uint64_t* half_free = pv_done + 2;            // [2] O drained: TMEM half reusable          (drain -> MMA)
-  uint64_t* qkv_ready = half_free + 2;          // [1] Q/K/V tiles written                    (drain -> MMA)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(qkv_ready + 1);
   float* madd = reinterpret_cast<float*>(smem + FA_OFF_MADD);
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  FusedAttnParams p = p_in;
-
-  if (warp == 0 && lane == 0) {
+  const int wg = threadIdx.x >> 7;
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_x);
     tma_prefetch_desc(&tmap_w);
     if (p.store_qkv) tma_prefetch_desc(&tmap_qkv);
     for (int s = 0; s < FA_STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], MC ? 2 : 1);   // MC: this CTA's and the peer's MMA both release the slot
+      mbar_init(&empty_bar[s], 2);  // one arrival per consumer warpgroup
     }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&acc_full[b], 1);
-      mbar_init(&s_full[b], 1);
-      mbar_init(&p_ready[b], 8);    // one arrival per softmax warp
-      mbar_init(&pv_done[b], 1);
-      mbar_init(&half_free[b], 4);  // one arrival per drain warp
-    }
-    mbar_init(qkv_ready, 4);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  tc_fence_before_sync();
-  if (MC) cluster_barrier();   // barrier inits of both CTAs visible cluster-wide before any remote TMA / commit signal
-  else __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
+  __syncthreads();
   pdl_wait();
 
-  const int crank = MC ? (int)cluster_rank() : 0;
-  FaItems items;
-  if (MC) items.init(p.item_order, (p.n_blocks + 1) >> 1, p.heads, (int)blockIdx.x >> 1, (int)gridDim.x >> 1);
-  else items.init(p.item_order, p.n_blocks, p.heads, (int)blockIdx.x, (int)gridDim.x);
-  const int n_items = items.count;
-  const int NK = p.RB;  // keys per block (S % 16 == 0, so RB is a multiple of 16)
+  int item_begin, item_end;
+  fa_item_range(p.n_blocks * p.heads, item_begin, item_end);
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ------------------------------------------ TMA producer ------------------------------------------
-    if (lane == 0) {
+    regs_dealloc<40>();
+    if (threadIdx.x == 0) {
       uint32_t it = 0;
-      for (int j = 0; j < n_items; ++j) {
-        int rb, h;
-        items.decode(j, rb, h);
-        if (MC) rb = 2 * rb + crank;   // (an odd tail leaves CTA 1 a block past the end: zero-filled loads, no outputs)
+      for (int w = item_begin; w < item_end; ++w) {
+        const int rb = w / p.heads, h = w - rb * p.heads;
         const int r0 = rb * p.RB;
         for (int kb = 0; kb < FA_KB; ++kb, ++it) {
           const int s = it % FA_STAGES;
@@ -204,397 +156,228 @@ fused_qkv_attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_x, const
           mbar_wait(&empty_bar[s], ph ^ 1);
           uint8_t* sx = smem + s * FA_STAGE_BYTES;
           uint8_t* sw = sx + FA_X_BYTES;
-          // the x box holds only the RB rows that carry queries / keys (tile rows RB..127 keep whatever the slot held:
-          // they feed accumulator rows nobody reads) — a quarter less operand traffic at S = 48 / 96
+          // the x box holds only the RB rows that carry queries / keys (tile rows RB..127 feed only rows nobody reads)
           mbar_arrive_expect_tx(&full_bar[s], (uint32_t)(p.x_box_rows * 128 + FA_W_BYTES));
           tma_load_2d(sx, &tmap_x, &full_bar[s], kb * 64, r0);  // rows >= T arrive as zeros
-          if (!MC) {
 #pragma unroll
-            for (int m = 0; m < 3; ++m)  // q / k / v weight rows of head h: rows m*H + h*64 of Wqkv[3H, 768]
-              tma_load_2d(sw + m * 8192, &tmap_w, &full_bar[s], kb * 64, m * p.heads * 64 + h * 64);
-          } else {
-            // six 32-row boxes (q lo/hi, k lo/hi, v lo/hi); this CTA issues three of them, to both CTAs
-#pragma unroll
-            for (int i = 0; i < 3; ++i) {
-              const int bx = 3 * crank + i;
-              tma_load_2d_mc(sw + bx * 4096, &tmap_w, &full_bar[s], kb * 64,
-                             (bx >> 1) * p.heads * 64 + h * 64 + (bx & 1) * 32, (uint16_t)3);
-            }
-          }
+          for (int m = 0; m < 3; ++m)  // q / k / v weight rows of head h: rows m*H + h*64 of Wqkv[3H, 768]
+            tma_load_2d(sw + m * 8192, &tmap_w, &full_bar[s], kb * 64, m * p.heads * 64 + h * 64);
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------ projection MMA issuer ----------------------------------
-    // all 32 lanes run the (warp-uniform) loop; one elected lane issues the MMAs and their commits
-    constexpr uint32_t idesc_proj = make_idesc_bf16(128, 192, false, false);
-    uint32_t it = 0;
-    for (int j = 0; j < n_items; ++j) {
-      const int b = j & 1;
-      mbar_wait(&half_free[b], (((uint32_t)j >> 1) & 1) ^ 1);  // O of item j-2 drained out of this half
-      tc_fence_after_sync();
-      FA_TRACE(0, j);
-      const uint32_t d_tmem = tmem_base + b * FA_HALF_COLS;
-      for (int kb = 0; kb < FA_KB; ++kb, ++it) {
-        const int s = it % FA_STAGES;
-        const uint32_t ph = (it / FA_STAGES) & 1;
-        mbar_wait(&full_bar[s], ph);
-        tc_fence_after_sync();
-        const uint32_t sx = smem_u32(smem + s * FA_STAGE_BYTES);
-        const uint64_t dx0 = make_smem_desc_sw128(sx, 16, 1024);
-        const uint64_t dw0 = make_smem_desc_sw128(sx + FA_X_BYTES, 16, 1024);
-        if (elect_one()) {
-#pragma unroll
-          for (int k = 0; k < 4; ++k)   // +32 bytes per K = 16 step: +2 in the descriptor's 16-byte address field
-            umma_bf16(d_tmem, dx0 + 2 * k, dw0 + 2 * k, idesc_proj, (kb > 0 || k > 0) ? 1u : 0u);
-          if (MC) umma_commit_mc(&empty_bar[s], (uint16_t)3);
-          else umma_commit(&empty_bar[s]);
-        }
-        __syncwarp();
-      }
-      if (elect_one()) umma_commit(&acc_full[b]);
-      __syncwarp();
-      FA_TRACE(1, j);
-    }
-  } else if (warp == 14) {
-    // ------------------------------------------ core MMA issuer (S = Q K^T, O = P V) --------------------
-    // a separate warp, so the projection issuer never polls: each product waits (sleeping) for its operands
-    const uint32_t idesc_s = make_idesc_bf16(128, NK, false, false);
-    constexpr uint32_t idesc_pv = make_idesc_bf16(128, 64, false, true);
-    const uint64_t dq0 = make_smem_desc_sw128(smem_u32(smem + FA_OFF_Q), 16, 1024);
-    const uint64_t dk0 = make_smem_desc_sw128(smem_u32(smem + FA_OFF_K), 16, 1024);
-    const uint32_t sV = smem_u32(smem + FA_OFF_V), sV2 = smem_u32(smem + FA_OFF_V2), sP = smem_u32(smem + FA_OFF_P);
-    // S(j) as soon as the Q / K tiles of item j are written, PV(j) as soon as its P is: S(j+1) may overtake PV(j) (they
-    // work in different TMEM halves), which is what lets the projection of item j+2 start on time.
-    int js = 0, jp = 0;
-    uint32_t spins = 0;
-    while (jp < n_items) {
-      bool did = false;
-      if (js < n_items && mbar_test_wait(qkv_ready, (uint32_t)js & 1)) {
-        const uint32_t half = tmem_base + (js & 1) * FA_HALF_COLS;
-        tc_fence_after_sync();
-        FA_TRACE(4, js);
-        if (elect_one()) {
-#pragma unroll
-          for (int k = 0; k < 4; ++k) umma_bf16(half, dq0 + 2 * k, dk0 + 2 * k, idesc_s, k > 0 ? 1u : 0u);
-          umma_commit(&s_full[js & 1]);
-        }
-        __syncwarp();
-        ++js;
-        did = true;
-      }
-      if (jp < js && mbar_test_wait(&p_ready[jp & 1], ((uint32_t)jp >> 1) & 1)) {
-        const uint32_t half = tmem_base + (jp & 1) * FA_HALF_COLS;
-        const uint32_t sVj = (jp & 1) ? sV2 : sV;
-        tc_fence_after_sync();
-        FA_TRACE(7, jp);
-        if (elect_one()) {
-          for (int kk = 0; kk < NK / 16; ++kk)  // contraction over keys: P K-major (64-key atoms), V MN-major
-            umma_bf16(half + FA_O_COL, make_smem_desc_sw128(sP + (kk >> 2) * FA_TILE_BYTES + (kk & 3) * 32, 16, 1024),
-                      make_smem_desc_sw128(sVj + kk * 2048, FA_TILE_BYTES, 1024), idesc_pv, kk > 0 ? 1u : 0u);
-          umma_commit(&pv_done[jp & 1]);
-        }
-        __syncwarp();
-        ++jp;
-        did = true;
-      }
-      if (did) spins = 0;
-      else if (++spins > (1u << 26)) {
-        if (lane == 0) printf("univl: fused attention core-MMA wait timed out (block %d)\n", blockIdx.x);
-        __trap();
-      }
-    }
-  } else if (warp < 6) {
-    // ------------------------------------------ drain warps -------------------------------------------
-    const int q = warp & 3;                 // TMEM lane quarter
-    const int row = q * 32 + lane;          // tile row this thread owns
-    const uint32_t lane_base = (uint32_t)(q * 32) << 16;
-    for (int jj = 0; jj <= n_items; ++jj) {
-      if (jj < n_items) {
-        // ---- projection accumulators of item jj -> Q / K / V operand tiles.  First thing in the iteration: it gates S(jj).
-        // The Q / K tiles are free once S(jj-1) has read them (s_full); V is double-buffered (item parity), its previous
-        // user PV(jj-2) was waited for by the O drain of the last iteration — so this never waits for PV(jj-1). ----
-        const int j = jj, b = j & 1;
-        int rb, h;
-        items.decode(j, rb, h);
-        if (MC) rb = 2 * rb + crank;   // (an odd tail leaves CTA 1 a block past the end: zero-filled loads, no outputs)
-        mbar_wait(&acc_full[b], ((uint32_t)j >> 1) & 1);
-        if (jj >= 1) mbar_wait(&s_full[(jj - 1) & 1], ((uint32_t)(jj - 1) >> 1) & 1);
-        tc_fence_after_sync();
-        if (q == 0) FA_TRACE(2, j);
-        if (p.store_qkv && jj >= 1) {
-          if (lane == 0) bulk_wait_read<0>();  // the bulk stores of item jj-1 have read this warp's tile rows
-          __syncwarp();
-        }
-        if (q == 0) FA_TRACE(10, j);
-        const uint32_t t_acc = tmem_base + b * FA_HALF_COLS + lane_base;
-#pragma unroll
-        for (int m = 0; m < 3; ++m) {
-          uint32_t r[4][16];
-#pragma unroll
-          for (int c = 0; c < 4; ++c) tmem_ld_32x32b_x16(t_acc + m * 64 + c * 16, r[c]);
-          tmem_ld_wait();
-          const float* bias = p.bias + m * p.heads * 64 + h * 64;
-          uint8_t* trow = smem + (m < 2 ? FA_OFF_Q + m * FA_TILE_BYTES : ((j & 1) ? FA_OFF_V2 : FA_OFF_V)) + row * 128;
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            float v[16];
-#pragma unroll
-            for (int e = 0; e < 16; e += 4) {
-              const float4 bb = __ldg(reinterpret_cast<const float4*>(bias + c * 16 + e));
-              v[e] = __uint_as_float(r[c][e]) + bb.x;
-              v[e + 1] = __uint_as_float(r[c][e + 1]) + bb.y;
-              v[e + 2] = __uint_as_float(r[c][e + 2]) + bb.z;
-              v[e + 3] = __uint_as_float(r[c][e + 3]) + bb.w;
-            }
-#pragma unroll
-            for (int g8 = 0; g8 < 2; ++g8) {
-              uint4 u;
-              u.x = pack_bf16x2(v[g8 * 8 + 0], v[g8 * 8 + 1]);
-              u.y = pack_bf16x2(v[g8 * 8 + 2], v[g8 * 8 + 3]);
-              u.z = pack_bf16x2(v[g8 * 8 + 4], v[g8 * 8 + 5]);
-              u.w = pack_bf16x2(v[g8 * 8 + 6], v[g8 * 8 + 7]);
-              const int chunk = c * 2 + g8;  // 16-byte chunk inside the 128-byte row; XOR swizzle = TMA/UMMA 128B swizzle
-              *reinterpret_cast<uint4*>(trow + ((chunk ^ (row & 7)) << 4)) = u;
-            }
-          }
-        }
-        fence_proxy_async_smem();  // generic-proxy writes -> visible to the tensor core and the bulk-copy engine
-        tc_fence_before_sync();
-        __syncwarp();
-        if (lane == 0) {
-          if (p.store_qkv && q * 32 < p.RB) {
-            const int r0 = rb * p.RB + q * 32;
-#pragma unroll
-            for (int m = 0; m < 3; ++m)
-              tma_store_2d(&tmap_qkv, smem + (m < 2 ? FA_OFF_Q + m * FA_TILE_BYTES : ((j & 1) ? FA_OFF_V2 : FA_OFF_V)) + q * 4096,
-                           m * p.heads * 64 + h * 64, r0);
-            bulk_commit();
-          }
-          if (q == 0) FA_TRACE(3, j);
-          mbar_arrive(qkv_ready);
-        }
-      }
-      if (jj >= 1) {
-        // ---- O of item jj-1 -> merged-head context rows ----
-        const int j = jj - 1, b = j & 1;
-        int rb, h;
-        items.decode(j, rb, h);
-        if (MC) rb = 2 * rb + crank;   // (an odd tail leaves CTA 1 a block past the end: zero-filled loads, no outputs)
-        mbar_wait(&pv_done[b], ((uint32_t)j >> 1) & 1);
-        tc_fence_after_sync();
-        if (q == 0) FA_TRACE(8, j);
-        const uint32_t t_o = tmem_base + b * FA_HALF_COLS + FA_O_COL + lane_base;
-        uint32_t r[4][16];
-#pragma unroll
-        for (int c = 0; c < 4; ++c) tmem_ld_32x32b_x16(t_o + c * 16, r[c]);
-        tmem_ld_wait();
-        const long long tok = (long long)rb * p.RB + row;
-        if (row < p.RB && tok < p.T) {
-          bf16* orow = p.o + tok * p.ldo + h * 64;
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            uint4 u0, u1;
-            u0.x = pack_bf16x2(__uint_as_float(r[c][0]), __uint_as_float(r[c][1]));
-            u0.y = pack_bf16x2(__uint_as_float(r[c][2]), __uint_as_float(r[c][3]));
-            u0.z = pack_bf16x2(__uint_as_float(r[c][4]), __uint_as_float(r[c][5]));
-            u0.w = pack_bf16x2(__uint_as_float(r[c][6]), __uint_as_float(r[c][7]));
-            u1.x = pack_bf16x2(__uint_as_float(r[c][8]), __uint_as_float(r[c][9]));
-            u1.y = pack_bf16x2(__uint_as_float(r[c][10]), __uint_as_float(r[c][11]));
-            u1.z = pack_bf16x2(__uint_as_float(r[c][12]), __uint_as_float(r[c][13]));
-            u1.w = pack_bf16x2(__uint_as_float(r[c][14]), __uint_as_float(r[c][15]));
-            *reinterpret_cast<uint4*>(orow + c * 16) = u0;
-            *reinterpret_cast<uint4*>(orow + c * 16 + 8) = u1;
-          }
-        }
-        tc_fence_before_sync();
-        __syncwarp();
-        if (q == 0) FA_TRACE(9, j);
-        if (lane == 0) mbar_arrive(&half_free[b]);
-      }
-    }
-    if (p.store_qkv && lane == 0) bulk_wait_read<0>();
-  } else if (warp < 14) {
-    // ------------------------------------------ softmax warps -----------------------------------------
-    // Two warps per TMEM lane quarter; a thread owns one query row and every other 16-key chunk (chunk parity = which
-    // warp of the pair), holds its <= 64 logits in registers (one TMEM read, one exp per element), and the pair combines
-    // row max / row sum through shared memory between two named barriers.
-    const uint64_t seed = (p.drop_on && p.rng != nullptr) ? p.rng[0] : 0ull;   // device-side {seed, epoch}
-    const uint64_t stream = p.stream + ((p.drop_on && p.rng != nullptr) ? (p.rng[1] << 20) : 0ull);
-    const int q = warp & 3;
-    const int half = (warp - 6) >> 2;
-    const int row = q * 32 + lane;
-    const uint32_t lane_base = (uint32_t)(q * 32) << 16;
-    const int g = row / p.S;                 // packed sequence this query row belongs to
-    const int c0 = g * p.S;                  // first key column of that sequence
-    const int qpos = row - c0;
-    const float sl2 = p.scale * 1.44269504088896340736f;
-    const float neg_big = -10000.0f * 1.44269504088896340736f;
-    float* xmax = reinterpret_cast<float*>(smem + FA_OFF_XCH);   // [2][128]
-    float* xsum = xmax + 256;                                    // [2][128]
-    const int pair_bar = 2 + q;
-    int cur_rb = -1;
-    for (int j = 0; j < n_items; ++j) {
-      const int b = j & 1;
-      int rb, h;
-      items.decode(j, rb, h);
-      if (MC) rb = 2 * rb + crank;
-      if (rb != cur_rb) {
-        // additive key mask of this row block (log2 domain): 0 / -10000 per key column; shared by the 12 heads
-        asm volatile("bar.sync 1, 256;" ::: "memory");  // every softmax warp is done with the previous block's mask
-        if (half == 0) {
-          float m = 0.f;
-          if (row < NK) {
-            const long long seq = (long long)rb * p.G + g;
-            long long mv = 1;
-            if (p.mask_a != nullptr && seq < p.n_seq) {
-              const long long mi = p.all_pairs ? seq / p.Nb : seq, mj = p.all_pairs ? seq % p.Nb : seq;
-              if (qpos < p.Wa) mv = p.mask_a[mi * p.Wa + qpos];
-              else if (p.mask_b != nullptr) mv = p.mask_b[mj * p.Fb + (qpos - p.Wa)];
-            }
-            m = mv != 0 ? 0.f : neg_big;
-          }
-          madd[row] = m;
-        }
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        cur_rb = rb;
-      }
-      mbar_wait(&s_full[b], ((uint32_t)j >> 1) & 1);
-      tc_fence_after_sync();
-      if (warp == 6) FA_TRACE(5, j);
-      const long long seq = (long long)rb * p.G + g;
-      const bool valid = row < p.RB && seq < p.n_seq;
-      const uint32_t t_s = tmem_base + b * FA_HALF_COLS + lane_base;
-      uint8_t* prow = smem + FA_OFF_P + row * 128;
-      const int sw = row & 7;
-      // logits of this thread's chunks (tcgen05.ld is warp-collective: every lane loads every chunk of the warp's parity;
-      // with packed sequences only the chunks of the lane's own sequence are used)
-      float t[4][16];
-      float mx = -INFINITY;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int c = half * 16 + i * 32;
-        if (c < NK) {   // warp-uniform
-          uint32_t r[16];
-          tmem_ld_32x32b_x16(t_s + c, r);
-          tmem_ld_wait();
-          const bool own = valid && c >= c0 && c < c0 + p.S;
-          const int kc = c - c0;
-          float a[16];
-#pragma unroll
-          for (int e4 = 0; e4 < 4; ++e4) {   // additive mask of the chunk: four 16-byte shared-memory loads
-            const float4 m4 = *reinterpret_cast<const float4*>(madd + c + e4 * 4);
-            a[e4 * 4] = m4.x; a[e4 * 4 + 1] = m4.y; a[e4 * 4 + 2] = m4.z; a[e4 * 4 + 3] = m4.w;
-          }
-          if (p.causal) {   // warp-uniform
-#pragma unroll
-            for (int e = 0; e < 16; ++e)
-              if ((kc + e) > qpos && a[e] == 0.f) a[e] = neg_big;
-          }
-#pragma unroll
-          for (int e = 0; e < 16; ++e) {
-            t[i][e] = own ? fmaf(__uint_as_float(r[e]), sl2, a[e]) : -INFINITY;
-            mx = fmaxf(mx, t[i][e]);
-          }
-        }
-      }
-      xmax[half * 128 + row] = mx;
-      asm volatile("bar.sync %0, 64;" ::"r"(pair_bar) : "memory");
-      mx = fmaxf(xmax[row], xmax[128 + row]);
-      const float mref = valid ? mx : 0.f;   // rows without a query: keep the arithmetic finite
-      float l = 0.f;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int c = half * 16 + i * 32;
-        if (c < NK) {
-#pragma unroll
-          for (int e = 0; e < 16; ++e) {
-            t[i][e] = ex2_approx(t[i][e] - mref);   // exp2(-inf) = 0 outside the own sequence
-            l += t[i][e];
-          }
-        }
-      }
-      xsum[half * 128 + row] = l;
-      asm volatile("bar.sync %0, 64;" ::"r"(pair_bar) : "memory");
-      l = xsum[row] + xsum[128 + row];
-      const float inv = valid ? (p.drop_on ? p.drop_scale : 1.0f) / l : 0.f;
-      const long long bh = seq * p.heads + h;
-      // the P tile is single-buffered: PV(j-1) must have read it (normally long done — it was issued when this warp
-      // finished item j-1)
-      if (j >= 1) mbar_wait(&pv_done[(j - 1) & 1], ((uint32_t)(j - 1) >> 1) & 1);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int c = half * 16 + i * 32;
-        if (c < NK) {
-          const bool own = valid && c >= c0 && c < c0 + p.S;
-          uint4 u0 = make_uint4(0, 0, 0, 0), u1 = make_uint4(0, 0, 0, 0);
-          if (own) {   // zeros outside the own sequence (block-diagonal) and for rows that carry no query
-            float pr[16];
-#pragma unroll
-            for (int e = 0; e < 16; ++e) pr[e] = t[i][e] * inv;
-            if (p.drop_on) {
-              // row-major dropout layout: element (bh, query, key) = 16-bit word (key & 7) of
-              // Philox(seed, stream, (bh * S + query) * (S / 8) + key / 8)
-              const int kc = c - c0;
-              const uint64_t base = ((uint64_t)bh * p.S + qpos) * (uint64_t)(p.S >> 3) + (uint64_t)(kc >> 3);
-#pragma unroll
-              for (int g8 = 0; g8 < 2; ++g8) {
-                const uint4 rnd = philox4x32(seed, stream, base + g8);
-#pragma unroll
-                for (int e = 0; e < 8; ++e)
-                  if (philox_u16(rnd, e) >= p.drop_threshold) pr[g8 * 8 + e] = 0.f;
-              }
-            }
-            u0.x = pack_bf16x2(pr[0], pr[1]);   u0.y = pack_bf16x2(pr[2], pr[3]);
-            u0.z = pack_bf16x2(pr[4], pr[5]);   u0.w = pack_bf16x2(pr[6], pr[7]);
-            u1.x = pack_bf16x2(pr[8], pr[9]);   u1.y = pack_bf16x2(pr[10], pr[11]);
-            u1.z = pack_bf16x2(pr[12], pr[13]); u1.w = pack_bf16x2(pr[14], pr[15]);
-          }
-          const int atom = c >> 6, chunk = (c & 63) >> 3;
-          *reinterpret_cast<uint4*>(prow + atom * FA_TILE_BYTES + ((chunk ^ sw) << 4)) = u0;
-          *reinterpret_cast<uint4*>(prow + atom * FA_TILE_BYTES + (((chunk + 1) ^ sw) << 4)) = u1;
-        }
-      }
-      if (half == 0 && valid && p.lse != nullptr)
-        p.lse[bh * p.S + qpos] = (mx + __log2f(l)) * 0.69314718055994530942f;
-      fence_proxy_async_smem();
-      tc_fence_before_sync();
-      __syncwarp();
-      if (warp == 6) FA_TRACE(6, j);
-      if (lane == 0) mbar_arrive(&p_ready[b]);
-    }
+    return;
   }
 
-  tc_fence_before_sync();
-  if (MC) cluster_barrier();   // the peer may still multicast into this CTA's shared memory / signal its barriers
-  else __syncthreads();
-  if (warp == 1) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 512);
+  // ------------------------------------------ consumer warpgroups ------------------------------------------
+  regs_alloc<232>();
+  const int c = wg - 1;
+  const int t = threadIdx.x & 127;
+  const int warp = t >> 5, lane = t & 31, quad = lane & 3;
+  const int r_lo = c * 64 + warp * 16 + (lane >> 2);  // tile rows r_lo and r_lo + 8 of the fragments
+  const uint64_t seed = (p.drop_on && p.rng != nullptr) ? p.rng[0] : 0ull;   // device-side {seed, epoch}
+  const uint64_t stream = p.stream + ((p.drop_on && p.rng != nullptr) ? (p.rng[1] << 20) : 0ull);
+  const float sl2 = p.scale * 1.44269504088896340736f;
+  const float neg_big = -10000.0f * 1.44269504088896340736f;
+  const uint32_t sQ = smem_u32(smem + FA_OFF_Q), sK = smem_u32(smem + FA_OFF_K), sV = smem_u32(smem + FA_OFF_V);
+  int cur_rb = -1;
+  uint32_t it = 0;
+  for (int w = item_begin; w < item_end; ++w) {
+    const int rb = w / p.heads, h = w - rb * p.heads;
+
+    // ---- 1. projection ----
+    float acc[96];
+#pragma unroll
+    for (int e = 0; e < 96; ++e) acc[e] = 0.f;
+    int prev_s = -1;
+    for (int kb = 0; kb < FA_KB; ++kb, ++it) {
+      const int s = it % FA_STAGES;
+      const uint32_t ph = (it / FA_STAGES) & 1;
+      mbar_wait(&full_bar[s], ph);
+      const uint32_t sx = smem_u32(smem + s * FA_STAGE_BYTES) + c * (64 * 128);
+      const uint32_t sw = smem_u32(smem + s * FA_STAGE_BYTES) + FA_X_BYTES;
+      wgmma_fence();
+      fence_regs(acc);
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        WgmmaSS<192>::mma<0, 0>(acc, make_smem_desc_sw128(sx + 32 * k, 16, 1024),
+                                make_smem_desc_sw128(sw + 32 * k, 16, 1024), (kb > 0 || k > 0) ? 1 : 0);
+      wgmma_commit();
+      fence_regs(acc);
+      wgmma_wait<1>();
+      if (prev_s >= 0 && t == 0) mbar_arrive(&empty_bar[prev_s]);
+      prev_s = s;
+    }
+    wgmma_wait<0>();
+    fence_regs(acc);
+    if (t == 0) mbar_arrive(&empty_bar[prev_s]);
+
+    // ---- 2. Q / K / V tiles (and the key mask when the row block changes) ----
+    if (p.store_qkv && t == 0) bulk_wait_read<0>();  // the previous item's q/k/v stores have read the tiles
+    named_bar(1, 256);  // both warpgroups are done with the previous item's tiles and mask
+    if (rb != cur_rb && c == 0)
+      madd[t] = fa_key_mask(p.mask_a, p.mask_b, p.Wa, p.Fb, p.Nb, p.all_pairs, p.S, p.G, p.n_seq, NK, rb, t);
+    cur_rb = rb;
+#pragma unroll
+    for (int m = 0; m < 3; ++m) {
+      const float* bias = p.bias + m * p.heads * 64 + h * 64;
+      uint8_t* tile = smem + FA_OFF_Q + m * FA_TILE_BYTES;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + 2 * quad));
+        const float* a = acc + 4 * (8 * m + j);
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          const int r = r_lo + 8 * hr;
+          *reinterpret_cast<uint32_t*>(tile + r * 128 + ((j ^ (r & 7)) << 4) + quad * 4) =
+              pack_bf16x2(a[2 * hr] + bb.x, a[2 * hr + 1] + bb.y);
+        }
+      }
+    }
+    fence_proxy_async_smem();  // generic-proxy writes -> visible to the tensor core and the bulk-copy engine
+    named_bar(2, 256);
+    if (p.store_qkv && t == 0) {
+      // this warpgroup's 64 rows, in 32-row boxes that start inside the block (a box may spill past RB into the next
+      // block's rows: with x_box_rows = 128 those are that block's true values)
+#pragma unroll
+      for (int m = 0; m < 3; ++m)
+#pragma unroll
+        for (int hb = 0; hb < 2; ++hb) {
+          const int rr = c * 64 + hb * 32;
+          if (rr < p.RB)
+            tma_store_2d(&tmap_qkv, smem + FA_OFF_Q + m * FA_TILE_BYTES + rr * 128, m * p.heads * 64 + h * 64,
+                         rb * p.RB + rr);
+        }
+      bulk_commit();
+    }
+
+    // ---- 3. S = Q K^T ----
+    float sa[NK / 2];
+#pragma unroll
+    for (int e = 0; e < NK / 2; ++e) sa[e] = 0.f;
+    wgmma_fence();
+    fence_regs(sa);
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      WgmmaSS<NK>::template mma<0, 0>(sa, make_smem_desc_sw128(sQ + c * (64 * 128) + 32 * k, 16, 1024),
+                                      make_smem_desc_sw128(sK + 32 * k, 16, 1024), k > 0 ? 1 : 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(sa);
+
+    // ---- 4. softmax of rows r_lo (hr = 0) and r_lo + 8 (hr = 1) ----
+    uint32_t pa[NK / 16][4];  // P as the register A operand of O = P V
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      const int row = r_lo + 8 * hr;
+      const int g = row / p.S, c0 = g * p.S, qpos = row - c0;
+      const long long seq = (long long)rb * p.G + g;
+      const bool valid = row < p.RB && seq < p.n_seq;
+      float mx = -INFINITY;
+#pragma unroll
+      for (int j = 0; j < NK / 8; ++j) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int key = 8 * j + 2 * quad + e;
+          const bool own = valid && key >= c0 && key < c0 + p.S;
+          float a = madd[key];
+          if (p.causal && (key - c0) > qpos && a == 0.f) a = neg_big;
+          const float v = own ? fmaf(sa[4 * j + 2 * hr + e], sl2, a) : -INFINITY;
+          sa[4 * j + 2 * hr + e] = v;
+          mx = fmaxf(mx, v);
+        }
+      }
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float mref = valid ? mx : 0.f;  // rows without a query: keep the arithmetic finite
+      float l = 0.f;
+#pragma unroll
+      for (int j = 0; j < NK / 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float v = ex2_approx(sa[4 * j + 2 * hr + e] - mref);  // exp2(-inf) = 0 outside the own sequence
+          sa[4 * j + 2 * hr + e] = v;
+          l += v;
+        }
+      l += __shfl_xor_sync(0xffffffffu, l, 1);
+      l += __shfl_xor_sync(0xffffffffu, l, 2);
+      const float inv = valid ? (p.drop_on ? p.drop_scale : 1.0f) / l : 0.f;
+      const long long bh = seq * p.heads + h;
+      uint32_t keep[(NK / 8 + 15) / 16];
+      if (p.drop_on) {
+        const uint64_t base = ((uint64_t)bh * p.S + qpos) * (uint64_t)(p.S >> 3);
+        fa_keep_bits<NK>(seed, stream, base, c0 >> 3, p.drop_threshold, quad, keep);
+      }
+#pragma unroll
+      for (int j = 0; j < NK / 8; ++j) {
+        float pr0 = sa[4 * j + 2 * hr] * inv, pr1 = sa[4 * j + 2 * hr + 1] * inv;
+        if (p.drop_on) {
+          const uint32_t kb2 = keep[j >> 4] >> (2 * (j & 15));
+          if (!(kb2 & 1u)) pr0 = 0.f;
+          if (!(kb2 & 2u)) pr1 = 0.f;
+        }
+        // A fragment of k-slice j / 2: {row, k 0-7}, {row + 8, k 0-7}, {row, k 8-15}, {row + 8, k 8-15}
+        pa[j >> 1][(j & 1) * 2 + hr] = pack_bf16x2(pr0, pr1);
+      }
+      if (quad == 0 && valid && p.lse != nullptr)
+        p.lse[bh * p.S + qpos] = (mx + __log2f(l)) * 0.69314718055994530942f;
+    }
+
+    // ---- 5. O = P V, merged-head context rows ----
+    float oa[32];
+#pragma unroll
+    for (int e = 0; e < 32; ++e) oa[e] = 0.f;
+    wgmma_fence();
+    fence_regs(oa);
+#pragma unroll
+    for (int kk = 0; kk < NK / 16; ++kk)  // contraction over keys: V [keys][64] is the MN-major B operand
+      WgmmaRS<64>::mma<1>(oa, pa[kk], make_smem_desc_sw128(sV + kk * 2048, FA_TILE_BYTES, 1024), kk > 0 ? 1 : 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(oa);
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      const int row = r_lo + 8 * hr;
+      const long long tok = (long long)rb * p.RB + row;
+      if (row < p.RB && tok < p.T) {
+        bf16* orow = p.o + tok * p.ldo + h * 64 + 2 * quad;
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+          *reinterpret_cast<uint32_t*>(orow + 8 * j) = pack_bf16x2(oa[4 * j + 2 * hr], oa[4 * j + 2 * hr + 1]);
+      }
+    }
   }
+  if (p.store_qkv && t == 0) bulk_wait_read<0>();
 }
 
 }  // namespace univl
 
 using namespace univl;
 
-// bring-up only (not part of include/univl_b200.h): device buffer of 16 x 16 int64 that CTA 0 of the next forward launches
-// fills with per-phase clock64 stamps
-static long long* g_fa_trace = nullptr;
-extern "C" int univl_debug_set_fused_attention_trace(void* device_buffer) {
-  g_fa_trace = reinterpret_cast<long long*>(device_buffer);
-  return UNIVL_OK;
-}
-
-// 1 if univl_fused_qkv_attention_fwd supports this shape (else the caller uses the unfused QKV GEMM + attention core)
+// 1 if univl_fused_qkv_attention_supported supports this shape (else the caller uses the unfused QKV GEMM + attention core)
 extern "C" int univl_fused_qkv_attention_supported(int n_seq, int heads, int S, int H) {
   return (n_seq > 0 && heads == 12 && H == 768 && S >= 16 && S <= 128 && (S % 16) == 0) ? 1 : 0;
 }
 
+// the kernel instantiation for the row-block width RB = floor(128 / S) * S
+template <template <int> class K, typename Fn>
+static int fa_dispatch(int RB, Fn&& fn) {
+  switch (RB) {
+    case 80: return fn(K<80>::kernel);
+    case 96: return fn(K<96>::kernel);
+    case 112: return fn(K<112>::kernel);
+    case 128: return fn(K<128>::kernel);
+  }
+  return set_error(UNIVL_ERR_ARG, "fused_attention: row block %d", RB);
+}
+template <int NK>
+struct FaFwdKernel {
+  static constexpr auto kernel = fused_qkv_attention_fwd_kernel<NK>;
+};
+
 // ctx[T, H] = MHA(x[T, H]) with q/k/v = x Wqkv^T + bias computed in the same kernel (T = n_seq * S, H = heads * 64 = 768).
 // wqkv: bf16 [3H, H] (rows: query | key | value weights), bias fp32 [3H].  qkv_out (nullable): bf16 [T, 3H] copy of the
 // projected q | k | v for the backward pass.  Mask / dropout arguments as univl_attention_fwd, except the dropout
-// layout, which is row-major (see the kernel) and matched by univl_attention_bwd(..., rng_layout = 1).
+// layout, which is row-major (see fa_keep_bits) and matched by univl_attention_bwd(..., rng_layout = 1).
 extern "C" int univl_fused_qkv_attention_fwd(const void* x, long long ldx, const void* wqkv, long long ldw,
                                              const float* bias, void* qkv_out, long long ld_qkv, void* o,
                                              long long ldo, float* lse, const long long* mask_a,
@@ -628,65 +411,43 @@ extern "C" int univl_fused_qkv_attention_fwd(const void* x, long long ldx, const
   p.drop_scale = p_drop > 0.f ? 1.0f / (1.0f - p_drop) : 1.0f;
   p.rng = rng_state; p.stream = stream_id;
   p.store_qkv = qkv_out != nullptr;
-  p.trace = g_fa_trace;
-  {
-    static int order = -1;  // tuning: UNIVL_FA_ORDER=0 (default) contiguous item ranges, 1 synchronised heads (measured 8% slower)
-    if (order < 0) {
-      const char* e = getenv("UNIVL_FA_ORDER");
-      order = e ? atoi(e) : 0;
-    }
-    p.item_order = order;
-  }
   CUtensorMap tx, tw, tq;
   int rc;
   // x box = the RB rows of the block when the q/k/v copies go out in whole 32-row boxes; otherwise all 128 tile rows, so
   // that the rows a partial box spills into the next block are that block's true values
   p.x_box_rows = (p.RB % 32 == 0) ? p.RB : 128;
   if ((rc = make_tmap(&tx, x, p.T, H, ldx, p.x_box_rows))) return rc;   // box {64 k, x_box_rows}
-  const int sms = usable_sms();
-  // tuning: UNIVL_FA_MULTICAST=1 enables the 2-CTA weight multicast.  Measured (1024 x 96): L2 slice reads -30% but the
-  // same 6.2 GB cross the crossbar into the SMs and the kernel is 5% slower: the bound is per-SM ingress, not L2 slices.
-  static int mc_mode = -1;
-  if (mc_mode < 0) {
-    const char* e = getenv("UNIVL_FA_MULTICAST");
-    mc_mode = e ? atoi(e) : 0;
-  }
-  const long long items = (long long)p.n_blocks * heads;
-  const bool mc = mc_mode != 0 && items >= 2LL * sms;   // pairs only pay when every SM has work either way
-  if ((rc = make_tmap(&tw, wqkv, 3 * H, H, ldw, mc ? 32 : 64))) return rc;    // box {64 k, 64 (32) weight rows}
+  if ((rc = make_tmap(&tw, wqkv, 3 * H, H, ldw, 64))) return rc;        // box {64 k, 64 weight rows}
   if (qkv_out != nullptr) {
     if ((rc = make_tmap_epi(&tq, qkv_out, false, p.T, 3 * H, ld_qkv))) return rc;  // box {64 cols, 32 rows}
   } else {
     tq = tx;
   }
-  auto kern = mc ? fused_qkv_attention_fwd_kernel<true> : fused_qkv_attention_fwd_kernel<false>;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, FA_SMEM_BYTES);
-  if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "fused_attention smem attribute: %s", cudaGetErrorString(e));
-  int grid = (int)(items < sms ? items : sms);
-  if (mc) grid &= ~1;
-  if (p.n_blocks < 2 * sms) p.item_order = 0;  // synchronised heads only pays (and only balances) with many row blocks per CTA
-  e = launch_kernel_cluster(kern, dim3(grid), dim3(FA_THREADS), (size_t)FA_SMEM_BYTES, (cudaStream_t)stream,
-                            mc ? 2 : 1, tx, tw, tq, p);
-  if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "fused_attention launch: %s", cudaGetErrorString(e));
-  UNIVL_CHECK_LAUNCH("fused_qkv_attention_fwd");
-  return UNIVL_OK;
+  const int sms = usable_sms();
+  const long long items = (long long)p.n_blocks * heads;
+  const int grid = (int)(items < sms ? items : sms);
+  return fa_dispatch<FaFwdKernel>(p.RB, [&](auto kern) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, FA_SMEM_BYTES);
+    if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "fused_attention smem attribute: %s", cudaGetErrorString(e));
+    e = launch_kernel(kern, dim3(grid), dim3(FA_THREADS), (size_t)FA_SMEM_BYTES, (cudaStream_t)stream, tx, tw, tq, p);
+    if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "fused_attention launch: %s", cudaGetErrorString(e));
+    UNIVL_CHECK_LAUNCH("fused_qkv_attention_fwd");
+    return UNIVL_OK;
+  });
 }
 
 // =====================================================================================================================
-// Backward of the attention core on tcgen05 (same row-block x head decomposition, same masks and dropout layout as the
-// forward above).  Inputs: the saved q | k | v [T, 3H], the context O and its gradient dO [T, H], the log-sum-exp.
-// Per item, five small tensor-core products with every intermediate on chip:
-//     S  = Q K^T,  dP = dO V^T                         (TMEM, fp32)
+// Backward of the attention core (same row-block x head decomposition, same masks and dropout layout as the forward
+// above).  Inputs: the saved q | k | v [T, 3H], the context O and its gradient dO [T, H], the log-sum-exp.  Per item,
+// with warpgroup c of the two consumer warpgroups owning query rows (and, for dK / dV, key rows) [64 c, 64 c + 64):
+//     S  = Q K^T,  dP = dO V^T                         (wgmma into registers)
 //     P  = exp(S * scale + mask - lse);  P~ = dropout(P);  dS = P o (dropout'(dP) - D) * scale,  D_i = sum_d dO_id O_id
-//          one thread per (query row, half of the key chunks): tcgen05.ld, Philox, bf16 P~ and dS tiles -> shared memory
-//     dQ = dS K   (A = dS K-major,  B = K MN-major)    dV = P~^T dO (A = P~ MN-major, B = dO MN-major)
-//     dK = dS^T Q (A = dS MN-major, B = Q MN-major)    -> TMEM -> bf16 rows of dq | dk | dv [T, 3H]
-// and the projection-bias gradients (column sums of dQ / dK / dV) by a shuffle transpose-reduction + red.global.add.
-// The Q, K, V, dO (and O, for D) tiles arrive by TMA straight in the 128B-swizzled layout every product reads (the "major"
-// of an operand is a descriptor bit), double-buffered; TMEM is split in two buffers so S / dP of item j+1 are computed
-// while the compute warps are still busy with item j.
-// Warp roles (320 threads): warp 0 TMA producer, warp 1 MMA issuer, warps 2-9 compute (two per TMEM lane quarter,
-// alternating 16-key chunks in the softmax-backward phase and splitting the 192 gradient columns in the drain phase).
+//     dQ = dS K   (dS from registers, K MN-major)
+//     dV = P~^T dO, dK = dS^T Q   (P~ and dS through shared memory as MN-major A operands; contraction over queries)
+//     -> bf16 rows of dq | dk | dv [T, 3H], and the projection-bias gradients (column sums): shuffles, then one
+//        partial row per (row block, warp) that partials_reduce adds in order.
+// The Q, K, V, dO, O tiles arrive by TMA straight in the 128B-swizzled layout every product reads, double-buffered, so
+// the next item's operands load while this one computes.
 // =====================================================================================================================
 namespace univl {
 
@@ -694,24 +455,16 @@ constexpr int FB_IN_BYTES = 5 * FA_TILE_BYTES;              // Q, K, V, dO, O ti
 constexpr int FB_OFF_P = 2 * FB_IN_BYTES;                   // P~ tile (two 64-key atoms)
 constexpr int FB_OFF_DS = FB_OFF_P + 2 * FA_TILE_BYTES;     // dS tile
 constexpr int FB_OFF_MADD = FB_OFF_DS + 2 * FA_TILE_BYTES;
-constexpr int FB_OFF_BAR = FB_OFF_MADD + 512;
-constexpr int FB_NUM_BARS = 11;                             // in_full[2] in_empty[2] sd_full[2] pds_ready acc_full[2] acc_free[2]
-constexpr int FB_SMEM_BYTES = FB_OFF_BAR + FB_NUM_BARS * 8 + 16 + 1024;
-// TMEM: two 256-column buffers alternate between consecutive items.  Inside a buffer S and dP come first; once the compute
-// warps have consumed them the same columns receive dQ | dK | dV.
-constexpr int FB_BUF_COLS = 256;
-constexpr int FB_COL_S = 0, FB_COL_DP = 128, FB_COL_DQ = 0, FB_COL_DK = 64, FB_COL_DV = 128;
+constexpr int FB_OFF_BAR = FB_OFF_MADD + 512;               // in_full[2] in_empty[2]
+constexpr int FB_SMEM_BYTES = FB_OFF_BAR + 4 * 8 + 1024;
+static_assert(FB_SMEM_BYTES <= 227 * 1024, "shared memory per block");
 
 struct FusedAttnBwdParams {
   int T, S, G, RB, n_seq, heads, n_blocks;
-  const bf16* o;
-  long long ldo;
-  const bf16* d_o;
-  long long lddo;
   const float* lse;
   bf16* dqkv;
   long long ld_dqkv;
-  float* dbias;               // [3 * heads * 64] accumulated into, or null
+  float* dbias;               // partial rows [n_blocks * 8][3 * heads * 64], or null
   const long long* mask_a;
   const long long* mask_b;
   int Wa, Fb, Nb, all_pairs, causal;
@@ -723,72 +476,71 @@ struct FusedAttnBwdParams {
   uint64_t stream;
 };
 
-// column totals of a 32-lane x 32-column block held one row per lane: after the call lane l holds the sum over the 32
-// lanes of v[l].  Halving butterfly: 16 + 8 + 4 + 2 + 1 shuffles instead of 32 x 5.
-__device__ __forceinline__ float warp_colsum32(float (&v)[32], int lane) {
+// rows r_lo, r_lo + 8 of a 64-column gradient fragment -> bf16 rows of dqkv, and this warp's column sums into its
+// partial row of dbias (row rb * 8 + warpgroup * 4 + warp; summed in row order after the kernel)
+__device__ __forceinline__ void fb_drain(const FusedAttnBwdParams& p, const float (&v)[32], int rb, int r_lo, int quad,
+                                         int lane, int col0, int part_row) {
 #pragma unroll
-  for (int half = 16; half >= 1; half >>= 1) {
-    const bool upper = (lane & half) != 0;
+  for (int hr = 0; hr < 2; ++hr) {
+    const int row = r_lo + 8 * hr;
+    const long long tok = (long long)rb * p.RB + row;
+    if (row < p.RB && tok < p.T) {
+      bf16* dst = p.dqkv + tok * p.ld_dqkv + col0 + 2 * quad;
 #pragma unroll
-    for (int i = 0; i < half; ++i) {
-      // keep the columns whose bit `half` equals this lane's; send the other half to the partner lane
-      const float keep = upper ? v[i + half] : v[i];
-      const float send = upper ? v[i] : v[i + half];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, half);
+      for (int j = 0; j < 8; ++j)
+        *reinterpret_cast<uint32_t*>(dst + 8 * j) = pack_bf16x2(v[4 * j + 2 * hr], v[4 * j + 2 * hr + 1]);
     }
   }
-  return v[0];
+  if (p.dbias == nullptr) return;
+  const bool ok0 = r_lo < p.RB && (long long)rb * p.RB + r_lo < p.T;
+  const bool ok1 = r_lo + 8 < p.RB && (long long)rb * p.RB + r_lo + 8 < p.T;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      float s = (ok0 ? v[4 * j + e] : 0.f) + (ok1 ? v[4 * j + 2 + e] : 0.f);
+      s += __shfl_xor_sync(0xffffffffu, s, 4);
+      s += __shfl_xor_sync(0xffffffffu, s, 8);
+      s += __shfl_xor_sync(0xffffffffu, s, 16);
+      if (lane < 4) p.dbias[(long long)part_row * 3 * p.heads * 64 + col0 + 8 * j + 2 * quad + e] = s;
+    }
+  }
 }
 
-__global__ void __launch_bounds__(FB_THREADS, 1)
+template <int NK>
+__global__ void __launch_bounds__(FA_THREADS, 1)
 fused_attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_constant__ CUtensorMap tmap_do,
-                           const __grid_constant__ CUtensorMap tmap_o, const FusedAttnBwdParams p_in) {
+                           const __grid_constant__ CUtensorMap tmap_o, const FusedAttnBwdParams p) {
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* in_full = reinterpret_cast<uint64_t*>(smem + FB_OFF_BAR);   // [2] TMA -> MMA
-  uint64_t* in_empty = in_full + 2;                                      // [2] MMA commit -> TMA
-  uint64_t* sd_full = in_empty + 2;                                      // [2] S, dP complete      (MMA commit -> compute)
-  uint64_t* pds_ready = sd_full + 2;                                     // P~, dS tiles written; S / dP read (compute -> MMA)
-  uint64_t* acc_full = pds_ready + 1;                                    // [2] dQ, dK, dV complete (MMA commit -> compute)
-  uint64_t* acc_free = acc_full + 2;                                     // [2] dQ, dK, dV drained  (compute -> MMA)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_free + 2);
+  uint64_t* in_full = reinterpret_cast<uint64_t*>(smem + FB_OFF_BAR);   // [2] TMA -> consumers
+  uint64_t* in_empty = in_full + 2;                                      // [2] consumers -> TMA
   float* madd = reinterpret_cast<float*>(smem + FB_OFF_MADD);
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  FusedAttnBwdParams p = p_in;
-
-  if (warp == 0 && lane == 0) {
+  const int wg = threadIdx.x >> 7;
+  const int H = p.heads * 64;
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_qkv);
     tma_prefetch_desc(&tmap_do);
     tma_prefetch_desc(&tmap_o);
     for (int b = 0; b < 2; ++b) {
       mbar_init(&in_full[b], 1);
-      mbar_init(&in_empty[b], 1);
-      mbar_init(&sd_full[b], 1);
-      mbar_init(&acc_full[b], 1);
-      mbar_init(&acc_free[b], 8);
+      mbar_init(&in_empty[b], 2);
     }
-    mbar_init(pds_ready, 8);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();
 
   int item_begin, item_end;
   fa_item_range(p.n_blocks * p.heads, item_begin, item_end);
   const int n_items = item_end - item_begin;
-  const int NK = p.RB;
-  const int H = p.heads * 64;
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ------------------------------------------ TMA producer ------------------------------------------
-    if (lane == 0) {
+    regs_dealloc<40>();
+    if (threadIdx.x == 0) {
       for (int j = 0; j < n_items; ++j) {
         const int b = j & 1;
         const int w = item_begin + j;
@@ -803,240 +555,170 @@ fused_attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const _
         tma_load_2d(dst + 4 * FA_TILE_BYTES, &tmap_o, &in_full[b], h * 64, r0);
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------ MMA issuer --------------------------------------------
-    // warp-uniform loop, one elected lane issues (see elect_one in common.cuh)
-    const uint32_t idesc_s = make_idesc_bf16(128, NK, false, false);
-    constexpr uint32_t idesc_dq = make_idesc_bf16(128, 64, false, true);
-    constexpr uint32_t idesc_t = make_idesc_bf16(128, 64, true, true);
-    const uint32_t sP = smem_u32(smem + FB_OFF_P), sdS = smem_u32(smem + FB_OFF_DS);
-    const uint64_t dP_mn = make_smem_desc_sw128(sP, FA_TILE_BYTES, 1024);     // P~ as MN-major A (dV)
-    const uint64_t dS_mn = make_smem_desc_sw128(sdS, FA_TILE_BYTES, 1024);    // dS as MN-major A (dK)
-    // S = Q K^T and dP = dO V^T of item j into TMEM buffer j & 1 (free once the gradients of item j-2 are drained)
-    auto issue_sdp = [&](int j) {
-      const int b = j & 1;
-      const uint32_t sQ = smem_u32(smem + b * FB_IN_BYTES);
-      const uint64_t dQ = make_smem_desc_sw128(sQ, 16, 1024), dK = make_smem_desc_sw128(sQ + FA_TILE_BYTES, 16, 1024);
-      const uint64_t dV = make_smem_desc_sw128(sQ + 2 * FA_TILE_BYTES, 16, 1024);
-      const uint64_t dO = make_smem_desc_sw128(sQ + 3 * FA_TILE_BYTES, 16, 1024);
-      const uint32_t tb = tmem_base + b * FB_BUF_COLS;
-      mbar_wait(&in_full[b], ((uint32_t)j >> 1) & 1);
-      mbar_wait(&acc_free[b], (((uint32_t)j >> 1) & 1) ^ 1);
-      tc_fence_after_sync();
-      if (elect_one()) {
-#pragma unroll
-        for (int k = 0; k < 4; ++k) umma_bf16(tb + FB_COL_S, dQ + 2 * k, dK + 2 * k, idesc_s, k > 0 ? 1u : 0u);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) umma_bf16(tb + FB_COL_DP, dO + 2 * k, dV + 2 * k, idesc_s, k > 0 ? 1u : 0u);
-        umma_commit(&sd_full[b]);
-      }
-      __syncwarp();
-    };
-    if (n_items > 0) issue_sdp(0);
-    for (int j = 0; j < n_items; ++j) {
-      const int b = j & 1;
-      const uint32_t sQ = smem_u32(smem + b * FB_IN_BYTES);
-      const uint64_t dQ_mn = make_smem_desc_sw128(sQ, FA_TILE_BYTES, 1024);                       // Q as MN-major B (dK)
-      const uint64_t dK_mn = make_smem_desc_sw128(sQ + FA_TILE_BYTES, FA_TILE_BYTES, 1024);       // K as MN-major B (dQ)
-      const uint64_t dO_mn = make_smem_desc_sw128(sQ + 3 * FA_TILE_BYTES, FA_TILE_BYTES, 1024);   // dO as MN-major B (dV)
-      const uint32_t tb = tmem_base + b * FB_BUF_COLS;
-      if (j + 1 < n_items) issue_sdp(j + 1);   // runs while the compute warps work on item j
-      mbar_wait(pds_ready, (uint32_t)j & 1);
-      tc_fence_after_sync();
-      if (elect_one()) {
-        for (int kk = 0; kk < NK / 16; ++kk)  // dQ[q, d] = sum_key dS[q, key] K[key, d]   (16 keys = +128 in MN-major K)
-          umma_bf16(tb + FB_COL_DQ, make_smem_desc_sw128(sdS + (kk >> 2) * FA_TILE_BYTES + (kk & 3) * 32, 16, 1024),
-                    dK_mn + 128 * kk, idesc_dq, kk > 0 ? 1u : 0u);
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {      // contraction over the 128 query rows of the tile (rows >= RB hold zeros)
-          umma_bf16(tb + FB_COL_DV, dP_mn + 128 * kk, dO_mn + 128 * kk, idesc_t, kk > 0 ? 1u : 0u);
-          umma_bf16(tb + FB_COL_DK, dS_mn + 128 * kk, dQ_mn + 128 * kk, idesc_t, kk > 0 ? 1u : 0u);
-        }
-        umma_commit(&acc_full[b]);
-        umma_commit(&in_empty[b]);
-      }
-      __syncwarp();
+    return;
+  }
+
+  // ------------------------------------------ consumer warpgroups ------------------------------------------
+  regs_alloc<232>();
+  const int c = wg - 1;
+  const int t = threadIdx.x & 127;
+  const int warp = t >> 5, lane = t & 31, quad = lane & 3;
+  const int r_lo = c * 64 + warp * 16 + (lane >> 2);
+  const uint64_t seed = (p.drop_on && p.rng != nullptr) ? p.rng[0] : 0ull;
+  const uint64_t stream = p.stream + ((p.drop_on && p.rng != nullptr) ? (p.rng[1] << 20) : 0ull);
+  const float sl2 = p.scale * 1.44269504088896340736f;
+  const float neg_big = -10000.0f * 1.44269504088896340736f;
+  const float ds_scale = p.drop_on ? p.drop_scale : 1.0f;
+  const uint32_t sP = smem_u32(smem + FB_OFF_P), sdS = smem_u32(smem + FB_OFF_DS);
+  int cur_rb = -1;
+  for (int j = 0; j < n_items; ++j) {
+    const int w = item_begin + j;
+    const int rb = w / p.heads, h = w - rb * p.heads;
+    const int b = j & 1;
+    uint8_t* in = smem + b * FB_IN_BYTES;
+    const uint32_t sQ = smem_u32(in), sK = sQ + FA_TILE_BYTES, sV = sQ + 2 * FA_TILE_BYTES,
+                   sdO = sQ + 3 * FA_TILE_BYTES;
+
+    named_bar(1, 256);  // both warpgroups are done with the previous item's P~ / dS tiles and mask
+    if (rb != cur_rb) {
+      if (c == 0)
+        madd[t] = fa_key_mask(p.mask_a, p.mask_b, p.Wa, p.Fb, p.Nb, p.all_pairs, p.S, p.G, p.n_seq, NK, rb, t);
+      named_bar(2, 256);
+      cur_rb = rb;
     }
-  } else {
-    // ------------------------------------------ compute warps -----------------------------------------
-    const uint64_t seed = (p.drop_on && p.rng != nullptr) ? p.rng[0] : 0ull;
-    const uint64_t stream = p.stream + ((p.drop_on && p.rng != nullptr) ? (p.rng[1] << 20) : 0ull);
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;       // which warp of the lane quarter's pair
-    const int row = q * 32 + lane;
-    const uint32_t lane_base = (uint32_t)(q * 32) << 16;
-    const int g = row / p.S;
-    const int c0 = g * p.S;
-    const int qpos = row - c0;
-    const float sl2 = p.scale * 1.44269504088896340736f;
-    const float neg_big = -10000.0f * 1.44269504088896340736f;
-    int cur_rb = -1;
-    for (int j = 0; j < n_items; ++j) {
-      const int w = item_begin + j;
-      const int rb = w / p.heads, h = w - rb * p.heads;
-      if (rb != cur_rb) {
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        if (half == 0) {
-          float m = 0.f;
-          if (row < NK) {
-            const long long seq = (long long)rb * p.G + g;
-            long long mv = 1;
-            if (p.mask_a != nullptr && seq < p.n_seq) {
-              const long long mi = p.all_pairs ? seq / p.Nb : seq, mj = p.all_pairs ? seq % p.Nb : seq;
-              if (qpos < p.Wa) mv = p.mask_a[mi * p.Wa + qpos];
-              else if (p.mask_b != nullptr) mv = p.mask_b[mj * p.Fb + (qpos - p.Wa)];
-            }
-            m = mv != 0 ? 0.f : neg_big;
-          }
-          madd[row] = m;
+    mbar_wait(&in_full[b], ((uint32_t)j >> 1) & 1);
+
+    // ---- S = Q K^T, dP = dO V^T for this warpgroup's 64 query rows ----
+    float sa[NK / 2], dpa[NK / 2];
+#pragma unroll
+    for (int e = 0; e < NK / 2; ++e) sa[e] = dpa[e] = 0.f;
+    wgmma_fence();
+    fence_regs(sa);
+    fence_regs(dpa);
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      WgmmaSS<NK>::template mma<0, 0>(sa, make_smem_desc_sw128(sQ + c * (64 * 128) + 32 * k, 16, 1024),
+                                      make_smem_desc_sw128(sK + 32 * k, 16, 1024), k > 0 ? 1 : 0);
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      WgmmaSS<NK>::template mma<0, 0>(dpa, make_smem_desc_sw128(sdO + c * (64 * 128) + 32 * k, 16, 1024),
+                                      make_smem_desc_sw128(sV + 32 * k, 16, 1024), k > 0 ? 1 : 0);
+    wgmma_commit();
+
+    // D_i = <dO_i, O_i> over the 64 dims of this head (each quad lane: 16 of them), while the products run
+    float D[2];
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      const int row = r_lo + 8 * hr;
+      const uint8_t* drow = in + 3 * FA_TILE_BYTES + row * 128;
+      const uint8_t* orow = drow + FA_TILE_BYTES;
+      float d = 0.f;
+#pragma unroll
+      for (int cc = 0; cc < 2; ++cc) {
+        const int off = ((2 * quad + cc) ^ (row & 7)) << 4;
+        const uint4 ud = *reinterpret_cast<const uint4*>(drow + off), uo = *reinterpret_cast<const uint4*>(orow + off);
+        const uint32_t wo[4] = {uo.x, uo.y, uo.z, uo.w}, wd[4] = {ud.x, ud.y, ud.z, ud.w};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float2 a = unpack_bf16x2(wo[e]), bb = unpack_bf16x2(wd[e]);
+          d = fmaf(a.x, bb.x, d);
+          d = fmaf(a.y, bb.y, d);
         }
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        cur_rb = rb;
       }
+      d += __shfl_xor_sync(0xffffffffu, d, 1);
+      d += __shfl_xor_sync(0xffffffffu, d, 2);
+      D[hr] = d;
+    }
+    wgmma_wait<0>();
+    fence_regs(sa);
+    fence_regs(dpa);
+
+    // ---- P~, dS: to registers (dS as the A operand of dQ) and to the shared-memory tiles (dK, dV) ----
+    uint32_t dsa[NK / 16][4];
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      const int row = r_lo + 8 * hr;
+      const int g = row / p.S, c0 = g * p.S, qpos = row - c0;
       const long long seq = (long long)rb * p.G + g;
-      const long long tok = (long long)rb * p.RB + row;
       const bool valid = row < p.RB && seq < p.n_seq;
       const long long bh = seq * p.heads + h;
-      const int b = j & 1;
-      const uint32_t tb = tmem_base + b * FB_BUF_COLS;
       const float lse2 = valid ? p.lse[bh * p.S + qpos] * 1.44269504088896340736f : 0.f;
-      mbar_wait(&in_full[b], ((uint32_t)j >> 1) & 1);   // the item's operand tiles (dO, O read below) have landed
-      mbar_wait(&sd_full[b], ((uint32_t)j >> 1) & 1);   // S, dP in TMEM
-      tc_fence_after_sync();
-      // D_i = <dO_i, O_i> over the 64 dims of this head, from the swizzled dO / O tiles in shared memory
-      float D = 0.f;
-      {
-        const uint8_t* drow = smem + b * FB_IN_BYTES + 3 * FA_TILE_BYTES + row * 128;
-        const uint8_t* orow = drow + FA_TILE_BYTES;
-#pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          const int off = (c ^ (row & 7)) << 4;
-          const uint4 ud = *reinterpret_cast<const uint4*>(drow + off), uo = *reinterpret_cast<const uint4*>(orow + off);
-          const uint32_t wo[4] = {uo.x, uo.y, uo.z, uo.w}, wd[4] = {ud.x, ud.y, ud.z, ud.w};
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float2 a = unpack_bf16x2(wo[e]), bb = unpack_bf16x2(wd[e]);
-            D = fmaf(a.x, bb.x, D);
-            D = fmaf(a.y, bb.y, D);
-          }
-        }
+      uint32_t keep[(NK / 8 + 15) / 16];
+      if (p.drop_on) {
+        const uint64_t base = ((uint64_t)bh * p.S + qpos) * (uint64_t)(p.S >> 3);
+        fa_keep_bits<NK>(seed, stream, base, c0 >> 3, p.drop_threshold, quad, keep);
       }
       uint8_t* prow = smem + FB_OFF_P + row * 128;
       uint8_t* srow = smem + FB_OFF_DS + row * 128;
-      const int sw = row & 7;
-      const float ds_scale = p.drop_on ? p.drop_scale : 1.0f;
-      for (int c = half * 16; c < NK; c += 32) {   // this warp's 16-key chunks
-        uint4 pu0 = make_uint4(0, 0, 0, 0), pu1 = pu0, su0 = pu0, su1 = pu0;
-        uint32_t rs[16], rp[16];
-        // warp-collective loads (one column address per warp); lanes of other packed sequences ignore the chunk
-        tmem_ld_32x32b_x16(tb + FB_COL_S + lane_base + c, rs);
-        tmem_ld_32x32b_x16(tb + FB_COL_DP + lane_base + c, rp);
-        tmem_ld_wait();
-        if (valid && c >= c0 && c < c0 + p.S) {
-          const int kc = c - c0;
-          uint32_t keep = 0xFFFFu;
-          if (p.drop_on) {
-            const uint64_t base = ((uint64_t)bh * p.S + qpos) * (uint64_t)(p.S >> 3) + (uint64_t)(kc >> 3);
-            keep = 0;
 #pragma unroll
-            for (int g8 = 0; g8 < 2; ++g8) {
-              const uint4 rnd = philox4x32(seed, stream, base + g8);
+      for (int jj = 0; jj < NK / 8; ++jj) {
+        float pd[2], dsv[2];
 #pragma unroll
-              for (int e = 0; e < 8; ++e)
-                if (philox_u16(rnd, e) < p.drop_threshold) keep |= 1u << (g8 * 8 + e);
-            }
-          }
-          float pd[16], dsv[16];
-          float a[16];
-#pragma unroll
-          for (int e4 = 0; e4 < 4; ++e4) {
-            const float4 m4 = *reinterpret_cast<const float4*>(madd + c + e4 * 4);
-            a[e4 * 4] = m4.x; a[e4 * 4 + 1] = m4.y; a[e4 * 4 + 2] = m4.z; a[e4 * 4 + 3] = m4.w;
-          }
-          if (p.causal) {   // warp-uniform
-#pragma unroll
-            for (int e = 0; e < 16; ++e)
-              if ((kc + e) > qpos && a[e] == 0.f) a[e] = neg_big;
-          }
-#pragma unroll
-          for (int e = 0; e < 16; ++e) {
-            const float pr = ex2_approx(fmaf(__uint_as_float(rs[e]), sl2, a[e]) - lse2);
-            const bool kp = (keep >> e) & 1u;
-            const float gdrop = kp ? __uint_as_float(rp[e]) * ds_scale : 0.f;
-            pd[e] = kp ? pr * ds_scale : 0.f;
-            dsv[e] = pr * (gdrop - D) * p.scale;
-          }
-          pu0.x = pack_bf16x2(pd[0], pd[1]);   pu0.y = pack_bf16x2(pd[2], pd[3]);
-          pu0.z = pack_bf16x2(pd[4], pd[5]);   pu0.w = pack_bf16x2(pd[6], pd[7]);
-          pu1.x = pack_bf16x2(pd[8], pd[9]);   pu1.y = pack_bf16x2(pd[10], pd[11]);
-          pu1.z = pack_bf16x2(pd[12], pd[13]); pu1.w = pack_bf16x2(pd[14], pd[15]);
-          su0.x = pack_bf16x2(dsv[0], dsv[1]);   su0.y = pack_bf16x2(dsv[2], dsv[3]);
-          su0.z = pack_bf16x2(dsv[4], dsv[5]);   su0.w = pack_bf16x2(dsv[6], dsv[7]);
-          su1.x = pack_bf16x2(dsv[8], dsv[9]);   su1.y = pack_bf16x2(dsv[10], dsv[11]);
-          su1.z = pack_bf16x2(dsv[12], dsv[13]); su1.w = pack_bf16x2(dsv[14], dsv[15]);
+        for (int e = 0; e < 2; ++e) {
+          const int key = 8 * jj + 2 * quad + e;
+          const bool own = valid && key >= c0 && key < c0 + p.S;
+          float a = madd[key];
+          if (p.causal && (key - c0) > qpos && a == 0.f) a = neg_big;
+          const float pr = ex2_approx(fmaf(sa[4 * jj + 2 * hr + e], sl2, a) - lse2);
+          const bool kp = !p.drop_on || ((keep[jj >> 4] >> (2 * (jj & 15) + e)) & 1u);
+          const float gdrop = kp ? dpa[4 * jj + 2 * hr + e] * ds_scale : 0.f;
+          pd[e] = own && kp ? pr * ds_scale : 0.f;
+          dsv[e] = own ? pr * (gdrop - D[hr]) * p.scale : 0.f;
         }
-        const int atom = c >> 6, chunk = (c & 63) >> 3;
-        const int o0 = atom * FA_TILE_BYTES + ((chunk ^ sw) << 4), o1 = atom * FA_TILE_BYTES + (((chunk + 1) ^ sw) << 4);
-        *reinterpret_cast<uint4*>(prow + o0) = pu0;
-        *reinterpret_cast<uint4*>(prow + o1) = pu1;
-        *reinterpret_cast<uint4*>(srow + o0) = su0;
-        *reinterpret_cast<uint4*>(srow + o1) = su1;
+        const uint32_t pu = pack_bf16x2(pd[0], pd[1]), su = pack_bf16x2(dsv[0], dsv[1]);
+        dsa[jj >> 1][(jj & 1) * 2 + hr] = su;
+        const int off = (jj >> 3) * FA_TILE_BYTES + (((jj & 7) ^ (row & 7)) << 4) + quad * 4;
+        *reinterpret_cast<uint32_t*>(prow + off) = pu;
+        *reinterpret_cast<uint32_t*>(srow + off) = su;
       }
-      fence_proxy_async_smem();
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(pds_ready);
-
-      // ---- drain: rows = tile rows (queries for dQ, keys for dK / dV); this warp's 96 of the 192 gradient columns ----
-      mbar_wait(&acc_full[b], ((uint32_t)j >> 1) & 1);
-      tc_fence_after_sync();
-      const bool row_ok = row < p.RB && tok < p.T;
-#pragma unroll
-      for (int part = 0; part < 3; ++part) {
-        // warp half 0: dQ[0:32) dQ[32:64) dK[0:32) ; half 1: dK[32:64) dV[0:32) dV[32:64)
-        const int idx = half * 3 + part;             // 32-column block index 0..5 over dQ | dK | dV
-        const int m = idx >> 1, cb = (idx & 1) * 32;
-        const uint32_t tcol = (m == 0 ? FB_COL_DQ : m == 1 ? FB_COL_DK : FB_COL_DV) + cb;
-        uint32_t r0[16], r1[16];
-        tmem_ld_32x32b_x16(tb + tcol + lane_base, r0);
-        tmem_ld_32x32b_x16(tb + tcol + 16 + lane_base, r1);
-        tmem_ld_wait();
-        float v[32];
-#pragma unroll
-        for (int e = 0; e < 16; ++e) {
-          v[e] = row_ok ? __uint_as_float(r0[e]) : 0.f;
-          v[16 + e] = row_ok ? __uint_as_float(r1[e]) : 0.f;
-        }
-        if (row_ok) {
-          bf16* dst = p.dqkv + tok * p.ld_dqkv + m * H + h * 64 + cb;
-#pragma unroll
-          for (int c8 = 0; c8 < 4; ++c8) {
-            uint4 u;
-            u.x = pack_bf16x2(v[c8 * 8 + 0], v[c8 * 8 + 1]);
-            u.y = pack_bf16x2(v[c8 * 8 + 2], v[c8 * 8 + 3]);
-            u.z = pack_bf16x2(v[c8 * 8 + 4], v[c8 * 8 + 5]);
-            u.w = pack_bf16x2(v[c8 * 8 + 6], v[c8 * 8 + 7]);
-            *reinterpret_cast<uint4*>(dst + c8 * 8) = u;
-          }
-        }
-        if (p.dbias != nullptr) {
-          const float tot = warp_colsum32(v, lane);  // lane l: column cb + l summed over this warp's 32 rows
-          if (tot != 0.f) atomicAdd(p.dbias + m * H + h * 64 + cb + lane, tot);
-        }
-      }
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_free[b]);
     }
-  }
 
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 512);
+    // ---- dQ = dS K (contraction over keys; K [keys][64] is the MN-major B operand) ----
+    float dqa[32];
+#pragma unroll
+    for (int e = 0; e < 32; ++e) dqa[e] = 0.f;
+    wgmma_fence();
+    fence_regs(dqa);
+#pragma unroll
+    for (int kk = 0; kk < NK / 16; ++kk)
+      WgmmaRS<64>::mma<1>(dqa, dsa[kk], make_smem_desc_sw128(sK + kk * 2048, FA_TILE_BYTES, 1024), kk > 0 ? 1 : 0);
+    wgmma_commit();
+
+    fence_proxy_async_smem();  // P~ / dS tile writes -> visible to the tensor core
+    named_bar(3, 256);         // both warpgroups' query rows are in the tiles
+
+    // ---- dV = P~^T dO, dK = dS^T Q for key rows [64 c, 64 c + 64): contraction over the RB query rows ----
+    float dva[32], dka[32];
+#pragma unroll
+    for (int e = 0; e < 32; ++e) dva[e] = dka[e] = 0.f;
+    wgmma_fence();
+    fence_regs(dva);
+    fence_regs(dka);
+#pragma unroll
+    for (int kk = 0; kk < NK / 16; ++kk) {
+      WgmmaSS<64>::mma<1, 1>(dva, make_smem_desc_sw128(sP + c * FA_TILE_BYTES + kk * 2048, FA_TILE_BYTES, 1024),
+                             make_smem_desc_sw128(sdO + kk * 2048, FA_TILE_BYTES, 1024), kk > 0 ? 1 : 0);
+      WgmmaSS<64>::mma<1, 1>(dka, make_smem_desc_sw128(sdS + c * FA_TILE_BYTES + kk * 2048, FA_TILE_BYTES, 1024),
+                             make_smem_desc_sw128(sQ + kk * 2048, FA_TILE_BYTES, 1024), kk > 0 ? 1 : 0);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(dqa);
+    fence_regs(dva);
+    fence_regs(dka);
+    if (t == 0) mbar_arrive(&in_empty[b]);  // this warpgroup no longer reads the item's input tiles
+
+    const int part_row = rb * 8 + c * 4 + warp;
+    fb_drain(p, dqa, rb, r_lo, quad, lane, h * 64, part_row);
+    fb_drain(p, dka, rb, r_lo, quad, lane, H + h * 64, part_row);
+    fb_drain(p, dva, rb, r_lo, quad, lane, 2 * H + h * 64, part_row);
   }
 }
+
+template <int NK>
+struct FaBwdKernel {
+  static constexpr auto kernel = fused_attention_bwd_kernel<NK>;
+};
 
 }  // namespace univl
 
@@ -1066,8 +748,8 @@ extern "C" int univl_fused_attention_bwd(const void* qkv, long long ld_qkv, cons
   FusedAttnBwdParams p = {};
   p.T = n_seq * S; p.S = S; p.G = 128 / S; p.RB = p.G * S; p.n_seq = n_seq; p.heads = heads;
   p.n_blocks = (n_seq + p.G - 1) / p.G;
-  p.o = (const bf16*)o; p.ldo = ldo; p.d_o = (const bf16*)d_o; p.lddo = lddo; p.lse = lse;
-  p.dqkv = (bf16*)dqkv; p.ld_dqkv = ld_dqkv; p.dbias = dbias;
+  p.lse = lse;
+  p.dqkv = (bf16*)dqkv; p.ld_dqkv = ld_dqkv;
   p.mask_a = mask_a; p.mask_b = mask_b; p.Wa = Wa; p.Fb = Fb; p.Nb = Nb > 0 ? Nb : 1; p.all_pairs = all_pairs;
   p.causal = causal; p.scale = scale;
   p.drop_on = p_drop > 0.f;
@@ -1079,15 +761,21 @@ extern "C" int univl_fused_attention_bwd(const void* qkv, long long ld_qkv, cons
   if ((rc = make_tmap(&tq, qkv, p.T, 3 * H, ld_qkv, 128))) return rc;   // box {64 cols, 128 rows}
   if ((rc = make_tmap(&td, d_o, p.T, H, lddo, 128))) return rc;
   if ((rc = make_tmap(&to, o, p.T, H, ldo, 128))) return rc;
-  cudaError_t e = cudaFuncSetAttribute(fused_attention_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       FB_SMEM_BYTES);
-  if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "fused_attention_bwd smem attribute: %s", cudaGetErrorString(e));
   const int sms = usable_sms();
   const long long items = (long long)p.n_blocks * heads;
   const int grid = (int)(items < sms ? items : sms);
-  e = launch_kernel(fused_attention_bwd_kernel, dim3(grid), dim3(FB_THREADS), (size_t)FB_SMEM_BYTES,
-                    (cudaStream_t)stream, tq, td, to, p);
-  if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "fused_attention_bwd launch: %s", cudaGetErrorString(e));
-  UNIVL_CHECK_LAUNCH("fused_attention_bwd");
-  return UNIVL_OK;
+  const int n_parts = p.n_blocks * 8;
+  if (dbias != nullptr)
+    if ((rc = scratch_alloc((void**)&p.dbias, (size_t)n_parts * 3 * H * sizeof(float), (cudaStream_t)stream))) return rc;
+  rc = fa_dispatch<FaBwdKernel>(p.RB, [&](auto kern) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, FB_SMEM_BYTES);
+    if (e != cudaSuccess)
+      return set_error(UNIVL_ERR_CUDA, "fused_attention_bwd smem attribute: %s", cudaGetErrorString(e));
+    e = launch_kernel(kern, dim3(grid), dim3(FA_THREADS), (size_t)FB_SMEM_BYTES, (cudaStream_t)stream, tq, td, to, p);
+    if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "fused_attention_bwd launch: %s", cudaGetErrorString(e));
+    UNIVL_CHECK_LAUNCH("fused_attention_bwd");
+    return UNIVL_OK;
+  });
+  if (rc != UNIVL_OK || dbias == nullptr) return rc;
+  return partials_reduce(p.dbias, n_parts, 1, 3 * H, dbias, 3 * H, (cudaStream_t)stream);
 }

@@ -8,7 +8,8 @@
 // One warp owns one row at a time (cols <= 1024, cols % 256 == 0 -> 1..4 16-byte vectors per lane); all statistics are
 // fp32 and two-pass over registers, exactly the reference's mean -> centred variance order.  Backward regenerates the
 // dropout mask from (seed, stream) and accumulates dgamma / dbeta / dbias column sums in registers across the rows a
-// warp walks, then reduces through shared memory and issues one atomicAdd per column per CTA.
+// warp walks, then reduces through shared memory into one partial row per CTA; partials_reduce adds the rows in CTA
+// order.
 #include "common.cuh"
 
 namespace univl {
@@ -191,7 +192,7 @@ static void launch_ln_fwd(int grid, cudaStream_t st, const TIn* x, const bf16* r
 // Backward.  dz = rstd * (g - mean(g) - xhat * mean(g * xhat)),  g = dy_eff * gamma.
 //   dx_res   (bf16, may be null): dz                       — gradient w.r.t. the residual input (and x when no dropout)
 //   dx_dense (bf16, may be null): dz * keep/(1-p)          — gradient w.r.t. x under drop_mode 1
-//   dgamma, dbeta (fp32, atomically accumulated), dbias (fp32, optional) += column sums of dx_dense (or dz)
+//   dgamma, dbeta (fp32), dbias (fp32, optional) += column sums of dx_dense (or dz), summed in a fixed order
 
 // one 8-wide vector of the row: z = pre-LayerNorm value, d = effective upstream gradient, keep = dropout bit mask
 template <typename TIn>
@@ -300,7 +301,7 @@ layernorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ dy2, 
       if (dx_dense != nullptr && dx_dense != dx_res) store8(dx_dense + row * cols + c, dd);
     }
   }
-  // column sums: add the LNB_WARPS slices, one atomic per column per CTA
+  // column sums: add the LNB_WARPS slices, one partial row per column and CTA
   __syncthreads();
   for (int which = 0; which < 3; ++which) {
     float* dst = which == 0 ? dgamma : which == 1 ? dbeta : dbias;
@@ -309,22 +310,34 @@ layernorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ dy2, 
       float t = 0.f;
 #pragma unroll
       for (int w = 0; w < LNB_WARPS; ++w) t += lnb_acc[(w * 3 + which) * cols + e];
-      atomicAdd(dst + e, t);
+      dst[(long long)blockIdx.x * cols + e] = t;  // this CTA's partial (partials_reduce sums them in order)
     }
   }
 }
 
 template <typename TIn>
-static void launch_ln_bwd(int grid, cudaStream_t st, const bf16* dy, const bf16* dy2, const TIn* x, const bf16* res,
-                          const float* gamma, const float* mean, const float* rstd, bf16* dx_res, bf16* dx_dense,
-                          float* dgamma, float* dbeta, float* dbias, int rows, int cols, DropCfg drop) {
+static int launch_ln_bwd(int grid, cudaStream_t st, const bf16* dy, const bf16* dy2, const TIn* x, const bf16* res,
+                         const float* gamma, const float* mean, const float* rstd, bf16* dx_res, bf16* dx_dense,
+                         float* dgamma_out, float* dbeta_out, float* dbias_out, int rows, int cols, DropCfg drop) {
   const size_t smem = (size_t)LNB_WARPS * 3 * cols * sizeof(float);
+  // parameter gradients: per-CTA partial rows, summed in CTA order after the kernel
+  float* outs[3] = {dgamma_out, dbeta_out, dbias_out};
+  float* parts[3] = {nullptr, nullptr, nullptr};
+  for (int w = 0; w < 3; ++w)
+    if (outs[w] != nullptr)
+      if (int rc = scratch_alloc((void**)&parts[w], (size_t)grid * cols * sizeof(float), st)) return rc;
+  float *dgamma = parts[0], *dbeta = parts[1], *dbias = parts[2];
   switch (cols >> 8) {
     case 1: launch_kernel(layernorm_bwd_kernel<TIn, 1>, dim3(grid), dim3(LNB_WARPS * 32), smem, st, dy, dy2, x, res, gamma, mean, rstd, dx_res, dx_dense, dgamma, dbeta, dbias, rows, drop); break;
     case 2: launch_kernel(layernorm_bwd_kernel<TIn, 2>, dim3(grid), dim3(LNB_WARPS * 32), smem, st, dy, dy2, x, res, gamma, mean, rstd, dx_res, dx_dense, dgamma, dbeta, dbias, rows, drop); break;
     case 3: launch_kernel(layernorm_bwd_kernel<TIn, 3>, dim3(grid), dim3(LNB_WARPS * 32), smem, st, dy, dy2, x, res, gamma, mean, rstd, dx_res, dx_dense, dgamma, dbeta, dbias, rows, drop); break;
     default: launch_kernel(layernorm_bwd_kernel<TIn, 4>, dim3(grid), dim3(LNB_WARPS * 32), smem, st, dy, dy2, x, res, gamma, mean, rstd, dx_res, dx_dense, dgamma, dbeta, dbias, rows, drop); break;
   }
+  UNIVL_CHECK_LAUNCH("layernorm_bwd");
+  for (int w = 0; w < 3; ++w)
+    if (parts[w] != nullptr)
+      if (int rc = partials_reduce(parts[w], grid, 1, cols, outs[w], cols, st)) return rc;
+  return UNIVL_OK;
 }
 
 static int check_ln_shape(const char* what, int rows, int cols) {
@@ -347,12 +360,12 @@ static DropCfg make_drop(int mode, float p, const unsigned long long* rng, unsig
 
 static int lnb_grid(int rows) {
   long long blocks = ((long long)rows + LNB_WARPS - 1) / LNB_WARPS;
-  const long long cap = 148LL * 5;
+  const long long cap = (long long)device_sms() * 5;
   return (int)(blocks < 1 ? 1 : (blocks > cap ? cap : blocks));
 }
 static int ln_grid(int rows) {
   long long blocks = ((long long)rows + LN_WARPS - 1) / LN_WARPS;
-  const long long cap = 148LL * 8;
+  const long long cap = (long long)device_sms() * 8;
   return (int)(blocks < 1 ? 1 : (blocks > cap ? cap : blocks));
 }
 
@@ -386,11 +399,9 @@ extern "C" int univl_layernorm_bwd(const void* dy, const void* dy2, const void* 
   UNIVL_CHECK_ARG(p_drop == 0.f || rng_state != nullptr, "layernorm_bwd: dropout needs rng_state");
   UNIVL_CHECK_ARG(p_drop >= 0.f && p_drop < 1.f && drop_mode >= 0 && drop_mode <= 2, "layernorm_bwd: bad dropout");
   if (rows == 0) return UNIVL_OK;
-  launch_ln_bwd<bf16>(lnb_grid(rows), (cudaStream_t)stream, (const bf16*)dy, (const bf16*)dy2, (const bf16*)x,
-                      (const bf16*)res, gamma, mean, rstd, (bf16*)dx_res, (bf16*)dx_dense, dgamma, dbeta, dbias, rows,
-                      cols, make_drop(drop_mode, p_drop, rng_state, stream_id));
-  UNIVL_CHECK_LAUNCH("layernorm_bwd");
-  return UNIVL_OK;
+  return launch_ln_bwd<bf16>(lnb_grid(rows), (cudaStream_t)stream, (const bf16*)dy, (const bf16*)dy2, (const bf16*)x,
+                             (const bf16*)res, gamma, mean, rstd, (bf16*)dx_res, (bf16*)dx_dense, dgamma, dbeta, dbias,
+                             rows, cols, make_drop(drop_mode, p_drop, rng_state, stream_id));
 }
 
 // fp32 input rows (NormalizeVideo, reference modules/modeling.py:88-92): y(bf16) = LN(x_f32); no dropout.
@@ -412,8 +423,6 @@ extern "C" int univl_layernorm_f32_bwd(const void* dy, const float* x, const flo
   if (int rc = check_ln_shape("layernorm_f32_bwd", rows, cols)) return rc;
   UNIVL_CHECK_ARG(dy && x && gamma && mean && rstd && dgamma && dbeta, "layernorm_f32_bwd: null pointer");
   if (rows == 0) return UNIVL_OK;
-  launch_ln_bwd<float>(lnb_grid(rows), (cudaStream_t)stream, (const bf16*)dy, nullptr, x, nullptr, gamma, mean, rstd,
-                       nullptr, nullptr, dgamma, dbeta, nullptr, rows, cols, make_drop(0, 0.f, nullptr, 0));
-  UNIVL_CHECK_LAUNCH("layernorm_f32_bwd");
-  return UNIVL_OK;
+  return launch_ln_bwd<float>(lnb_grid(rows), (cudaStream_t)stream, (const bf16*)dy, nullptr, x, nullptr, gamma, mean,
+                              rstd, nullptr, nullptr, dgamma, dbeta, nullptr, rows, cols, make_drop(0, 0.f, nullptr, 0));
 }

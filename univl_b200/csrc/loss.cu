@@ -143,9 +143,24 @@ maxmargin_kernel(const float* __restrict__ sim, float* __restrict__ loss, float*
     const float a = margin + s - sim[i * B + i];
     const float c = margin + s - sim[j * B + j];
     float gs = 0.f;
-    if (a > 0.f) { acc += w * a; gs += w * inv; atomicAdd(&dsim[i * B + i], -w * inv); }
-    if (c > 0.f) { acc += w * c; gs += w * inv; atomicAdd(&dsim[j * B + j], -w * inv); }
-    if (gs != 0.f) atomicAdd(&dsim[e], gs);
+    if (a > 0.f) { acc += w * a; gs += w * inv; }
+    if (c > 0.f) { acc += w * c; gs += w * inv; }
+    dsim[e] = gs;
+  }
+  __syncthreads();
+  // the diagonal s_kk appears in every term of row k (a) and column k (c): add those in a fixed order
+  for (int k = threadIdx.x; k < B; k += blockDim.x) {
+    const float skk = sim[k * B + k];
+    float t = 0.f;
+    for (int j = 0; j < B; ++j) {
+      const float w = (n_pair > 0) ? ((k / n_pair == j / n_pair) ? w_same : w_diff) : 1.f;
+      if (margin + sim[k * B + j] - skk > 0.f) t -= w * inv;
+    }
+    for (int i = 0; i < B; ++i) {
+      const float w = (n_pair > 0) ? ((i / n_pair == k / n_pair) ? w_same : w_diff) : 1.f;
+      if (margin + sim[i * B + k] - skk > 0.f) t -= w * inv;
+    }
+    dsim[k * B + k] += t;
   }
   acc = block_sum(acc, red);
   if (threadIdx.x == 0) *loss = acc * inv;
@@ -318,7 +333,7 @@ pooler_sim_fwd_kernel(const bf16* __restrict__ u, const float* __restrict__ w, c
 __global__ void __launch_bounds__(256)
 pooler_sim_bwd_kernel(const bf16* __restrict__ u, const float* __restrict__ w, const float* __restrict__ dout,
                       bf16* __restrict__ du, float* __restrict__ dw, float* __restrict__ db, int N, int H) {
-  // one CTA handles a slab of rows; threads own columns so dw needs one atomic per column per CTA
+  // one CTA handles a slab of rows; threads own columns; dw / db receive this CTA's partial row (summed in CTA order)
   const int rows_per = (N + gridDim.x - 1) / gridDim.x;
   const int r0 = blockIdx.x * rows_per, r1 = min(N, r0 + rows_per);
   for (int c = threadIdx.x; c < H; c += blockDim.x) {
@@ -330,12 +345,12 @@ pooler_sim_bwd_kernel(const bf16* __restrict__ u, const float* __restrict__ w, c
       acc += g * th;
       du[(long long)r * H + c] = __float2bfloat16(g * wc * (1.f - th * th));
     }
-    atomicAdd(dw + c, acc);
+    dw[(long long)blockIdx.x * H + c] = acc;
   }
   if (threadIdx.x == 0) {
     float s = 0.f;
     for (int r = r0; r < r1; ++r) s += dout[r];
-    atomicAdd(db, s);
+    db[blockIdx.x] = s;
   }
 }
 
@@ -442,17 +457,22 @@ extern "C" int univl_pooler_sim_bwd(const void* u, const float* w, const float* 
                                     int N, int H, void* stream) {
   UNIVL_CHECK_ARG(u && w && dout && du && dw && db && N > 0 && H > 0, "pooler_sim_bwd: bad arguments");
   int blocks = (N + 15) / 16;
-  if (blocks > 148) blocks = 148;
-  pooler_sim_bwd_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>((const bf16*)u, w, dout, (bf16*)du, dw, db, N, H);
+  if (blocks > device_sms()) blocks = device_sms();
+  cudaStream_t st = (cudaStream_t)stream;
+  float *pw, *pb;
+  if (int rc = scratch_alloc((void**)&pw, (size_t)blocks * H * sizeof(float), st)) return rc;
+  if (int rc = scratch_alloc((void**)&pb, (size_t)blocks * sizeof(float), st)) return rc;
+  pooler_sim_bwd_kernel<<<blocks, 256, 0, st>>>((const bf16*)u, w, dout, (bf16*)du, pw, pb, N, H);
   UNIVL_CHECK_LAUNCH("pooler_sim_bwd");
-  return UNIVL_OK;
+  if (int rc = partials_reduce(pw, blocks, 1, H, dw, H, st)) return rc;
+  return partials_reduce(pb, blocks, 1, 1, db, 1, st);
 }
 // dst[i] = src[i] * (*gscale)   — applies autograd's upstream scalar without a host round trip
 extern "C" int univl_scale_f32(float* dst, const float* src, long long n, const float* gscale, void* stream) {
   UNIVL_CHECK_ARG(dst && src && gscale && n >= 0, "scale_f32: bad arguments");
   if (n == 0) return UNIVL_OK;
   long long blocks = (n + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > device_sms() * 8) blocks = device_sms() * 8;
   scale_f32_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(dst, src, n, gscale);
   UNIVL_CHECK_LAUNCH("scale_f32");
   return UNIVL_OK;

@@ -10,7 +10,8 @@ __device__ __forceinline__ uint4 ld_nc_v4(const bf16* p) {
   return u;
 }
 
-// out[c] += sum_r x[r, c]   (bf16 in, fp32 atomic accumulate).  Block = 32 column-vectors (256 cols) x 8 row lanes.
+// partial[row block][c] = sum_r x[r, c] over the block's rows (bf16 in, fp32); univl_colsum_bf16 adds the partials
+// to out[c] in row-block order.  Block = 32 column-vectors (256 cols) x 8 row lanes.
 __global__ void __launch_bounds__(256)
 colsum_bf16_kernel(const bf16* __restrict__ x, long long ld, float* __restrict__ out, int rows, int cols,
                    int rows_per_block) {
@@ -64,7 +65,7 @@ colsum_bf16_kernel(const bf16* __restrict__ x, long long ld, float* __restrict__
     float t = 0.f;
 #pragma unroll
     for (int w = 0; w < 8; ++w) t += red[w][e];
-    atomicAdd(out + c, t);
+    out[(long long)blockIdx.y * cols + c] = t;  // this row block's partial (partials_reduce sums them in order)
   }
 }
 
@@ -147,22 +148,24 @@ extern "C" int univl_colsum_bf16(const void* x, long long ld, float* out, int ro
   UNIVL_CHECK_ARG(x && out && rows >= 0 && cols > 0, "colsum: bad arguments");
   if (rows == 0) return UNIVL_OK;
   const int col_blocks = (cols + 255) / 256;
-  int row_blocks = (148 * 4 + col_blocks - 1) / col_blocks;
+  int row_blocks = (device_sms() * 4 + col_blocks - 1) / col_blocks;
   if (row_blocks > (rows + 63) / 64) row_blocks = (rows + 63) / 64;
   if (row_blocks < 1) row_blocks = 1;
   const int rpb = (rows + row_blocks - 1) / row_blocks;
   row_blocks = (rows + rpb - 1) / rpb;
+  float* part;
+  if (int rc = scratch_alloc((void**)&part, (size_t)row_blocks * cols * sizeof(float), (cudaStream_t)stream)) return rc;
   launch_kernel(colsum_bf16_kernel, dim3(col_blocks, row_blocks), dim3(256), 0, (cudaStream_t)stream, (const bf16*)x, ld,
-                out, rows, cols, rpb);
+                part, rows, cols, rpb);
   UNIVL_CHECK_LAUNCH("colsum_bf16");
-  return UNIVL_OK;
+  return partials_reduce(part, row_blocks, 1, cols, out, cols, (cudaStream_t)stream);
 }
 
 extern "C" int univl_cast_f32_to_bf16(const float* src, void* dst, long long n, void* stream) {
   UNIVL_CHECK_ARG(src && dst && n >= 0, "cast: bad arguments");
   if (n == 0) return UNIVL_OK;
   long long blocks = (n + 2047) / 2048;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > device_sms() * 8) blocks = device_sms() * 8;
   cast_f32_bf16_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(src, (bf16*)dst, n);
   UNIVL_CHECK_LAUNCH("cast_f32_to_bf16");
   return UNIVL_OK;
@@ -188,7 +191,7 @@ extern "C" int univl_cast_bf16_to_f32(const void* src, float* dst, long long n, 
   UNIVL_CHECK_ARG(((uintptr_t)src & 15) == 0 && ((uintptr_t)dst & 15) == 0, "cast_bf16_to_f32: 16-byte alignment");
   if (n == 0) return UNIVL_OK;
   long long blocks = (n + 2047) / 2048;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > device_sms() * 8) blocks = device_sms() * 8;
   cast_bf16_f32_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>((const bf16*)src, dst, n);
   UNIVL_CHECK_LAUNCH("cast_bf16_to_f32");
   return UNIVL_OK;
@@ -208,7 +211,7 @@ extern "C" int univl_multi_cast_f32_to_bf16(const unsigned long long* device_tab
 static int launch_eltwise(const void* dy, const void* x, void* out, long long n, int mode, void* stream) {
   if (n == 0) return UNIVL_OK;
   long long blocks = (n + 511) / 512;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > device_sms() * 8) blocks = device_sms() * 8;
   eltwise_bf16_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>((const bf16*)dy, (const bf16*)x, (bf16*)out, n,
                                                                      mode);
   UNIVL_CHECK_LAUNCH("eltwise_bf16");
@@ -240,7 +243,7 @@ extern "C" int univl_fill_f32(float* p, float value, long long n, void* stream) 
     return UNIVL_OK;
   }
   long long blocks = (n + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > device_sms() * 16) blocks = device_sms() * 16;
   fill_f32_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(p, value, n);
   UNIVL_CHECK_LAUNCH("fill_f32");
   return UNIVL_OK;

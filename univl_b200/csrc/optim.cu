@@ -47,7 +47,7 @@ __device__ __forceinline__ float load_grad(const bf16* g, long long e) { return 
 
 template <typename G>
 __global__ void __launch_bounds__(256)
-adam_sumsq_kernel(const G* __restrict__ g, const AdamSeg* __restrict__ segs, float* __restrict__ sumsq,
+adam_sumsq_kernel(const G* __restrict__ g, const AdamSeg* __restrict__ segs, float* __restrict__ part,
                   float grad_scale) {
   __shared__ float red[8];
   const AdamSeg s = segs[blockIdx.x];
@@ -69,8 +69,20 @@ adam_sumsq_kernel(const G* __restrict__ g, const AdamSeg* __restrict__ segs, flo
   if (threadIdx.x == 0) {
     float t = 0.f;
     for (int w = 0; w < 8; ++w) t += red[w];
-    if (t != 0.f) atomicAdd(sumsq + s.tensor, t);
+    part[blockIdx.x] = t;  // this chunk's share; adam_tensor_sums_kernel adds a tensor's chunks in order
   }
+}
+
+// per-chunk sums of squares -> sumsq[tensor], each tensor's chunks added in chunk order
+__global__ void __launch_bounds__(256)
+adam_tensor_sums_kernel(const float* __restrict__ part, const AdamSeg* __restrict__ segs, int n_chunks,
+                        float* __restrict__ sumsq, int n_tensors) {
+  const int i = blockIdx.x * 256 + threadIdx.x;
+  if (i >= n_tensors) return;
+  float t = 0.f;
+  for (int c = 0; c < n_chunks; ++c)
+    if (segs[c].tensor == i) t += part[c];
+  sumsq[i] = t;
 }
 
 // sumsq[n_tensors] -> sumsq[n_tensors] holds the total
@@ -164,9 +176,11 @@ static int adam_step(float* p, const G* g, float* m, float* v, void* p_bf16, con
   UNIVL_CHECK_ARG(n_tensors > 0 && n_chunks >= n_tensors, "bert_adam_step: bad tensor / chunk count");
   cudaStream_t st = (cudaStream_t)stream;
   const AdamSeg* s = reinterpret_cast<const AdamSeg*>(segs);
-  cudaError_t e = cudaMemsetAsync(scratch, 0, (size_t)(n_tensors + 1) * sizeof(float), st);
-  if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "bert_adam_step memset: %s", cudaGetErrorString(e));
-  adam_sumsq_kernel<G><<<n_chunks, 256, 0, st>>>(g, s, scratch, cfg.grad_scale);
+  float* part;
+  if (int rc = scratch_alloc((void**)&part, (size_t)n_chunks * sizeof(float), st)) return rc;
+  adam_sumsq_kernel<G><<<n_chunks, 256, 0, st>>>(g, s, part, cfg.grad_scale);
+  adam_tensor_sums_kernel<<<(n_tensors + 255) / 256, 256, 0, st>>>(part, s, n_chunks, scratch, n_tensors);
+  cudaFreeAsync(part, st);
   adam_total_kernel<<<1, 256, 0, st>>>(scratch, n_tensors);
   adam_update_kernel<G><<<n_chunks, 256, 0, st>>>(p, g, m, v, (bf16*)p_bf16, s, scratch, n_tensors, step, cfg);
   adam_step_inc_kernel<<<1, 1, 0, st>>>(step);

@@ -1,4 +1,4 @@
-// univl_b200 — host-side TMA tensor-map construction shared by the tcgen05 kernels' launchers.
+// univl_b200 — host-side TMA tensor-map construction shared by the wgmma kernels' launchers.
 #pragma once
 
 #include "common.cuh"

@@ -1,5 +1,5 @@
 """UniVL orchestrator — the drop-in surface of the reference's modules/modeling.py (UniVLPreTrainedModel :39-81,
-NormalizeVideo :83-92, UniVL :109-428) driving the fused sm_100a kernels.
+NormalizeVideo :83-92, UniVL :109-428) driving the fused sm_90a kernels.
 
 Same constructor, `from_pretrained`, `forward` (a scalar loss in train mode, None in eval), `get_sequence_visual_output`,
 `get_similarity_logits`, `decoder_caption`, sub-module names, parameter names / tying and stage flags, so the reference
@@ -169,7 +169,7 @@ class UniVL(UniVLPreTrainedModel):
     def _encode(self, input_ids, token_type_ids, attention_mask, video_norm, video_mask):
         """reference :299-313 (inputs already flattened / normalised).  The text and the visual stacks are independent
         until the similarity / cross encoder, and at M = B*W = 1536 rows each of their kernels fills a fraction of the
-        148 SMs: the visual stack runs on a side stream forked from (and joined back into) the current one, so the two
+        132 SMs: the visual stack runs on a side stream forked from (and joined back into) the current one, so the two
         stacks' sub-wave kernels share the machine — forward here, and backward too, because autograd replays every
         node on the stream its forward ran on.  Captured as two parallel branches under CUDA-graph capture."""
         side = rt.side_stream(self._device())

@@ -1,5 +1,5 @@
 """Text encoder — surface of the reference's modules/module_bert.py (BertConfig :44-116, BertModel :364-447,
-BertOnlyMLMHead :333-340) over the fused sm_100a layer kernels."""
+BertOnlyMLMHead :333-340) over the fused sm_90a layer kernels."""
 import logging
 
 import torch

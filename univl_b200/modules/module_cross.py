@@ -1,5 +1,5 @@
 """Cross-modal encoder — surface of the reference's modules/module_cross.py (CrossConfig :44-107, CrossModel
-:355-394) over the fused sm_100a layer kernels."""
+:355-394) over the fused sm_90a layer kernels."""
 import logging
 
 import torch

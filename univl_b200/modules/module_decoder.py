@@ -1,5 +1,5 @@
 """Caption decoder — surface of the reference's modules/module_decoder.py (DecoderConfig :45-109, DecoderModel
-:351-406) over the fused sm_100a layer kernels."""
+:351-406) over the fused sm_90a layer kernels."""
 import logging
 
 import torch

@@ -1,5 +1,5 @@
 """Visual (S3D feature) encoder — surface of the reference's modules/module_visual.py (VisualConfig :44-102,
-VisualModel :364-425, VisualOnlyMLMHead :314-321) over the fused sm_100a layer kernels."""
+VisualModel :364-425, VisualOnlyMLMHead :314-321) over the fused sm_90a layer kernels."""
 import logging
 
 import torch

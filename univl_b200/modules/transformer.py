@@ -3,7 +3,7 @@
 The reference has four copy-pasted BERT stacks (module_bert.py / module_visual.py / module_cross.py /
 module_decoder.py); here ONE set of parameter-holder modules reproduces their attribute paths (and therefore their
 `state_dict` keys, SURVEY.md Appendix A) while the arithmetic of a whole layer is a single fused autograd node
-(univl_b200/ops.py: EncoderLayerFn / DecoderLayerFn) over the sm_100a kernels.  The nn.Linear / nn.Embedding children
+(univl_b200/ops.py: EncoderLayerFn / DecoderLayerFn) over the sm_90a kernels.  The nn.Linear / nn.Embedding children
 only own parameters — their stock forwards are never called.
 """
 import torch

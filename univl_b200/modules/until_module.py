@@ -1,6 +1,6 @@
 """Primitives, the PreTrainedModel base and the similarity losses — the surface of the reference's
 modules/until_module.py (LayerNorm :40-53, gelu :28-33, PreTrainedModel :55-177, CrossEn :182-191, MILNCELoss
-:193-221, MaxMarginRankingLoss :223-251) on top of the sm_100a kernels.  No CPU path: every forward here requires CUDA
+:193-221, MaxMarginRankingLoss :223-251) on top of the sm_90a kernels.  No CPU path: every forward here requires CUDA
 tensors and raises otherwise.
 """
 import logging
@@ -17,7 +17,7 @@ logger = logging.getLogger(__name__)
 
 def _require_cuda(t, what):
     if not t.is_cuda:
-        raise RuntimeError("univl_b200: %s needs CUDA tensors (sm_100a kernels only, no CPU fallback)" % what)
+        raise RuntimeError("univl_b200: %s needs CUDA tensors (sm_90a kernels only, no CPU fallback)" % what)
 
 
 def gelu(x):

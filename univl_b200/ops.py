@@ -3,7 +3,7 @@
 Everything here is plumbing: allocate outputs with torch, hand raw device pointers to the library on the current
 stream, keep what backward needs.  No arithmetic on the hot path is done by torch ops; the forward/backward
 orchestration of a whole transformer block lives in ONE autograd.Function so a layer costs one autograd node and the
-saved activations are exactly the tensors listed in DESIGN.md.
+saved activations are exactly the tensors the backward kernels read.
 """
 import math
 import os
@@ -186,7 +186,7 @@ def fused_attention_supported(n_seq, S, H):
 
 
 def fused_qkv_attention_fwd(x, wqkv, bqkv, n_seq, S, mask, p=0.0, seed=0, stream=0, save_qkv=True):
-    """ctx, lse, qkv = fused QKV projection + self-attention of x[T, H] (one tcgen05 kernel; q/k/v only reach HBM when
+    """ctx, lse, qkv = fused QKV projection + self-attention of x[T, H] (one wgmma kernel; q/k/v only reach HBM when
     `save_qkv` — the copy the backward pass reads)."""
     T, H = x.shape
     _check2d(x, "fused attention x"); _check2d(wqkv, "fused attention wqkv")
@@ -200,7 +200,7 @@ def fused_qkv_attention_fwd(x, wqkv, bqkv, n_seq, S, mask, p=0.0, seed=0, stream
 
 
 def fused_attention_bwd(qkv, o, lse, d_o, dqkv, n_seq, S, mask, p=0.0, seed=0, stream=0, dbias=None):
-    """dqkv[T, 3H] = backward of the attention core on tcgen05 (csrc/fused_attn.cu) for the shapes the fused forward
+    """dqkv[T, 3H] = backward of the attention core on wgmma (csrc/fused_attn.cu) for the shapes the fused forward
     takes; dbias: optional contiguous fp32 [3H] the column sums are added to."""
     call("univl_fused_attention_bwd", qkv.data_ptr(), qkv.stride(0), o.data_ptr(), o.stride(0), lse.data_ptr(),
          d_o.data_ptr(), d_o.stride(0), dqkv.data_ptr(), dqkv.stride(0), ptr(dbias), ptr(mask.a), ptr(mask.b), mask.Wa,
@@ -558,7 +558,7 @@ class EmbedSrcFn(torch.autograd.Function):
 
 
 class LinearFn(torch.autograd.Function):
-    """y = x W^T + b on the tcgen05 GEMM (bf16 in/out, fp32 accumulate); optional fused erf-GELU.
+    """y = x W^T + b on the wgmma GEMM (bf16 in/out, fp32 accumulate); optional fused erf-GELU.
     x may be a strided row view (e.g. the [CLS] rows h[:, 0]).  needs_dx=False skips the input gradient."""
 
     @staticmethod

@@ -142,7 +142,7 @@ class FusedBertAdam(torch.optim.Optimizer):
         first = self.param_groups[0]["params"][0]
         dev = first.device
         if dev.type != "cuda":
-            raise RuntimeError("FusedBertAdam needs CUDA parameters (sm_100a kernels only)")
+            raise RuntimeError("FusedBertAdam needs CUDA parameters (sm_90a kernels only)")
         if self.model is not None:
             flat = flatten(self.model, self.sink_grads)
             self.flat = flat

@@ -186,8 +186,8 @@ class use_model:
     def __enter__(self):
         if self.device.type != "cuda":
             raise RuntimeError(
-                "univl_b200 runs on CUDA (sm_100a) only — there is no CPU path; move the model and inputs to a "
-                "B200 (got device %s)" % self.device)
+                "univl_b200 runs on CUDA (sm_90a) only — there is no CPU path; move the model and inputs to a "
+                "H100 (got device %s)" % self.device)
         prev = getattr(_tls, "arena", None)
         self.prev = prev
         if prev is not None and prev.root is not self.root and _covers(prev, self.root):
