@@ -81,16 +81,20 @@ def test_submodel_forward_surfaces():
     assert float(pooled.float().abs().max()) <= 1.0  # tanh
 
 
-def test_flat_gradient_sinks_match_autograd_gradients():
-    """backward kernels accumulating straight into the flat gradient buffer (fast path) give the same gradients as
-    the autograd-returned ones (the path the reference's DistributedDataParallel wrap uses)."""
+def _flat_sink_case(mode):
     from univl_b200.optim import flatten
-    cfg = _small("pretrain2", batch_size=3)
+    cfg = _small(mode, batch_size=3)
     sd = synth.make_state_dict(cfg)
     batch = synth.make_batch(cfg, seed=6)
     ref_model = build_model(cfg, sd=sd)
     ref_model(**to_device(batch)).backward()
     ref = grads_by_name(ref_model)
+    # a parameter used by several layers (tied weights) gets one gradient per use: autograd adds them in its own
+    # order, the flat sink in kernel launch order, so with three or more uses the last bits may differ
+    uses = {}
+    for name, p in ref_model.named_parameters(remove_duplicate=False):
+        uses.setdefault(id(p), []).append(name)
+    tied = {names[0] for names in uses.values() if len(names) > 1}
     model = build_model(cfg, sd=sd)
     flat = flatten(model, sink_grads=True)
     for _ in range(2):  # second pass checks zero_grad + re-accumulation
@@ -101,11 +105,25 @@ def test_flat_gradient_sinks_match_autograd_gradients():
     assert set(got) >= set(ref)
     for k, r in ref.items():
         g = got[k]
-        tol = 2e-2 * float(r.abs().max()) + 1e-7   # atomic accumulation order differs run to run
-        assert (g - r).abs().max() <= tol, k
+        if k in tied:
+            assert (g - r).abs().max() <= 1e-5 * float(r.abs().max()) + 1e-12, k
+        else:
+            assert torch.equal(g, r), k
     # state_dict is unchanged by flattening (parameters are views now)
     for k, v in sd.items():
         assert torch.equal(model.state_dict()[k].cpu(), v), k
+
+
+def test_flat_gradient_sinks_match_autograd_gradients():
+    """backward kernels accumulating straight into the flat gradient buffer (fast path) give the same gradients as
+    the autograd-returned ones (the path the reference's DistributedDataParallel wrap uses): the same bits, since every
+    kernel adds its sums in a fixed order into a zeroed buffer either way (pretraining stage two: every head)."""
+    _flat_sink_case("pretrain2")
+
+
+def test_flat_gradient_sinks_match_autograd_gradients_ft_align():
+    """the same on the retrieval fine-tuning path, which has no tied weights: every gradient bit for bit"""
+    _flat_sink_case("ft_align")
 
 
 def test_training_steps_with_fused_optimizer_reduce_the_loss():

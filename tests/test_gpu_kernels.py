@@ -8,6 +8,7 @@ import torch
 
 pytestmark = pytest.mark.gpu
 
+from tests import gemm_check as gc  # noqa: E402
 from univl_b200 import ops  # noqa: E402
 from univl_b200 import runtime as rt  # noqa: E402
 
@@ -21,25 +22,20 @@ def _bf(t):
 
 
 # ---------------------------------------------------------------------------------------------------------
+# GEMM: the automatic plan and every epilogue, per element against fp64 (tests/gemm_check.py; the template instances,
+# split-K, scalar path and production shapes are in tests/test_gpu_gemm.py)
 @pytest.mark.parametrize("a_mn,b_mn", [(0, 0), (0, 1), (1, 1), (1, 0)])
 @pytest.mark.parametrize("shape", [(128, 64, 64), (300, 200, 136), (1536, 768, 768), (520, 30522, 768)])
 def test_gemm_all_operand_majors(a_mn, b_mn, shape):
+    """automatic plan (tile width and split-K chosen by the library); MN-major extents that are not multiples of 8 are
+    stored with the leading dimension padded to 64, as the vocab projection stores them"""
     M, N, K = shape
-    if (a_mn and M % 8) or (b_mn and N % 8):
-        pytest.skip("MN-major storage needs the MN extent to be a multiple of 8")
     g = torch.Generator(device=DEV).manual_seed(1)
-    A = _bf(torch.randn(M, K, device=DEV, generator=g) * 0.5)
-    B = _bf(torch.randn(N, K, device=DEV, generator=g) * 0.5)
-    bias = torch.randn(N, device=DEV, generator=g)
-    ref = A.float() @ B.float().t() + bias
-    Am = A.t().contiguous() if a_mn else A
-    Bm = B.t().contiguous() if b_mn else B
-    out = torch.empty(M, N, device=DEV, dtype=torch.float32)
-    ops.gemm(Am, Bm, M, N, K, out, epi=ops.EPI_F32, bias=bias, a_mn=a_mn, b_mn=b_mn)
-    assert (out - ref).abs().max() <= 2e-3 * ref.abs().max()
-    acc = torch.ones(M, N, device=DEV)
-    ops.gemm(Am, Bm, M, N, K, acc, epi=ops.EPI_ATOMIC, a_mn=a_mn, b_mn=b_mn)  # split-K + accumulate
-    assert (acc - (ref - bias + 1.0)).abs().max() <= 2e-3 * ref.abs().max()
+    A, B = gc.bf_randn((M, K), 0.5, g), gc.bf_randn((N, K), 0.5, g)
+    As, Bs = gc.store(A, a_mn, 64), gc.store(B, b_mn, 64)
+    gc.run_epi(ops.EPI_F32, A, B, As, Bs, a_mn, b_mn, g=g, what="auto %s a_mn%d b_mn%d F32" % (shape, a_mn, b_mn))
+    gc.run_epi(ops.EPI_ATOMIC, A, B, As, Bs, a_mn, b_mn, g=g,
+               what="auto %s a_mn%d b_mn%d ATOMIC" % (shape, a_mn, b_mn))
 
 
 def test_reserved_sms_shrink_persistent_grids_not_results():
@@ -76,26 +72,21 @@ def test_reserved_sms_shrink_persistent_grids_not_results():
 
 # ---------------------------------------------------------------------------------------------------------
 def test_gemm_fused_epilogues():
-    M, N, K = 384, 3072, 768
-    g = torch.Generator(device=DEV).manual_seed(2)
-    A = _bf(torch.randn(M, K, device=DEV, generator=g) * 0.3)
-    B = _bf(torch.randn(N, K, device=DEV, generator=g) * 0.05)
-    bias = torch.randn(N, device=DEV, generator=g) * 0.1
-    pre_ref = A.float() @ B.float().t() + bias
-    pre = torch.empty(M, N, device=DEV, dtype=torch.bfloat16)
-    h = torch.empty_like(pre)
-    ops.gemm(A, B, M, N, K, h, epi=ops.EPI_GELU, bias=bias, aux_out=pre)
-    gelu_ref = pre_ref * 0.5 * (1 + torch.erf(pre_ref / math.sqrt(2)))
-    assert (pre.float() - pre_ref).abs().max() <= 2e-2
-    assert (h.float() - gelu_ref).abs().max() <= 2e-2
-    # gelu backward epilogue: out = acc * gelu'(aux)
-    dy = _bf(torch.randn(M, K, device=DEV, generator=g) * 0.3)
-    out = torch.empty(M, N, device=DEV, dtype=torch.bfloat16)
-    ops.gemm(dy, B, M, N, K, out, epi=ops.EPI_GELU_BWD, aux_in=pre)
-    x = pre.float()
-    gp = 0.5 * (1 + torch.erf(x / math.sqrt(2))) + x * torch.exp(-0.5 * x * x) / math.sqrt(2 * math.pi)
-    ref = (dy.float() @ B.float().t()) * gp
-    assert (out.float() - ref).abs().max() <= 3e-2 * max(1.0, float(ref.abs().max()))
+    """each of the six epilogues on a tail shape with strided out / aux_in / aux_out (ld > N, sentinel padding, rows
+    past M untouched), with alpha = 1 and a bias, then alpha != 1 and bias=None (GELU and GELU-backward keep alpha = 1:
+    their callers never scale).  The GELU epilogues run at the FFN's scale (pre-activations of order 1, where gelu' is
+    far from 0 and 1)."""
+    M, N, K = 300, 520, 760                         # 300 % 128 = 44, 520 % 256 = 8, 760 % 64 = 56
+    for epi in (ops.EPI_BIAS, ops.EPI_GELU, ops.EPI_GELU_BWD, ops.EPI_ADD, ops.EPI_F32, ops.EPI_ATOMIC):
+        for alpha, with_bias in ((1.0, True), (-0.75, False)):
+            if epi in (ops.EPI_GELU, ops.EPI_GELU_BWD):
+                alpha = 1.0
+            g = torch.Generator(device=DEV).manual_seed(2 + epi)
+            A, B = gc.bf_randn((M, K), 0.3, g), gc.bf_randn((N, K), 0.05, g)
+            for a_mn, b_mn in ((0, 0), (0, 1), (1, 1)):
+                gc.run_epi(epi, A, B, gc.store(A, a_mn, 8), gc.store(B, b_mn, 8), a_mn, b_mn, alpha=alpha,
+                           with_bias=with_bias, ldo=N + 8, ld_aux=N + 24, g=g,
+                           what="epi%d alpha%g bias%d a_mn%d b_mn%d" % (epi, alpha, with_bias, a_mn, b_mn))
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -172,7 +163,8 @@ def _attn_ref(q, k, v, add_mask):
 
 @pytest.mark.parametrize("n_seq,Sq,Sk,causal", [(3, 48, 48, False), (2, 96, 96, False), (2, 20, 52, False),
                                                  (2, 128, 128, True), (1, 224, 224, False), (2, 33, 33, True),
-                                                 (3, 1, 96, False)])  # Sq = 1: first-token-only last cross layer
+                                                 (3, 1, 96, False),   # Sq = 1: first-token-only last cross layer
+                                                 (1024, 96, 96, False), (1024, 1, 96, False)])  # all-pairs cross encoder
 def test_attention_fwd_bwd(n_seq, Sq, Sk, causal):
     H, h = 768, 12
     g = torch.Generator(device=DEV).manual_seed(Sq + Sk)
@@ -216,6 +208,15 @@ def test_attention_fwd_bwd(n_seq, Sq, Sk, causal):
         # is relative to the summed magnitudes, not to the sum.)
         tol = got.float().abs().sum(0) * 2.0 ** -8 + 1e-3
         assert bool(((dbias[n] - 1.0 - got.float().sum(0)).abs() <= tol).all())
+    # the bias gradients are per-sequence partial rows added in order: the same bits on every launch
+    def again():
+        dq_, dkv_ = torch.empty_like(q), torch.empty_like(kv)
+        db_ = torch.ones(3, H, device=DEV)
+        ops.attention_bwd(q, k, v, o, lse, d_o, dq_, dkv_[:, :H], dkv_[:, H:], n_seq, Sq, Sk, spec,
+                          dbias=(db_[0], db_[1], db_[2]))
+        return [dq_, dkv_, db_]
+    for a, b in zip((dq, dkv, dbias), _same_bits(again, launches=2)):
+        assert torch.equal(a, b)
     # the same launch without the bias pointers leaves everything else unchanged
     dq2, dkv2 = torch.empty_like(q), torch.empty_like(kv)
     ops.attention_bwd(q, k, v, o, lse, d_o, dq2, dkv2[:, :H], dkv2[:, H:], n_seq, Sq, Sk, spec)
@@ -320,7 +321,7 @@ def test_fused_qkv_attention_fwd_matches_unfused_and_fp32(n_seq, S, causal):
 @pytest.mark.parametrize("n_seq,S,causal,p", [(3, 48, False, 0.0), (2, 96, False, 0.0), (2, 128, True, 0.0),
                                               (5, 32, False, 0.0), (9, 16, True, 0.0), (1, 112, False, 0.0),
                                               (40, 96, False, 0.0), (3, 48, False, 0.25), (2, 128, False, 0.25),
-                                              (301, 48, False, 0.1)])
+                                              (301, 48, False, 0.1), (1024, 96, False, 0.0), (1024, 96, False, 0.1)])
 def test_fused_attention_bwd_matches_fp32_and_unfused_backward(n_seq, S, causal, p):
     """wgmma attention backward: (p = 0) against fp32 autograd of the same op, and (any p) against the mma.sync
     backward kernel regenerating the same row-major dropout mask; bias-gradient column sums included."""
@@ -347,6 +348,13 @@ def test_fused_attention_bwd_matches_fp32_and_unfused_backward(n_seq, S, causal,
     assert rel <= 1e-2, rel
     tol = dqkv.float().abs().sum(0) * 2.0 ** -7 + 2e-3
     assert bool(((dbias - 1.0 - dqkv.float().sum(0)).abs() <= tol).all())
+
+    def again():
+        dq_, db_ = torch.empty_like(qkv), torch.ones(3 * H, device=DEV)
+        ops.fused_attention_bwd(qkv, o, lse, d_o, dq_, n_seq, S, spec, p=p, seed=RNG.data_ptr(), stream=7, dbias=db_)
+        return [dq_, db_]
+    for a, b in zip((dqkv, dbias), _same_bits(again, launches=2)):
+        assert torch.equal(a, b)
     if p == 0.0:
         # (b) fp32 autograd
         def heads(t):
@@ -366,16 +374,31 @@ def test_fused_attention_bwd_matches_fp32_and_unfused_backward(n_seq, S, causal,
             assert (got - want).abs().max() <= 4e-2 * max(1.0, float(want.abs().max())), n
 
 
-def test_fused_qkv_attention_all_pairs_masks():
-    Na, Nb, W, F, H = 3, 4, 16, 32, 768
+def _all_pairs_fused_case(Na, Nb, W, F):
+    H = 768
     S = W + F
     x, w, b, _ = _fused_inputs(Na * Nb, S, 11)
-    ma = (torch.arange(W, device=DEV).unsqueeze(0) < torch.tensor([5, 16, 1], device=DEV).unsqueeze(1)).long()
-    mb = (torch.arange(F, device=DEV).unsqueeze(0) < torch.tensor([3, 32, 9, 20], device=DEV).unsqueeze(1)).long()
-    o, _, _ = ops.fused_qkv_attention_fwd(x, w, b, Na * Nb, S, ops.MaskSpec(ma, mb, all_pairs=True))
+    g = torch.Generator().manual_seed(Na + W)
+    ma = (torch.arange(W).unsqueeze(0) < torch.randint(1, W + 1, (Na,), generator=g).unsqueeze(1)).long().to(DEV)
+    mb = (torch.arange(F).unsqueeze(0) < torch.randint(1, F + 1, (Nb,), generator=g).unsqueeze(1)).long().to(DEV)
     full = torch.cat([ma.unsqueeze(1).expand(Na, Nb, W), mb.unsqueeze(0).expand(Na, Nb, F)], -1).reshape(Na * Nb, S)
-    o2, _, _ = ops.fused_qkv_attention_fwd(x, w, b, Na * Nb, S, ops.MaskSpec(full))
-    assert torch.equal(o, o2)
+    d_o = _bf(torch.randn(Na * Nb * S, H, device=DEV, generator=torch.Generator(device=DEV).manual_seed(3)))
+    outs = []
+    for spec in (ops.MaskSpec(ma, mb, all_pairs=True), ops.MaskSpec(full)):
+        o, lse, qkv = ops.fused_qkv_attention_fwd(x, w, b, Na * Nb, S, spec)
+        dqkv = torch.empty_like(qkv)
+        dbias = torch.zeros(3 * H, device=DEV)
+        ops.fused_attention_bwd(qkv, o, lse, d_o, dqkv, Na * Nb, S, spec, dbias=dbias)
+        outs.append((o, lse, dqkv, dbias))
+    for a, c in zip(*outs):
+        assert torch.equal(a, c)
+
+
+def test_fused_qkv_attention_all_pairs_masks():
+    """all-pairs masks (text mask i, video mask j for pair (i, j)) give the bits of the same masks expanded to one full
+    mask, forward and backward (bias gradient included); also at the cross encoder's 32 x 32 pairs of 48 + 48 tokens"""
+    _all_pairs_fused_case(3, 4, 16, 32)
+    _all_pairs_fused_case(32, 32, 48, 48)
 
 
 @pytest.mark.parametrize("n_seq,S", [(3, 48), (2, 96), (2, 128)])
@@ -552,3 +575,238 @@ def test_bert_adam_matches_reference_formula():
             p -= lr * sched * (m[i] / (v[i].sqrt() + 1e-6) + wd * p)
         for p, q in zip(params, ref_p):
             torch.testing.assert_close(p.detach(), q, rtol=1e-4, atol=1e-6)
+
+
+# ---------------------------------------------------------------------------------------------------------
+# ordered reductions: fp64 references at production and edge shapes, and bit-for-bit repeatability.  Every cross-block
+# sum of these kernels goes through per-block partial rows added in block order (csrc/api.cu partials_reduce) or per-key
+# row-ordered sums (csrc/embed.cu keyed_rows_sum_kernel), so the same launch gives the same bits, with or without SMs
+# reserved for a concurrent collective.
+# ---------------------------------------------------------------------------------------------------------
+U32 = 2.0 ** -24
+
+
+def _same_bits(run, launches=3):
+    """run() -> list of tensors: identical bits over `launches` launches and with 40 SMs reserved"""
+    base = [t.clone() for t in run()]
+    torch.cuda.synchronize()
+    for i in range(launches - 1):
+        for a, b in zip(base, run()):
+            assert torch.equal(a, b), "launch %d differs" % (i + 1)
+    rt.reserve_sms(40)
+    try:
+        for a, b in zip(base, run()):
+            assert torch.equal(a, b), "differs with 40 SMs reserved"
+    finally:
+        rt.reserve_sms(0)
+    return base
+
+
+def _within(got, ref, bound, what):
+    err = (got.double() - ref).abs()
+    ok = err <= bound
+    if not bool(ok.all()):
+        i = tuple(int(v) for v in (~ok).nonzero()[0])
+        raise AssertionError("%s: %d elements outside the bound; first %s: got %r ref %r bound %r"
+                             % (what, int((~ok).sum()), i, float(got[i]), float(ref[i]), float(bound[i])))
+
+
+def _ln_bwd64(z, d, gamma):
+    """fp64 LayerNorm backward of rows z [R, C] for upstream d: (xhat, dz, e_xhat, e_dz) where e_* bound the fp32
+    kernels' per-element error (C-term row sums for the mean, variance and the two backward row sums)"""
+    C = z.shape[1]
+    mean = z.mean(1, keepdim=True)
+    rstd = 1.0 / torch.sqrt(((z - mean) ** 2).mean(1, keepdim=True) + 1e-12)
+    xhat = (z - mean) * rstd
+    g = d * gamma.double()
+    gx = (g * xhat).mean(1, keepdim=True)
+    dz = rstd * (g - g.mean(1, keepdim=True) - xhat * gx)
+    k = (C + 16) * U32
+    e_xhat = k * (rstd * (z.abs().mean(1, keepdim=True) + z.abs()) + xhat.abs())
+    e_dz = 2 * k * (rstd * (g.abs() + g.abs().mean(1, keepdim=True) + (1 + xhat.abs()) * (g * xhat).abs().mean(1, keepdim=True))
+                    + dz.abs()) + rstd * (g * xhat).abs().mean(1, keepdim=True) * e_xhat
+    return xhat, dz, e_xhat, e_dz
+
+
+@pytest.mark.parametrize("rows,cols", [(1536, 768), (98304, 3072), (1, 768), (1000, 771)])
+def test_colsum_fp64_and_repeatable(rows, cols):
+    """bias column sums (b1 of every FFN, the vocab bias): odd cols take the scalar loads"""
+    g = torch.Generator(device=DEV).manual_seed(rows + cols)
+    x = _bf(torch.randn(rows, cols, device=DEV, generator=g))
+
+    def run():
+        out = torch.ones(cols, device=DEV)          # accumulated into
+        ops.colsum(x, out)
+        return [out]
+    got = _same_bits(run)[0]
+    xd = x.double()
+    _within(got - 1.0, xd.sum(0), (rows + 2) * U32 * xd.abs().sum(0) + 2 * U32, "colsum")
+
+
+@pytest.mark.parametrize("rows,cols,p", [(1, 768, 0.0), (37, 1024, 0.0), (1536, 768, 0.1), (98304, 768, 0.1)])
+def test_layernorm_bwd_param_grads_fp64_and_repeatable(rows, cols, p):
+    """dgamma / dbeta / dbias (the column sums of the residual LayerNorm backward, dropout mode 1 as every block runs
+    it); 98304 rows is the all-pairs cross encoder, where each CTA walks many rows into its partial"""
+    g = torch.Generator(device=DEV).manual_seed(rows + cols)
+    x = _bf(torch.randn(rows, cols, device=DEV, generator=g))
+    res = _bf(torch.randn(rows, cols, device=DEV, generator=g))
+    gamma = 1 + 0.1 * torch.randn(cols, device=DEV, generator=g)
+    beta = 0.1 * torch.randn(cols, device=DEV, generator=g)
+    dy = _bf(torch.randn(rows, cols, device=DEV, generator=g))
+    dy2 = _bf(torch.randn(rows, cols, device=DEV, generator=g))
+    _, mean, rstd = ops.layernorm_fwd(x, res, gamma, beta, p=p, mode=1, seed=RNG.data_ptr(), stream=5)
+
+    def run():
+        dx, dxd, dgamma, dbeta, dbias = ops.layernorm_bwd(dy, dy2, x, res, gamma, mean, rstd, p=p, mode=1,
+                                                          seed=RNG.data_ptr(), stream=5)
+        return [dx, dxd, dgamma, dbeta, dbias]
+    dx, dxd, dgamma, dbeta, dbias = _same_bits(run)
+    scale = float(torch.tensor(1.0 / (1.0 - p), dtype=torch.float32)) if p > 0 else 1.0
+    keep = (dxd != 0).double() if p > 0 else torch.ones(rows, cols, dtype=torch.float64, device=DEV)
+    if p > 0:
+        assert abs(float(keep.mean()) - (1 - p)) < 0.02
+    z = x.double() * keep * scale + res.double()
+    d = dy.double() + dy2.double()
+    xhat, dz, e_xhat, e_dz = _ln_bwd64(z, d, gamma)
+    n = rows + 2
+    _within(dbeta, d.sum(0), n * U32 * d.abs().sum(0) + 1e-30, "dbeta")
+    _within(dgamma, (d * xhat).sum(0), n * U32 * (d * xhat).abs().sum(0) + (d.abs() * e_xhat).sum(0), "dgamma")
+    kd = keep * scale
+    _within(dbias, (dz * kd).sum(0), n * U32 * (dz * kd).abs().sum(0) + (e_dz * kd).sum(0), "dbias")
+    _within(dx, dz, e_dz + 2.0 ** -8 * dz.abs(), "dx")
+
+
+def _embed_holder():
+    class Holder(torch.nn.Module):
+        pass
+    return Holder()
+
+
+def test_embed_text_table_grads_fp64_and_repeatable():
+    """the text embedding backward of the FT-Align step: 32 x 48 rows, most of them [PAD] (id 0, hundreds of rows of
+    one key spread over many CTAs), every sequence starting with [CLS], every position 32 times.  Word / position /
+    type tables and gamma / beta against fp64 index_add_; with dropout, the same bits on every launch."""
+    n, S, H, V = 32, 48, 768, 30522
+    g = torch.Generator(device=DEV).manual_seed(17)
+    word = 0.05 * torch.randn(V, H, device=DEV, generator=g)
+    pos = 0.05 * torch.randn(512, H, device=DEV, generator=g)
+    typ = 0.05 * torch.randn(2, H, device=DEV, generator=g)
+    gamma = 1 + 0.1 * torch.randn(H, device=DEV, generator=g)
+    beta = 0.1 * torch.randn(H, device=DEV, generator=g)
+    lens = torch.randint(4, 40, (n,), generator=torch.Generator().manual_seed(3))
+    ids = torch.zeros(n, S, dtype=torch.long)
+    for i, L in enumerate(lens.tolist()):
+        ids[i, 0] = 101                                                     # [CLS]
+        ids[i, 1:L - 1] = torch.randint(1000, 3000, (L - 2,), generator=torch.Generator().manual_seed(i))
+        ids[i, L - 1] = 102                                                 # [SEP]
+    ids = ids.to(DEV)
+    tids = torch.zeros(n, S, dtype=torch.long, device=DEV)
+    tids[:, S // 2:] = 1
+    dy = _bf(torch.randn(n * S, H, device=DEV, generator=g))
+    holder = _embed_holder()
+    dev = torch.device("cuda", torch.cuda.current_device())
+
+    def run(p):
+        ws = [t.clone().requires_grad_() for t in (word, pos, typ, gamma, beta)]
+        with rt.use_model(holder, dev) as arena:
+            arena.stream_counter = 0
+            arena.rng_state[1] = 3                                          # same dropout epoch every launch
+            y = ops.EmbedTextFn.apply(ids, tids, *ws, p, True)
+            y.backward(dy)
+        return [t.grad for t in ws]
+    dword, dpos, dtyp, dgamma, dbeta = _same_bits(lambda: run(0.0))
+    _same_bits(lambda: run(0.1), launches=2)
+    # fp64 reference
+    flat_ids, s_idx, t_idx = ids.reshape(-1), torch.arange(S, device=DEV).repeat(n), tids.reshape(-1)
+    z = word.double()[flat_ids] + pos.double()[s_idx] + typ.double()[t_idx]
+    d = dy.double()
+    xhat, dz, e_xhat, e_dz = _ln_bwd64(z, d, gamma)
+    for got, idx, rows_of, name in ((dword, flat_ids, V, "word"), (dpos, s_idx, 512, "position"),
+                                    (dtyp, t_idx, 2, "type")):
+        ref = torch.zeros(rows_of, H, dtype=torch.float64, device=DEV).index_add_(0, idx, dz)
+        cnt = torch.zeros(rows_of, dtype=torch.float64, device=DEV).index_add_(0, idx, torch.ones_like(idx, dtype=torch.float64))
+        mag = torch.zeros_like(ref).index_add_(0, idx, dz.abs())
+        err = torch.zeros_like(ref).index_add_(0, idx, e_dz)
+        _within(got, ref, (cnt.unsqueeze(1) + 2) * U32 * mag + err + 1e-30, name)
+    assert int((flat_ids == 0).sum()) > 500                              # [PAD] rows span many CTAs
+    nrow = n * S + 2
+    _within(dbeta, d.sum(0), nrow * U32 * d.abs().sum(0), "beta")
+    _within(dgamma, (d * xhat).sum(0), nrow * U32 * (d * xhat).abs().sum(0) + (d.abs() * e_xhat).sum(0), "gamma")
+
+
+def test_embed_src_all_pairs_grads_fp64_and_repeatable():
+    """the cross embedding of the all-pairs FT-Align step: Na = Nb = 32, W = F = 48 (98304 rows).  Position, type,
+    gamma, beta and the source gradients da / db (each summed over its 32-way fan-out) against fp64."""
+    Na, Nb, W, F, H = 32, 32, 48, 48, 768
+    S = W + F
+    g = torch.Generator(device=DEV).manual_seed(23)
+    a = _bf(torch.randn(Na * W, H, device=DEV, generator=g))
+    b = _bf(torch.randn(Nb * F, H, device=DEV, generator=g))
+    pos = 0.05 * torch.randn(512, H, device=DEV, generator=g)
+    typ = 0.05 * torch.randn(2, H, device=DEV, generator=g)
+    gamma = 1 + 0.1 * torch.randn(H, device=DEV, generator=g)
+    beta = 0.1 * torch.randn(H, device=DEV, generator=g)
+    dy = _bf(torch.randn(Na * Nb * S, H, device=DEV, generator=g))
+    holder = _embed_holder()
+    dev = torch.device("cuda", torch.cuda.current_device())
+
+    def run():
+        av, bv = a.clone().requires_grad_(), b.clone().requires_grad_()
+        ws = [t.clone().requires_grad_() for t in (pos, typ, gamma, beta)]
+        with rt.use_model(holder, dev):
+            y = ops.EmbedSrcFn.apply(av, bv, Na, W, Nb, F, True, *ws, 0.0, True)
+            y.backward(dy)
+        return [av.grad, bv.grad] + [t.grad for t in ws]
+    da, db, dpos, dtyp, dgamma, dbeta = _same_bits(run)
+    cat = torch.cat([a.double().view(Na, 1, W, H).expand(Na, Nb, W, H), b.double().view(1, Nb, F, H).expand(Na, Nb, F, H)],
+                    2)
+    types = torch.cat([torch.zeros(W, dtype=torch.long), torch.ones(F, dtype=torch.long)]).to(DEV)
+    z = (cat + pos.double()[:S] + typ.double()[types]).reshape(-1, H)
+    del cat
+    d = dy.double()
+    xhat, dz, e_xhat, e_dz = _ln_bwd64(z, d, gamma)
+    dz4, e4, m4 = dz.view(Na, Nb, S, H), e_dz.view(Na, Nb, S, H), dz.abs().view(Na, Nb, S, H)
+    R = Na * Nb + 2
+    _within(dpos[:S], dz4.sum((0, 1)), R * U32 * m4.sum((0, 1)) + e4.sum((0, 1)), "position")
+    assert bool((dpos[S:] == 0).all())
+    for t, sl in ((0, slice(0, W)), (1, slice(W, S))):
+        _within(dtyp[t], dz4[:, :, sl].sum((0, 1, 2)), (R * S) * U32 * m4[:, :, sl].sum((0, 1, 2))
+                + e4[:, :, sl].sum((0, 1, 2)), "type %d" % t)
+    ref_a = dz4[:, :, :W].sum(1).reshape(-1, H)
+    _within(da, ref_a, (Nb + 2) * U32 * m4[:, :, :W].sum(1).reshape(-1, H) + e4[:, :, :W].sum(1).reshape(-1, H)
+            + 2.0 ** -8 * ref_a.abs(), "da")
+    ref_b = dz4[:, :, W:].sum(0).reshape(-1, H)
+    _within(db, ref_b, (Na + 2) * U32 * m4[:, :, W:].sum(0).reshape(-1, H) + e4[:, :, W:].sum(0).reshape(-1, H)
+            + 2.0 ** -8 * ref_b.abs(), "db")
+    nrow = z.shape[0] + 2
+    _within(dbeta, d.sum(0), nrow * U32 * d.abs().sum(0), "beta")
+    _within(dgamma, (d * xhat).sum(0), nrow * U32 * (d * xhat).abs().sum(0) + (d.abs() * e_xhat).sum(0), "gamma")
+
+
+@pytest.mark.parametrize("N", [1024, 37])
+def test_pooler_sim_bwd_param_grads_fp64_and_repeatable(N):
+    """similarity head dw / db over the N = 32 x 32 pooled pairs, and N not a multiple of the 16 rows per CTA"""
+    H = 768
+    g = torch.Generator(device=DEV).manual_seed(N)
+    u = _bf(torch.randn(N, H, device=DEV, generator=g))
+    w = 0.05 * torch.randn(H, device=DEV, generator=g)
+    dout = torch.randn(N, device=DEV, generator=g)
+    from univl_b200.runtime import call
+
+    def run():
+        du = torch.empty(N, H, device=DEV, dtype=torch.bfloat16)
+        dw, db = torch.ones(H, device=DEV), torch.ones(1, device=DEV)        # accumulated into
+        call("univl_pooler_sim_bwd", u.data_ptr(), w.data_ptr(), dout.data_ptr(), du.data_ptr(), dw.data_ptr(),
+             db.data_ptr(), N, H)
+        return [du, dw, db]
+    du, dw, db = _same_bits(run)
+    th = torch.tanh(u.double())
+    d = dout.double()
+    # tanhf compiles to MUFU.TANH under --use_fast_math: relative error below 2^-10.9
+    th_err = 2.0 ** -10 * th.abs() + 2.0 ** -20
+    terms = (d.unsqueeze(1) * th).abs().sum(0)
+    _within(dw - 1.0, (d.unsqueeze(1) * th).sum(0), (N + 2) * U32 * terms + (d.abs().unsqueeze(1) * th_err).sum(0), "dw")
+    _within(db - 1.0, d.sum().view(1), (N + 2) * U32 * d.abs().sum().view(1), "db")
+    dw_ = (d.unsqueeze(1) * w.double()).abs()
+    ref_du = d.unsqueeze(1) * w.double() * (1 - th * th)
+    _within(du, ref_du, 2.0 ** -8 * ref_du.abs() + dw_ * (2 * th.abs() * th_err + 4 * U32), "du")

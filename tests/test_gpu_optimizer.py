@@ -166,3 +166,35 @@ def test_bf16_gradient_payload_equals_fp32_of_the_same_values():
     with pytest.raises(ValueError):
         opt.grad_payload = torch.zeros(3, device=DEV, dtype=torch.bfloat16)
         opt.step()
+
+
+def test_fused_step_is_bitwise_repeatable_over_many_chunks():
+    """the gradient norms (per-tensor and global clip) are per-chunk partial sums (adam_sumsq) added in chunk order
+    (adam_tensor_sums): two optimizers on identical parameters and gradients end with identical bits in parameters and
+    moments, over a flat buffer of 2.4M elements = 39 chunks of 64K, one tensor spanning 23 of them — also with SMs
+    reserved for a concurrent collective"""
+    from univl_b200 import runtime as rt
+    from univl_b200.optim import FusedBertAdam
+    shapes = [(1500, 1000), (300001,), (5, 7), (768, 768), (3,)]
+
+    def run(reserve):
+        torch.manual_seed(4)
+        ps = [torch.nn.Parameter(torch.randn(s, device=DEV) * 0.1) for s in shapes]
+        opt = FusedBertAdam([{"params": ps[:3], "weight_decay": 0.01}, {"params": ps[3:], "weight_decay": 0.0}],
+                            lr=1e-3, warmup=0.1, t_total=100, max_grad_norm=1.0, global_clip_norm=1.0)
+        rt.reserve_sms(reserve)
+        try:
+            for t in range(2):
+                gen = torch.Generator(device=DEV).manual_seed(30 + t)
+                for p in ps:
+                    p.grad = torch.randn(p.shape, device=DEV, generator=gen) * (3.0 if t == 0 else 0.2)
+                opt.step()
+            torch.cuda.synchronize()
+        finally:
+            rt.reserve_sms(0)
+        return [opt.p.clone(), opt.m.clone(), opt.v.clone()]
+    base = run(0)
+    assert base[0].numel() > 36 * 65536
+    for reserve in (0, 40):
+        for a, b in zip(base, run(reserve)):
+            assert torch.equal(a, b), reserve

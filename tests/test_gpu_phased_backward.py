@@ -51,8 +51,12 @@ def test_phases_reproduce_single_backward(mode, cuts):
 
     l0, g0 = flat_grads(None)
     l1, g1 = flat_grads(cuts)
-    # (the cross-entropy losses sum their rows with fp32 atomics: the last bits depend on the arrival order)
-    assert abs(l0 - l1) <= 1e-6 * max(1.0, abs(l0)), (l0, l1)
     assert float(g0.norm()) > 0
-    # same kernels on the same inputs; only the order of fp32 atomic accumulations may differ
-    torch.testing.assert_close(g1, g0, rtol=1e-4, atol=1e-5 * float(g0.abs().max()))
+    # same kernels on the same inputs, and every gradient sum is added in a fixed order: the same bits
+    assert torch.equal(g1, g0)
+    if mode == "ft_align":
+        assert l0 == l1
+    else:
+        # the vocab / frame cross-entropy adds its rows' losses with fp32 atomics (xent_fwd_kernel's loss_sum), so the
+        # loss's last bits depend on the arrival order; its gradient reads only the exact scored-row count
+        assert abs(l0 - l1) <= 1e-6 * max(1.0, abs(l0)), (l0, l1)
