@@ -87,8 +87,12 @@ int univl_embed_src_bwd(const void* dy, const void* a, const void* b, const floa
                         int H, float p_drop, const unsigned long long* rng_state, unsigned long long stream_id, void* stream);
 
 /* ---- attention core (module_bert.py:176-196; module_decoder.py:225-245, mask :385-396) -------------------------
- * ctx = dropout(softmax(Q K^T * scale + mask)) V per (sequence, head), head dim 64, S <= 256.
- * mask = -10000 * (key padded [or key > query if causal]); key padding = concat(mask_a[i,:Wa], mask_b[j,:Fb]). */
+ * ctx = dropout(softmax(Q K^T * scale + mask)) V per (sequence, head), head dim 64.
+ * mask = -10000 * (key padded [or key > query if causal]); key padding = concat(mask_a[i,:Wa], mask_b[j,:Fb]).
+ * univl_attention_fwd / _bwd take Sq, Sk <= 256 (whole K/V of a head in shared memory); univl_attention_long_fwd /
+ * _bwd take the same arguments for 0 < Sq, Sk <= 1024 with 12 heads (key-tiled; rng_layout must be 0), which covers
+ * the model's position tables: text, visual and decoder <= 512 tokens, cross encoder <= 1024.  Both draw the same
+ * dropout mask for the same (seed, stream, sequence, head, query, key). */
 int univl_attention_fwd(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv,
                         void* o, long long ldo, float* lse, const long long* mask_a, const long long* mask_b, int Wa,
                         int Fb, int Nb, int all_pairs, int n_seq, int heads, int Sq, int Sk, int causal, float scale,
@@ -99,6 +103,18 @@ int univl_attention_bwd(const void* q, long long ldq, const void* k, long long l
                         const long long* mask_b, int Wa, int Fb, int Nb, int all_pairs, int n_seq, int heads, int Sq,
                         int Sk, int causal, float scale, float p_drop, const unsigned long long* rng_state,
                         unsigned long long stream_id, int rng_layout, float* dbq, float* dbk, float* dbv, void* stream);
+int univl_attention_long_fwd(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv,
+                             void* o, long long ldo, float* lse, const long long* mask_a, const long long* mask_b,
+                             int Wa, int Fb, int Nb, int all_pairs, int n_seq, int heads, int Sq, int Sk, int causal,
+                             float scale, float p_drop, const unsigned long long* rng_state,
+                             unsigned long long stream_id, void* stream);
+int univl_attention_long_bwd(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv,
+                             const void* o, long long ldo, const float* lse, const void* d_o, long long lddo, void* dq,
+                             long long lddq, void* dk, long long lddk, void* dv, long long lddv,
+                             const long long* mask_a, const long long* mask_b, int Wa, int Fb, int Nb, int all_pairs,
+                             int n_seq, int heads, int Sq, int Sk, int causal, float scale, float p_drop,
+                             const unsigned long long* rng_state, unsigned long long stream_id, int rng_layout,
+                             float* dbq, float* dbk, float* dbv, void* stream);
 /* ---- fused QKV projection + self-attention, forward (wgmma / TMA; module_bert.py:171-197 as ONE kernel) --------------
  * ctx[T,H] = merge_heads(dropout(softmax((x Wq^T + bq)(x Wk^T + bk)^T * scale + mask)) (x Wv^T + bv)), T = n_seq * S,
  * H = heads * 64 = 768.  wqkv: bf16 [3H, H] (query | key | value rows), bias fp32 [3H].  The [T,3H] projections and the

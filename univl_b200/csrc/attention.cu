@@ -14,132 +14,12 @@
 // Dropout masks are Philox(seed, stream, element) and regenerated identically in every pass.
 #include <stdlib.h>
 
-#include "common.cuh"
+#include "attention_common.cuh"
 
 namespace univl {
 
-constexpr int HD = 64;        // head dim
-constexpr int LDS = 72;       // smem row stride in elements (144 B: conflict-free ldmatrix)
 constexpr int ATT_FWD_WARPS = 8;   // upper bounds; the launch uses one warp per 16-row task up to these
 constexpr int ATT_BWD_WARPS = 12;
-
-struct AttnParams {
-  const bf16 *q, *k, *v;
-  long long ldq, ldk, ldv;
-  bf16* o;
-  long long ldo;
-  float* lse;  // [n_seq, heads, Sq]
-  const long long* mask_a;  // [Na, Wa]
-  const long long* mask_b;  // [Nb, Fb] or null
-  int Wa, Fb, Nb, all_pairs;
-  int n_seq, heads, Sq, Sk, causal;
-  float scale;
-  uint32_t drop_threshold;
-  float drop_scale;
-  int drop_on;
-  uint64_t seed, stream;
-  const unsigned long long* rng;  // device {seed, epoch}, resolved at kernel entry (graph-replayable)
-  // backward only
-  const bf16* d_o;
-  long long lddo;
-  bf16 *dq, *dk, *dv;
-  long long lddq, lddk, lddv;
-  int share_tiles;  // backward: 1 = query-major pass shares P_drop / dS with the key-major pass through smem
-  int rng_rowmajor; // backward: dropout layout of the fused QKV+attention forward kernel (fused_attn.cu), see tile_rng_rowmajor
-  float *dbq, *dbk, *dbv;  // backward, optional: projection-bias gradients += column sums of dq / dk / dv  [heads*64]
-};
-
-__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void ldsm_x4_t(uint32_t addr, uint32_t (&r)[4]) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem)), "l"(gmem) : "memory");
-}
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
-
-// copy `rows` x 64 bf16 (head slice) into smem [rows16][LDS], zero-filling rows >= rows
-__device__ __forceinline__ void load_head_tile(bf16* dst, const bf16* src, long long ld, int rows, int rows16) {
-  for (int idx = threadIdx.x; idx < rows16 * 8; idx += blockDim.x) {
-    const int r = idx >> 3, c = idx & 7;
-    bf16* d = dst + r * LDS + c * 8;
-    if (r < rows) cp_async16(d, src + (long long)r * ld + c * 8);
-    else *reinterpret_cast<uint4*>(d) = make_uint4(0, 0, 0, 0);
-  }
-}
-
-// additive key mask for this sequence into smem: 0 / -10000 for real keys, -inf for padding beyond Sk
-__device__ __forceinline__ void build_key_mask(float* madd, const AttnParams& p, int seq, int Sk16) {
-  const long long i = p.all_pairs ? seq / p.Nb : seq;
-  const long long j = p.all_pairs ? seq % p.Nb : seq;
-  for (int c = threadIdx.x; c < Sk16; c += blockDim.x) {
-    float m;
-    if (c >= p.Sk) m = -INFINITY;
-    else {
-      long long v = 1;
-      if (p.mask_a != nullptr) {
-        if (c < p.Wa) v = p.mask_a[i * p.Wa + c];
-        else if (p.mask_b != nullptr) v = p.mask_b[j * p.Fb + (c - p.Wa)];
-      }
-      m = v != 0 ? 0.f : -10000.f;
-    }
-    madd[c] = m;
-  }
-}
-
-// A-operand fragments (16 rows x 64 dims) of smem matrix X starting at row r0
-__device__ __forceinline__ void load_a_frags(const bf16* X, int r0, int lane, uint32_t (&a)[4][4]) {
-  const int row = r0 + (lane & 7) + ((lane >> 3) & 1) * 8;
-#pragma unroll
-  for (int kc = 0; kc < 4; ++kc) ldsm_x4(smem_u32(X + row * LDS + kc * 16 + (lane >> 4) * 8), a[kc]);
-}
-
-// C[16 x 16] = A(16 x 64) * Y^T where Y rows n0..n0+15 are the "n" index (keys or queries), contraction over dims
-__device__ __forceinline__ void mma_a_yT(const uint32_t (&a)[4][4], const bf16* Y, int n0, int lane, float (&c)[2][4]) {
-#pragma unroll
-  for (int nb = 0; nb < 2; ++nb)
-#pragma unroll
-    for (int e = 0; e < 4; ++e) c[nb][e] = 0.f;
-  const int row = n0 + (lane & 7) + (lane >> 4) * 8;
-#pragma unroll
-  for (int kc = 0; kc < 4; ++kc) {
-    uint32_t b[4];
-    ldsm_x4(smem_u32(Y + row * LDS + kc * 16 + ((lane >> 3) & 1) * 8), b);
-    mma16816(c[0], a[kc], b[0], b[1]);
-    mma16816(c[1], a[kc], b[2], b[3]);
-  }
-}
-
-// acc[16 x 64] += P(16 x 16, bf16 A-fragments) * Z where Z rows k0..k0+15 are the contraction index
-__device__ __forceinline__ void mma_p_z(const uint32_t (&pa)[4], const bf16* Z, int k0, int lane, float (&acc)[8][4]) {
-  const int row = k0 + (lane & 7) + ((lane >> 3) & 1) * 8;
-#pragma unroll
-  for (int nd = 0; nd < 4; ++nd) {
-    uint32_t b[4];
-    ldsm_x4_t(smem_u32(Z + row * LDS + nd * 16 + (lane >> 4) * 8), b);
-    mma16816(acc[2 * nd], pa, b[0], b[1]);
-    mma16816(acc[2 * nd + 1], pa, b[2], b[3]);
-  }
-}
-
-// Dropout randoms are laid out to match the mma fragment: for the 16 x 16 tile (query block qb, key block kb) the
-// element (i, j) uses 16-bit word w = (j & 1) | ((i >> 3) & 1) << 1 | ((j >> 3) & 1) << 2 of
-// Philox(seed, stream, ((bh * nQb + qb) * nKb + kb) * 32 + lane_f),  lane_f = (i & 7) << 2 | (j & 7) >> 1.
-// In the query-major passes (forward, dQ) lane_f is the thread's own lane and its 8 tile elements are the 8 words of
-// ONE call; the key-major pass (dK/dV) needs two calls per tile.
-__device__ __forceinline__ uint4 tile_rng(const AttnParams& p, long long bh, int qb, int kb, int nQb, int nKb,
-                                          int lane_f) {
-  return philox4x32(p.seed, p.stream, (uint64_t)(((bh * nQb + qb) * (long long)nKb + kb) * 32 + lane_f));
-}
 
 // Row-major dropout layout (written by fused_attn.cu's forward): element (bh, query i, key j) is 16-bit word (j & 7) of
 // Philox(seed, stream, (bh * Sq + i) * (Sk / 8) + j / 8).  In the mma fragment a thread (g, t) holds, of the 16 x 16 tile
@@ -406,23 +286,6 @@ struct BwdSmem {
   int nQ, nK;
 };
 
-// column sums of a 16 x 64 accumulator tile (rows g / g+8 of the fragment layout) into this task's own 64-float slot:
-// butterfly over the 8 row groups (every lane ends up with the totals), then row group nb stores column block nb.  No
-// atomics: the slots are summed over the tasks at the end of the kernel.  (Shared-memory float atomics from four lanes
-// per warp cost 5.8 us per CTA: measured 893 vs 653 us on the cross-encoder shape.)
-__device__ __forceinline__ void tile_colsum(const float (&acc)[8][4], float* slot, int lane) {
-  const int g = lane >> 2, t = lane & 3;
-#pragma unroll
-  for (int nb = 0; nb < 8; ++nb) {
-    float c0 = acc[nb][0] + acc[nb][2], c1 = acc[nb][1] + acc[nb][3];
-#pragma unroll
-    for (int m = 4; m < 32; m <<= 1) {
-      c0 += __shfl_xor_sync(0xffffffffu, c0, m);
-      c1 += __shfl_xor_sync(0xffffffffu, c1, m);
-    }
-    if (g == nb) *reinterpret_cast<float2*>(slot + nb * 8 + 2 * t) = make_float2(c0, c1);
-  }
-}
 template <bool SHARE>
 __device__ __forceinline__ void bwd_dq_task(const AttnParams& p, const BwdSmem& sm, int task, int lane, int seq, int h,
                                             long long bh, int Sq16, int Sk16) {
@@ -732,32 +595,6 @@ attention_bwd_kernel(const AttnParams p_in) {
   }
 }
 
-static int fill_common(AttnParams& p, const void* q, long long ldq, const void* k, long long ldk, const void* v,
-                       long long ldv, const long long* mask_a, const long long* mask_b, int Wa, int Fb, int Nb,
-                       int all_pairs, int n_seq, int heads, int Sq, int Sk, int causal, float scale, float p_drop,
-                       const unsigned long long* rng_state, unsigned long long stream_id) {
-  UNIVL_CHECK_ARG(q && k && v, "attention: null q/k/v");
-  UNIVL_CHECK_ARG(n_seq >= 0 && heads > 0 && Sq > 0 && Sk > 0 && Sq <= 256 && Sk <= 256,
-                  "attention: unsupported shape n_seq=%d heads=%d Sq=%d Sk=%d (S <= 256)", n_seq, heads, Sq, Sk);
-  UNIVL_CHECK_ARG((ldq % 8) == 0 && (ldk % 8) == 0 && (ldv % 8) == 0, "attention: row strides must be multiples of 8");
-  UNIVL_CHECK_ARG(((uintptr_t)q & 15) == 0 && ((uintptr_t)k & 15) == 0 && ((uintptr_t)v & 15) == 0,
-                  "attention: q/k/v must be 16-byte aligned");
-  UNIVL_CHECK_ARG(mask_a == nullptr || Wa + Fb == Sk, "attention: mask parts (%d + %d) must cover Sk=%d", Wa, Fb, Sk);
-  UNIVL_CHECK_ARG(!(Fb > 0 && mask_a != nullptr && mask_b == nullptr), "attention: missing second mask part");
-  UNIVL_CHECK_ARG(!all_pairs || Nb > 0, "attention: all_pairs needs Nb > 0");
-  UNIVL_CHECK_ARG(p_drop >= 0.f && p_drop < 1.f, "attention: bad dropout probability");
-  p.q = (const bf16*)q; p.k = (const bf16*)k; p.v = (const bf16*)v;
-  p.ldq = ldq; p.ldk = ldk; p.ldv = ldv;
-  p.mask_a = mask_a; p.mask_b = mask_b; p.Wa = Wa; p.Fb = Fb; p.Nb = Nb > 0 ? Nb : 1; p.all_pairs = all_pairs;
-  p.n_seq = n_seq; p.heads = heads; p.Sq = Sq; p.Sk = Sk; p.causal = causal; p.scale = scale;
-  p.drop_on = p_drop > 0.f;
-  p.drop_threshold = dropout_threshold16(p_drop);
-  p.drop_scale = p_drop > 0.f ? 1.0f / (1.0f - p_drop) : 1.0f;
-  UNIVL_CHECK_ARG(p_drop == 0.f || rng_state != nullptr, "attention: dropout needs rng_state");
-  p.seed = 0; p.stream = stream_id; p.rng = rng_state;
-  return UNIVL_OK;
-}
-
 }  // namespace univl
 
 using namespace univl;
@@ -772,7 +609,7 @@ extern "C" int univl_attention_fwd(const void* q, long long ldq, const void* k, 
                                    unsigned long long stream_id, void* stream) {
   AttnParams p = {};
   if (int rc = fill_common(p, q, ldq, k, ldk, v, ldv, mask_a, mask_b, Wa, Fb, Nb, all_pairs, n_seq, heads, Sq, Sk,
-                           causal, scale, p_drop, rng_state, stream_id))
+                           causal, scale, p_drop, rng_state, stream_id, 256))
     return rc;
   UNIVL_CHECK_ARG(o != nullptr && (ldo % 2) == 0, "attention_fwd: bad output");
   if (n_seq == 0) return UNIVL_OK;
@@ -812,7 +649,7 @@ extern "C" int univl_attention_bwd(const void* q, long long ldq, const void* k, 
                                    int rng_layout, float* dbq, float* dbk, float* dbv, void* stream) {
   AttnParams p = {};
   if (int rc = fill_common(p, q, ldq, k, ldk, v, ldv, mask_a, mask_b, Wa, Fb, Nb, all_pairs, n_seq, heads, Sq, Sk,
-                           causal, scale, p_drop, rng_state, stream_id))
+                           causal, scale, p_drop, rng_state, stream_id, 256))
     return rc;
   UNIVL_CHECK_ARG(o && lse && d_o && dq && dk && dv, "attention_bwd: null pointer");
   UNIVL_CHECK_ARG((ldo % 8) == 0 && (lddo % 8) == 0 && (lddq % 2) == 0 && (lddk % 2) == 0 && (lddv % 2) == 0,

@@ -167,12 +167,23 @@ class MaskSpec:
         return self.b.shape[0] if self.b is not None else 0
 
 
+SHORT_ATTN_MAX_S = 256  # csrc/attention.cu keeps a head's whole K/V in shared memory up to this length
+
+
+def _attention_entry(kind, Sq, Sk):
+    """univl_attention_<kind> up to 256 tokens, the key-tiled univl_attention_long_<kind> (csrc/attention_long.cu,
+    <= 1024 tokens) beyond"""
+    if Sq > SHORT_ATTN_MAX_S or Sk > SHORT_ATTN_MAX_S:
+        return "univl_attention_long_" + kind
+    return "univl_attention_" + kind
+
+
 def attention_fwd(q, k, v, n_seq, Sq, Sk, mask, p=0.0, seed=0, stream=0):
     """q/k/v: 2-D views whose columns [h*64, h*64+64) hold head h (row stride arbitrary)."""
     o = _empty((n_seq * Sq, HEADS * 64), BF16, q)
     lse = _empty((n_seq * HEADS * Sq,), F32, q)
-    call("univl_attention_fwd", q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0), v.data_ptr(), v.stride(0),
-         o.data_ptr(), o.stride(0), lse.data_ptr(), ptr(mask.a), ptr(mask.b), mask.Wa, mask.Fb, mask.Nb,
+    call(_attention_entry("fwd", Sq, Sk), q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0), v.data_ptr(),
+         v.stride(0), o.data_ptr(), o.stride(0), lse.data_ptr(), ptr(mask.a), ptr(mask.b), mask.Wa, mask.Fb, mask.Nb,
          int(mask.all_pairs), n_seq, HEADS, Sq, Sk, int(mask.causal), 1.0 / math.sqrt(64.0), float(p), seed, stream)
     return o, lse
 
@@ -214,7 +225,10 @@ def attention_bwd(q, k, v, o, lse, d_o, dq, dk, dv, n_seq, Sq, Sk, mask, p=0.0, 
     bias gradients) to them, which saves the separate column-sum pass over the [T, 3H] gradient.
     rng_layout 1: the forward was the fused kernel (row-major dropout layout)."""
     dbq, dbk, dbv = dbias if dbias is not None else (None, None, None)
-    call("univl_attention_bwd", q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0), v.data_ptr(), v.stride(0),
+    entry = _attention_entry("bwd", Sq, Sk)
+    # the fused forward (the only source of rng_layout 1) runs at S <= 128 only
+    assert rng_layout == 0 or entry == "univl_attention_bwd", (rng_layout, Sq, Sk)
+    call(entry, q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0), v.data_ptr(), v.stride(0),
          o.data_ptr(), o.stride(0), lse.data_ptr(), d_o.data_ptr(), d_o.stride(0), dq.data_ptr(), dq.stride(0),
          dk.data_ptr(), dk.stride(0), dv.data_ptr(), dv.stride(0), ptr(mask.a), ptr(mask.b), mask.Wa, mask.Fb,
          mask.Nb, int(mask.all_pairs), n_seq, HEADS, Sq, Sk, int(mask.causal), 1.0 / math.sqrt(64.0), float(p), seed,
