@@ -38,7 +38,9 @@ int univl_set_reserved_sms(int n);
  * epilogue: 0 out(bf16)=alpha*acc+bias | 1 aux_out(bf16)=acc+bias, out(bf16)=gelu_erf(.) (until_module.py:28-33)
  *           2 out(bf16)=acc*gelu'(aux_in) | 3 out(bf16)=alpha*acc+aux_in | 4 out(f32)=alpha*acc+bias
  *           5 out(f32)+=alpha*acc (gradient accumulation; split-K partials are summed in split order)
- * block_n: 0 = auto | 64 | 128 | 256.  split_k: 0 = auto (epilogue 5 only). */
+ * block_n: 0 = auto | 64 | 128 | 256.  split_k: 0 = auto (epilogue 5 only).
+ * Aliasing: aux_in may be out itself (the same pointer and the same leading dimension, computed in place); any other
+ * overlap of aux_in or aux_out with out is undefined. */
 int univl_gemm_bf16(const void* A, long long lda, int a_mn_major, const void* B, long long ldb, int b_mn_major,
                     int M, int N, int Kc, void* out, long long ldo, int epilogue, const float* bias,
                     const void* aux_in, long long ld_aux_in, void* aux_out, long long ld_aux_out, float alpha,

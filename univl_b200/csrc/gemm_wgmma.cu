@@ -170,6 +170,103 @@ __device__ __forceinline__ void epi_pair(const GemmParams& p, int split, int row
   }
 }
 
+// 8-column groups per chunk of the unchecked epilogue: 16 aux_in words or 16 bias floats per chunk, two chunks in
+// flight; every instance compiles without spills under regs_alloc<232> (check with -Xptxas -v when changing it)
+constexpr int EPI_CHUNK = 8;
+
+// Unchecked epilogue of a work item whose 128 x BLOCK_N tile lies wholly inside M x N, with p.vec2 set (and, for
+// split-K partials, N even): no bounds checks, every access a 2-element vector.  The epilogue is a template argument,
+// so the fragment walk is straight-line code.  It runs in chunks of EPI_CHUNK 8-column groups.  Each chunk's global
+// loads (bias, aux_in, the accumulated output) are issued together, and before the previous chunk's arithmetic, so
+// their latencies overlap each other and that arithmetic instead of adding up.  Loading ahead of the previous chunk's
+// stores is safe for the exact in-place use epi_pair allows (aux_in == out, same leading dimension): each element is
+// read and written by the same thread, and a chunk's loads never touch the elements of an earlier chunk.
+// It computes exactly what epi_pair computes: the same fp32 operations in the same order, with __fmul_rn / __fadd_rn
+// so that alpha * acc and the add after it stay two roundings and are not contracted to an FFMA.
+// BIAS: p.bias is set (bias epilogues); PART: p.part is set (EPI_ATOMIC_F32 with split-K).
+template <int EPI, bool BIAS, bool PART, int BLOCK_N>
+__device__ __forceinline__ void epi_tile(const GemmParams& p, int split, int row, int col0,
+                                         const float (&acc)[BLOCK_N / 2]) {
+  constexpr int GROUPS = BLOCK_N / 8;
+  constexpr int CHUNK = GROUPS < EPI_CHUNK ? GROUPS : EPI_CHUNK;
+  constexpr bool AUX = EPI == EPI_GELU_BWD_BF16 || EPI == EPI_ADD_BF16;
+  constexpr bool OUT_F32 = EPI == EPI_BIAS_F32 || EPI == EPI_ATOMIC_F32;
+  constexpr bool ACCUM = EPI == EPI_ATOMIC_F32 && !PART;  // one split: out += alpha * acc
+  const float alpha = p.alpha;
+  const float* bias = p.bias + col0;
+  const bf16* ax = p.aux_in + (long long)row * p.ld_aux_in + col0;
+  const long long ax8 = 8 * p.ld_aux_in;
+  bf16* ao = p.aux_out + (long long)row * p.ld_aux_out + col0;
+  const long long ao8 = 8 * p.ld_aux_out;
+  const long long ld = PART ? (long long)p.N : p.ldo;
+  const long long o8 = 8 * ld;
+  float* of = PART ? p.part + ((long long)split * p.M + row) * p.N + col0
+                   : reinterpret_cast<float*>(p.out) + (long long)row * ld + col0;
+  bf16* ob = reinterpret_cast<bf16*>(p.out) + (long long)row * ld + col0;
+  // two load buffers, alternating between chunks
+  float b[2][CHUNK][2];
+  uint32_t x[2][CHUNK][2];
+  float2 a[2][CHUNK][2];
+  auto load = [&](int j0, int s) {
+#pragma unroll
+    for (int j = 0; j < CHUNK; ++j) {
+      const int c = (j0 + j) * 8;
+      if constexpr (BIAS) {
+        b[s][j][0] = __ldg(bias + c);
+        b[s][j][1] = __ldg(bias + c + 1);
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {  // rows row, row + 8
+        if constexpr (AUX) x[s][j][h] = *reinterpret_cast<const uint32_t*>(ax + h * ax8 + c);
+        if constexpr (ACCUM) a[s][j][h] = *reinterpret_cast<const float2*>(of + h * o8 + c);
+      }
+    }
+  };
+  load(0, 0);
+#pragma unroll
+  for (int j0 = 0; j0 < GROUPS; j0 += CHUNK) {
+    const int s = (j0 / CHUNK) & 1;
+    if (j0 + CHUNK < GROUPS) load(j0 + CHUNK, s ^ 1);
+#pragma unroll
+    for (int j = 0; j < CHUNK; ++j) {
+      const int c = (j0 + j) * 8;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float v0 = __fmul_rn(acc[4 * (j0 + j) + 2 * h], alpha);
+        float v1 = __fmul_rn(acc[4 * (j0 + j) + 2 * h + 1], alpha);
+        if constexpr (BIAS) {
+          v0 = __fadd_rn(v0, b[s][j][0]);
+          v1 = __fadd_rn(v1, b[s][j][1]);
+        }
+        if constexpr (AUX) {
+          const float2 f = unpack_bf16x2(x[s][j][h]);
+          if constexpr (EPI == EPI_GELU_BWD_BF16) {
+            v0 = __fmul_rn(v0, gelu_erf_grad(f.x));
+            v1 = __fmul_rn(v1, gelu_erf_grad(f.y));
+          } else {
+            v0 = __fadd_rn(v0, f.x);
+            v1 = __fadd_rn(v1, f.y);
+          }
+        }
+        if constexpr (OUT_F32) {
+          if constexpr (ACCUM) {
+            v0 = __fadd_rn(a[s][j][h].x, v0);
+            v1 = __fadd_rn(a[s][j][h].y, v1);
+          }
+          *reinterpret_cast<float2*>(of + h * o8 + c) = make_float2(v0, v1);
+        } else {
+          if constexpr (EPI == EPI_BIAS_GELU_BF16) {
+            *reinterpret_cast<uint32_t*>(ao + h * ao8 + c) = pack_bf16x2(v0, v1);
+            v0 = gelu_erf(v0);
+            v1 = gelu_erf(v1);
+          }
+          *reinterpret_cast<uint32_t*>(ob + h * o8 + c) = pack_bf16x2(v0, v1);
+        }
+      }
+    }
+  }
+}
+
 template <int BLOCK_N, int STAGES, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
@@ -276,11 +373,42 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       const int row = wi.m0 + c * 64 + warp * 16 + (lane >> 2);
       const int col0 = wi.n0 + 2 * (lane & 3);
       const int split = wi.kb_begin / kb_per;
+      // the epilogue is chosen once per work item: tiles wholly inside the output take the unchecked epi_tile, edge
+      // tiles and launches without 2-element vector access the checked per-pair epi_pair
+      const bool inside = p.vec2 && wi.m0 + BLOCK_M <= p.M && wi.n0 + BLOCK_N <= p.N &&
+                          (p.part == nullptr || (p.N & 1) == 0);
+      if (inside) {
+        const bool bias = p.bias != nullptr;
+        switch (p.epilogue) {
+          case EPI_BIAS_BF16:
+            if (bias) epi_tile<EPI_BIAS_BF16, true, false, BLOCK_N>(p, split, row, col0, acc);
+            else epi_tile<EPI_BIAS_BF16, false, false, BLOCK_N>(p, split, row, col0, acc);
+            break;
+          case EPI_BIAS_GELU_BF16:
+            if (bias) epi_tile<EPI_BIAS_GELU_BF16, true, false, BLOCK_N>(p, split, row, col0, acc);
+            else epi_tile<EPI_BIAS_GELU_BF16, false, false, BLOCK_N>(p, split, row, col0, acc);
+            break;
+          case EPI_GELU_BWD_BF16:
+            epi_tile<EPI_GELU_BWD_BF16, false, false, BLOCK_N>(p, split, row, col0, acc);
+            break;
+          case EPI_ADD_BF16:
+            epi_tile<EPI_ADD_BF16, false, false, BLOCK_N>(p, split, row, col0, acc);
+            break;
+          case EPI_BIAS_F32:
+            if (bias) epi_tile<EPI_BIAS_F32, true, false, BLOCK_N>(p, split, row, col0, acc);
+            else epi_tile<EPI_BIAS_F32, false, false, BLOCK_N>(p, split, row, col0, acc);
+            break;
+          default:
+            if (p.part != nullptr) epi_tile<EPI_ATOMIC_F32, false, true, BLOCK_N>(p, split, row, col0, acc);
+            else epi_tile<EPI_ATOMIC_F32, false, false, BLOCK_N>(p, split, row, col0, acc);
+        }
+      } else {
 #pragma unroll
-      for (int j = 0; j < BLOCK_N / 8; ++j) {
-        if (wi.n0 + j * 8 >= p.N) break;  // warp-uniform
-        epi_pair(p, split, row, col0 + j * 8, acc[4 * j], acc[4 * j + 1]);
-        epi_pair(p, split, row + 8, col0 + j * 8, acc[4 * j + 2], acc[4 * j + 3]);
+        for (int j = 0; j < BLOCK_N / 8; ++j) {
+          if (wi.n0 + j * 8 >= p.N) break;  // warp-uniform
+          epi_pair(p, split, row, col0 + j * 8, acc[4 * j], acc[4 * j + 1]);
+          epi_pair(p, split, row + 8, col0 + j * 8, acc[4 * j + 2], acc[4 * j + 3]);
+        }
       }
     }
   }
@@ -365,6 +493,10 @@ extern "C" int univl_gemm_plan(int M, int N, int Kc, int epilogue, int block_n, 
   return 1;
 }
 
+// Aliasing: aux_in may be out itself, with the same leading dimension (an in-place residual add or GELU backward):
+// every element is read and then written by the same thread, and epi_tile loads a chunk ahead only elements that thread
+// has not written yet.  Any other overlap of aux_in or aux_out with out is a race between threads and is not
+// supported.  No caller in ops.py aliases them.
 extern "C" int univl_gemm_bf16(const void* A, long long lda, int a_mn_major, const void* B, long long ldb,
                                int b_mn_major, int M, int N, int Kc, void* out, long long ldo, int epilogue,
                                const float* bias, const void* aux_in, long long ld_aux_in, void* aux_out,
