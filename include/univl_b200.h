@@ -77,8 +77,12 @@ int univl_embed_text_bwd(const void* dy, const long long* ids, const long long* 
                          int n_seq, int S, int H, int vocab, float p_drop, const unsigned long long* rng_state,
                          unsigned long long stream_id, void* stream);
 /* activation sources a[Na,Wa,H] (+ b[Nb,Fb,H]) + pos[s] (+ type[s>=Wa]) -> LN -> dropout
- * (module_visual.py:118-131; module_cross.py:123-138 with modeling.py:315-325; all_pairs=1 realises the B x B
- *  text-video pairing of modeling.py:341-375 without materialising the repeats) */
+ * (module_visual.py:118-131; module_cross.py:123-138 with modeling.py:315-325).  `all_pairs` is the number of pairing
+ * groups: 0 = aligned (sequence p reads a[p], b[p]; Na == Nb); 1 = the B x B text-video pairing of
+ * modeling.py:341-375 without materialising the repeats (p = i * Nb + j); G > 1 = G independent micro-batches, group g
+ * pairing a rows [g Na/G, (g+1) Na/G) with b rows [g Nb/G, (g+1) Nb/G): Na Nb / G sequences, sequence p of group
+ * g = p / (Gt Gv), r = p mod (Gt Gv), reads a[g Gt + r / Gv], b[g Gv + r % Gv] with Gt = Na/G, Gv = Nb/G (G must divide
+ * Na and Nb).  The backward sums a source row's gradient over the pairs of its own group only. */
 int univl_embed_src_fwd(const void* a, const void* b, const float* pos, const float* type, const float* gamma,
                         const float* beta, void* y, float* mean, float* rstd, int Na, int Wa, int Nb, int Fb,
                         int all_pairs, int H, float eps, float p_drop, const unsigned long long* rng_state,
@@ -90,7 +94,9 @@ int univl_embed_src_bwd(const void* dy, const void* a, const void* b, const floa
 
 /* ---- attention core (module_bert.py:176-196; module_decoder.py:225-245, mask :385-396) -------------------------
  * ctx = dropout(softmax(Q K^T * scale + mask)) V per (sequence, head), head dim 64.
- * mask = -10000 * (key padded [or key > query if causal]); key padding = concat(mask_a[i,:Wa], mask_b[j,:Fb]).
+ * mask = -10000 * (key padded [or key > query if causal]); key padding = concat(mask_a[i,:Wa], mask_b[j,:Fb]) with
+ * (i, j) the sources of the sequence under `all_pairs` pairing groups as in univl_embed_src_fwd (here Gv = Nb / G and
+ * Gt = n_seq / Nb; G > 1 needs G | Nb and Nb | n_seq).
  * univl_attention_fwd / _bwd take Sq, Sk <= 256 (whole K/V of a head in shared memory); univl_attention_long_fwd /
  * _bwd take the same arguments for 0 < Sq, Sk <= 1024 with 12 heads (key-tiled; rng_layout must be 0), which covers
  * the model's position tables: text, visual and decoder <= 512 tokens, cross encoder <= 1024.  Both draw the same
@@ -160,23 +166,32 @@ int univl_meanpool_fwd(const void* x, const long long* mask, float* out, float* 
                        int skip_first, int guard_zero, int l2norm, void* stream);
 int univl_meanpool_bwd(const float* dy, const float* y, const float* norm, const long long* mask, void* dx, int N,
                        int S, int H, int skip_first, int guard_zero, int l2norm, void* stream);
-/* sim = T V^T (modeling.py:389) */
-int univl_sim_matmul_fwd(const float* t, const float* v, float* sim, int Bt, int Bv, int H, void* stream);
+/* sim = T V^T (modeling.py:389).  groups = G >= 1: t [G Bt, H], v [G Bv, H] and sim the block diagonal [G, Bt, Bv],
+ * sim[g] = t[g Bt : (g+1) Bt] v[g Bv : (g+1) Bv]^T (one similarity matrix per micro-batch) */
+int univl_sim_matmul_fwd(const float* t, const float* v, float* sim, int Bt, int Bv, int H, int groups, void* stream);
 int univl_sim_matmul_bwd(const float* dsim, const float* t, const float* v, float* dt, float* dv, int Bt, int Bv,
-                         int H, void* stream);
-/* losses on sim[B,B]; each also writes dsim for an upstream gradient of 1 (until_module.py:182-251) */
+                         int H, int groups, void* stream);
+/* losses on sim[G,B,B] (until_module.py:182-251): loss = mean over the G groups of the reference loss of sim[g]; each
+ * also writes dsim for an upstream gradient of 1.  One CTA per group, the group losses averaged in group order: no
+ * floating-point atomics across groups, deterministic.  G = 1 is the single [B, B] loss. */
 int univl_maxmargin_loss(const float* sim, float* loss, float* dsim, int B, float margin, int n_pair, float w_same,
-                         float w_diff, void* stream);
-int univl_crossen_loss(const float* sim, float* loss, float* dsim, int B, void* stream);
-int univl_milnce_loss(const float* sim, float* loss, float* dsim, int batch_size, int n_pair, void* stream);
+                         float w_diff, int groups, void* stream);
+int univl_crossen_loss(const float* sim, float* loss, float* dsim, int B, int groups, void* stream);
+int univl_milnce_loss(const float* sim, float* loss, float* dsim, int batch_size, int n_pair, int groups,
+                      void* stream);
 /* CrossEntropyLoss(ignore_index) over wide rows (modeling.py:253, :275) and the MFM NCE (modeling.py:278-297:
- * target_mode 1 = diagonal target, pair_mask adds (1 - m_r m_c) * -1e8) */
+ * target_mode 1 = diagonal target, pair_mask adds (1 - m_r m_c) * -1e8).  groups = G >= 1 splits the T rows into G
+ * consecutive micro-batches of R = T / G rows: loss = mean over groups of (sum / count of the group's scored rows), a
+ * group without a scored row giving NaN like the reference's mean of an empty selection; the backward scales row r by
+ * (gscale / G) / count[group(r)].  Grouped target_mode 1 takes V = R: row r of group g holds its logits against the
+ * group's own R frames, target r - g R, mask columns pair_mask[g R + c].  sum_count: 2 G floats (sums, then counts). */
 int univl_softmax_xent_fwd(const float* logits, long long ld, const long long* labels, const long long* pair_mask,
                            float* lse, float* sum_count, float* loss, int T, int V, int target_mode,
-                           long long ignore_index, void* stream);
+                           long long ignore_index, int groups, void* stream);
 int univl_softmax_xent_bwd(const float* logits, long long ld, const long long* labels, const long long* pair_mask,
                            const float* lse, const float* sum_count, const float* gscale, void* dlogits,
-                           long long ld_d, int T, int V, int target_mode, long long ignore_index, void* stream);
+                           long long ld_d, int T, int V, int target_mode, long long ignore_index, int groups,
+                           void* stream);
 /* cross pooler tanh + similarity_dense (module_cross.py:281-287; modeling.py:371): out[r] = tanh(u[r,:]).w + b */
 int univl_pooler_sim_fwd(const void* u, const float* w, const float* b, float* out, int N, int H, void* stream);
 int univl_pooler_sim_bwd(const void* u, const float* w, const float* dout, void* du, float* dw, float* db, int N,

@@ -67,8 +67,8 @@ __device__ __forceinline__ void load_head_tile(bf16* dst, const bf16* src, long 
 
 // additive key mask for this sequence into smem: 0 / -10000 for real keys, -inf for padding beyond Sk
 __device__ __forceinline__ void build_key_mask(float* madd, const AttnParams& p, int seq, int Sk16) {
-  const long long i = p.all_pairs ? seq / p.Nb : seq;
-  const long long j = p.all_pairs ? seq % p.Nb : seq;
+  long long i, j;
+  pair_sources(seq, p.all_pairs, p.n_seq, p.Nb, i, j);
   for (int c = threadIdx.x; c < Sk16; c += blockDim.x) {
     float m;
     if (c >= p.Sk) m = -INFINITY;
@@ -162,6 +162,9 @@ static inline int fill_common(AttnParams& p, const void* q, long long ldq, const
   UNIVL_CHECK_ARG(mask_a == nullptr || Wa + Fb == Sk, "attention: mask parts (%d + %d) must cover Sk=%d", Wa, Fb, Sk);
   UNIVL_CHECK_ARG(!(Fb > 0 && mask_a != nullptr && mask_b == nullptr), "attention: missing second mask part");
   UNIVL_CHECK_ARG(!all_pairs || Nb > 0, "attention: all_pairs needs Nb > 0");
+  UNIVL_CHECK_ARG(all_pairs >= 0 && (all_pairs <= 1 || (Nb % all_pairs == 0 && n_seq % Nb == 0)),
+                  "attention: %d pairing groups need Nb=%d divisible by them and n_seq=%d divisible by Nb", all_pairs,
+                  Nb, n_seq);
   UNIVL_CHECK_ARG(p_drop >= 0.f && p_drop < 1.f, "attention: bad dropout probability");
   p.q = (const bf16*)q; p.k = (const bf16*)k; p.v = (const bf16*)v;
   p.ldq = ldq; p.ldk = ldk; p.ldv = ldv;

@@ -85,6 +85,33 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 }
 __device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31u; }
 
+// Text x video pairing of the cross encoder's sequences (reference modeling.py:341-375, one micro-batch per group).
+// `groups` (the ABI's `all_pairs`): 0 = aligned, sequence p reads (text p, video p); G >= 1 = G groups of Gt x Gv
+// pairs, Gv = Nb / G video rows and Gt = n_seq / Nb text rows per group, group g pairing text rows [g Gt, (g+1) Gt)
+// with video rows [g Gv, (g+1) Gv).  Sequence p of group g = p / (Gt Gv), r = p mod (Gt Gv), reads text g Gt + r / Gv
+// and video g Gv + r % Gv; G = 1 is the full B x B pairing (p / Nb, p % Nb).
+__device__ __forceinline__ void pair_sources(long long p, int groups, long long n_seq, long long Nb, long long& i,
+                                             long long& j) {
+  if (groups == 0) {
+    i = j = p;
+    return;
+  }
+  const long long Gv = Nb / groups;
+  const long long g = groups > 1 ? p / (n_seq / groups) : 0;
+  const long long r = p - g * (n_seq / groups);
+  i = g * (n_seq / Nb) + r / Gv;
+  j = g * Gv + r % Gv;
+}
+// The inverse, for one source row's fan-out: the sequence of the f-th pair of text row i (which == 0; f < Gv) or of
+// video row j (which == 1; f < Gt).  Every pair of a source row lies inside the source row's own group.
+__device__ __forceinline__ long long pair_sequence(int which, long long owner, int f, int groups, long long Gt,
+                                                   long long Gv) {
+  if (groups == 0) return owner;
+  if (which == 0) return owner * Gv + f;
+  const long long g = owner / Gv;
+  return (g * Gt + f) * Gv + (owner - g * Gv);
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -285,11 +285,11 @@ struct SrcCfg {
   const bf16* a;  // [Na, Wa, H]
   const bf16* b;  // [Nb, Fb, H] or null (Fb = 0)
   int Na, Wa, Nb, Fb;
-  int all_pairs;  // 0: sequence p reads (a[p], b[p]); 1: p = i * Nb + j reads (a[i], b[j])
+  int groups;  // pairing groups (common.cuh pair_sources): 0 = aligned, G = G groups of (Na/G) x (Nb/G) pairs
 };
 
 // Shared by both source kernels: one warp owns one SOURCE row (text row of a, or video row of b; blockIdx.y selects).
-// Every output sequence that reads this row (1 in aligned mode; Nb or Na in all-pairs mode) sees the SAME pre-LN
+// Every output sequence that reads this row (1 in aligned mode; Nb/G or Na/G with G pairing groups) sees the SAME pre-LN
 // vector z = src + pos (+ type), hence the same mean / rstd / normalised row: LayerNorm runs once per source row and
 // only the dropout mask differs between the fan-out rows.
 struct SrcRow {
@@ -302,11 +302,12 @@ __device__ __forceinline__ SrcRow src_row_info(const SrcCfg& c, int which, long 
   SrcRow r;
   r.owner = sr / len;
   r.s = (int)(sr % len) + (which == 0 ? 0 : c.Wa);
-  r.fan = c.all_pairs ? (which == 0 ? c.Nb : c.Na) : 1;
+  r.fan = c.groups ? (which == 0 ? c.Nb : c.Na) / c.groups : 1;
   return r;
 }
 __device__ __forceinline__ long long src_out_row(const SrcCfg& c, int which, const SrcRow& r, int f) {
-  const long long p = c.all_pairs ? (which == 0 ? r.owner * c.Nb + f : (long long)f * c.Nb + r.owner) : r.owner;
+  const int G = c.groups ? c.groups : 1;
+  const long long p = pair_sequence(which, r.owner, f, c.groups, c.Na / G, c.Nb / G);
   return p * (c.Wa + c.Fb) + r.s;
 }
 __device__ __forceinline__ void src_load_z(const SrcCfg& c, int which, long long sr, const SrcRow& r,
@@ -594,8 +595,10 @@ extern "C" int univl_embed_src_fwd(const void* a, const void* b, const float* po
   UNIVL_CHECK_ARG(a && pos && gamma && beta && y && mean && rstd, "embed_src_fwd: null pointer");
   UNIVL_CHECK_ARG(Na >= 0 && Wa > 0 && Fb >= 0 && (Fb == 0 || (b != nullptr && Nb > 0)), "embed_src_fwd: bad shape");
   UNIVL_CHECK_ARG(all_pairs || Fb == 0 || Na == Nb, "embed_src_fwd: aligned mode needs Na == Nb");
-  SrcCfg src{(const bf16*)a, (const bf16*)b, Na, Wa, Fb == 0 ? 1 : Nb, Fb, all_pairs && Fb > 0};
-  const long long n_seq = src.all_pairs ? (long long)Na * Nb : Na;
+  UNIVL_CHECK_ARG(all_pairs >= 0 && (all_pairs <= 1 || Fb == 0 || (Na % all_pairs == 0 && Nb % all_pairs == 0)),
+                  "embed_src_fwd: %d pairing groups must divide Na=%d and Nb=%d", all_pairs, Na, Nb);
+  SrcCfg src{(const bf16*)a, (const bf16*)b, Na, Wa, Fb == 0 ? 1 : Nb, Fb, Fb > 0 ? all_pairs : 0};
+  const long long n_seq = src.groups ? (long long)Na * Nb / src.groups : Na;
   if (n_seq == 0) return UNIVL_OK;
   const long long rows_a = (long long)Na * Wa, rows_b = (long long)(Fb == 0 ? 0 : Nb) * Fb;
   dim3 grid(emb_grid(rows_a > rows_b ? rows_a : rows_b), Fb == 0 ? 1 : 2);
@@ -613,7 +616,9 @@ extern "C" int univl_embed_src_bwd(const void* dy, const void* a, const void* b,
   UNIVL_CHECK_ARG(H == EMB_H, "embed_src_bwd: hidden size must be %d (got %d)", EMB_H, H);
   UNIVL_CHECK_ARG(dy && a && pos && gamma && mean && rstd && dpos && dgamma && dbeta, "embed_src_bwd: null pointer");
   UNIVL_CHECK_ARG(Fb == 0 || b != nullptr, "embed_src_bwd: missing second source");
-  SrcCfg src{(const bf16*)a, (const bf16*)b, Na, Wa, Fb == 0 ? 1 : Nb, Fb, all_pairs && Fb > 0};
+  UNIVL_CHECK_ARG(all_pairs >= 0 && (all_pairs <= 1 || Fb == 0 || (Na % all_pairs == 0 && Nb % all_pairs == 0)),
+                  "embed_src_bwd: %d pairing groups must divide Na=%d and Nb=%d", all_pairs, Na, Nb);
+  SrcCfg src{(const bf16*)a, (const bf16*)b, Na, Wa, Fb == 0 ? 1 : Nb, Fb, Fb > 0 ? all_pairs : 0};
   if (Na == 0) return UNIVL_OK;
   const long long rows_a = (long long)Na * Wa, rows_b = (long long)(Fb == 0 ? 0 : Nb) * Fb;
   dim3 grid(emb_bwd_grid(rows_a > rows_b ? rows_a : rows_b), Fb == 0 ? 1 : 2);

@@ -78,7 +78,8 @@ __device__ __forceinline__ float fa_key_mask(const long long* mask_a, const long
   const long long seq = (long long)rb * G + g;
   long long mv = 1;
   if (mask_a != nullptr && seq < n_seq) {
-    const long long mi = all_pairs ? seq / Nb : seq, mj = all_pairs ? seq % Nb : seq;
+    long long mi, mj;
+    pair_sources(seq, all_pairs, n_seq, Nb, mi, mj);
     if (kpos < Wa) mv = mask_a[mi * Wa + kpos];
     else if (mask_b != nullptr) mv = mask_b[mj * Fb + (kpos - Wa)];
   }
@@ -396,6 +397,9 @@ extern "C" int univl_fused_qkv_attention_fwd(const void* x, long long ldx, const
   UNIVL_CHECK_ARG(mask_a == nullptr || Wa + Fb == S, "fused_attention: mask parts (%d + %d) must cover S=%d", Wa, Fb, S);
   UNIVL_CHECK_ARG(!(Fb > 0 && mask_a != nullptr && mask_b == nullptr), "fused_attention: missing second mask part");
   UNIVL_CHECK_ARG(!all_pairs || Nb > 0, "fused_attention: all_pairs needs Nb > 0");
+  UNIVL_CHECK_ARG(all_pairs >= 0 && (all_pairs <= 1 || (Nb % all_pairs == 0 && n_seq % Nb == 0)),
+                  "fused_attention: %d pairing groups need Nb=%d divisible by them and n_seq=%d divisible by Nb", all_pairs,
+                  Nb, n_seq);
   UNIVL_CHECK_ARG(p_drop >= 0.f && p_drop < 1.f, "fused_attention: bad dropout probability");
   UNIVL_CHECK_ARG(p_drop == 0.f || rng_state != nullptr, "fused_attention: dropout needs rng_state");
   UNIVL_CHECK_ARG(qkv_out == nullptr || ((ld_qkv % 8) == 0 && ((uintptr_t)qkv_out & 15) == 0),
@@ -743,6 +747,9 @@ extern "C" int univl_fused_attention_bwd(const void* qkv, long long ld_qkv, cons
   UNIVL_CHECK_ARG(mask_a == nullptr || Wa + Fb == S, "fused_attention_bwd: mask parts must cover S");
   UNIVL_CHECK_ARG(!(Fb > 0 && mask_a != nullptr && mask_b == nullptr), "fused_attention_bwd: missing second mask part");
   UNIVL_CHECK_ARG(!all_pairs || Nb > 0, "fused_attention_bwd: all_pairs needs Nb > 0");
+  UNIVL_CHECK_ARG(all_pairs >= 0 && (all_pairs <= 1 || (Nb % all_pairs == 0 && n_seq % Nb == 0)),
+                  "fused_attention_bwd: %d pairing groups need Nb=%d divisible by them and n_seq=%d divisible by Nb", all_pairs,
+                  Nb, n_seq);
   UNIVL_CHECK_ARG(p_drop >= 0.f && p_drop < 1.f && (p_drop == 0.f || rng_state != nullptr),
                   "fused_attention_bwd: bad dropout arguments");
   FusedAttnBwdParams p = {};

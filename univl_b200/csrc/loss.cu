@@ -91,23 +91,29 @@ meanpool_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ y, c
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// sim = T V^T  (tiny)
+// sim = T V^T  (tiny); with G groups the block diagonal sim[g] = T[g Bt : (g+1) Bt] V[g Bv : (g+1) Bv]^T, [G, Bt, Bv]
 // ------------------------------------------------------------------------------------------------------------
 __global__ void sim_fwd_kernel(const float* __restrict__ t, const float* __restrict__ v, float* __restrict__ sim,
-                               int Bt, int Bv, int H) {
+                               int Bt, int Bv, int H, int groups) {
   const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (gw >= Bt * Bv) return;
-  const int i = gw / Bv, j = gw % Bv;
+  if (gw >= groups * Bt * Bv) return;
+  const int g = gw / (Bt * Bv), e = gw - g * (Bt * Bv);
+  const int i = g * Bt + e / Bv, j = g * Bv + e % Bv;
   float acc = 0.f;
   for (int c = lane; c < H; c += 32) acc += t[(long long)i * H + c] * v[(long long)j * H + c];
   acc = warp_sum(acc);
   if (lane == 0) sim[gw] = acc;
 }
-// dt[i,:] = sum_j dsim[i,j] v[j,:] ; dv[j,:] = sum_i dsim[i,j] t[i,:]
+// dt[i,:] = sum_j dsim[i,j] v[j,:] ; dv[j,:] = sum_i dsim[i,j] t[i,:]   (within group blockIdx.x / (Bt + Bv))
 __global__ void sim_bwd_kernel(const float* __restrict__ dsim, const float* __restrict__ t,
                                const float* __restrict__ v, float* __restrict__ dt, float* __restrict__ dv, int Bt,
                                int Bv, int H) {
-  const int r = blockIdx.x;
+  const int g = blockIdx.x / (Bt + Bv), r = blockIdx.x - g * (Bt + Bv);
+  dsim += (long long)g * Bt * Bv;
+  t += (long long)g * Bt * H;
+  dt += (long long)g * Bt * H;
+  v += (long long)g * Bv * H;
+  dv += (long long)g * Bv * H;
   if (r < Bt) {
     for (int c = threadIdx.x; c < H; c += blockDim.x) {
       float acc = 0.f;
@@ -125,13 +131,28 @@ __global__ void sim_bwd_kernel(const float* __restrict__ dsim, const float* __re
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// losses on a [B, B] similarity matrix (single CTA)
+// losses on a [B, B] similarity matrix, one CTA per group of a [G, B, B] stack.  With G = 1 the CTA writes the loss
+// itself; with G > 1 it writes its group's loss to parts[g] (group_mean_kernel averages them in group order) and scales
+// its dsim by 1/G, the gradient of the mean over groups.
 // ------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void group_scale_dsim(float* dsim, int n) {
+  if (gridDim.x == 1) return;
+  __syncthreads();
+  const float s = 1.0f / (float)gridDim.x;
+  for (int e = threadIdx.x; e < n; e += blockDim.x) dsim[e] *= s;
+}
+__global__ void group_mean_kernel(const float* __restrict__ parts, int groups, float* __restrict__ out) {
+  float acc = 0.f;
+  for (int g = 0; g < groups; ++g) acc += parts[g];
+  *out = acc / (float)groups;
+}
 // mean_ij w_ij * ( relu(m + s_ij - s_ii) + relu(m + s_ij - s_jj) ), diagonal included (until_module.py:245-251)
 __global__ void __launch_bounds__(256)
 maxmargin_kernel(const float* __restrict__ sim, float* __restrict__ loss, float* __restrict__ dsim, int B, float margin,
                  int n_pair, float w_same, float w_diff) {
   __shared__ float red[32];
+  sim += (long long)blockIdx.x * B * B;
+  dsim += (long long)blockIdx.x * B * B;
   const float inv = 1.0f / ((float)B * (float)B);
   for (int e = threadIdx.x; e < B * B; e += blockDim.x) dsim[e] = 0.f;
   __syncthreads();
@@ -163,13 +184,16 @@ maxmargin_kernel(const float* __restrict__ sim, float* __restrict__ loss, float*
     dsim[k * B + k] += t;
   }
   acc = block_sum(acc, red);
-  if (threadIdx.x == 0) *loss = acc * inv;
+  if (threadIdx.x == 0) loss[blockIdx.x] = acc * inv;
+  group_scale_dsim(dsim, B * B);
 }
 
 // -mean_i log_softmax(sim[i,:])[i]   (until_module.py:186-191)
 __global__ void __launch_bounds__(256)
 crossen_kernel(const float* __restrict__ sim, float* __restrict__ loss, float* __restrict__ dsim, int B) {
   __shared__ float red[32];
+  sim += (long long)blockIdx.x * B * B;
+  dsim += (long long)blockIdx.x * B * B;
   float acc = 0.f;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
   for (int i = warp; i < B; i += nw) {
@@ -185,7 +209,8 @@ crossen_kernel(const float* __restrict__ sim, float* __restrict__ loss, float* _
     if (lane == 0) acc += lse - sim[i * B + i];
   }
   acc = block_sum(acc, red);
-  if (threadIdx.x == 0) *loss = acc / (float)B;
+  if (threadIdx.x == 0) loss[blockIdx.x] = acc / (float)B;
+  group_scale_dsim(dsim, B * B);
 }
 
 // MIL-NCE (until_module.py:201-221) on sim [N, N], N = bs * P.  For each picked row r = k*P + P/2:
@@ -195,6 +220,8 @@ __global__ void __launch_bounds__(256)
 milnce_kernel(const float* __restrict__ sim, float* __restrict__ loss, float* __restrict__ dsim, int bs, int P) {
   __shared__ float red[32];
   const int N = bs * P;
+  sim += (long long)blockIdx.x * N * N;
+  dsim += (long long)blockIdx.x * N * N;
   for (int e = threadIdx.x; e < N * N; e += blockDim.x) dsim[e] = 0.f;
   __syncthreads();
   float acc = 0.f;
@@ -237,7 +264,8 @@ milnce_kernel(const float* __restrict__ sim, float* __restrict__ loss, float* __
     }
   }
   acc = block_sum(acc, red);
-  if (threadIdx.x == 0) *loss = acc / (float)bs;
+  if (threadIdx.x == 0) loss[blockIdx.x] = acc / (float)bs;
+  group_scale_dsim(dsim, N * N);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -245,10 +273,13 @@ milnce_kernel(const float* __restrict__ sim, float* __restrict__ loss, float* __
 // ------------------------------------------------------------------------------------------------------------
 // target_mode 0: target = labels[r]; 1: target = r.  Row is scored iff labels[r] != ignore_index.
 // Optional pairwise mask (MFM): logit += (1 - vm[r] * vm[c]) * -1e8   (modeling.py:286-288).
+// G groups of R = T / G consecutive rows (micro-batches) keep their own sum and count: loss_sum[g], count[g].  In
+// target_mode 1 a row of group g holds logits against its own group's R frames only (the MFM NCE of one micro-batch):
+// its target is r - g R and its mask columns are vm[g R + c].
 __global__ void __launch_bounds__(256)
 xent_fwd_kernel(const float* __restrict__ logits, long long ld, const long long* __restrict__ labels,
                 const long long* __restrict__ vm, float* __restrict__ lse_out, float* __restrict__ loss_sum,
-                float* __restrict__ count, int V, int target_mode, long long ignore_index) {
+                float* __restrict__ count, int V, int target_mode, long long ignore_index, int rows_per_group) {
   __shared__ float red[32];
   const int r = blockIdx.x;
   const long long lab = labels[r];
@@ -256,8 +287,11 @@ xent_fwd_kernel(const float* __restrict__ logits, long long ld, const long long*
     if (threadIdx.x == 0) lse_out[r] = 0.f;
     return;
   }
+  const int g = r / rows_per_group;
+  const long long off = target_mode == 1 ? (long long)g * rows_per_group : 0;
   const float* row = logits + (long long)r * ld;
   const float vr = vm ? (vm[r] != 0 ? 1.f : 0.f) : 1.f;
+  if (vm) vm += off;
   float m = -INFINITY;
   for (int c = threadIdx.x; c < V; c += blockDim.x) {
     float x = row[c];
@@ -275,20 +309,21 @@ xent_fwd_kernel(const float* __restrict__ logits, long long ld, const long long*
   if (threadIdx.x == 0) {
     const float lse = m + logf(l);
     lse_out[r] = lse;
-    const long long tgt = target_mode == 0 ? lab : r;
+    const long long tgt = target_mode == 0 ? lab : r - off;
     float xt = row[tgt];
     if (vm) xt += (1.0f - vr * (vm[tgt] != 0 ? 1.f : 0.f)) * -1e8f;
-    atomicAdd(loss_sum, lse - xt);
-    atomicAdd(count, 1.f);
+    atomicAdd(loss_sum + g, lse - xt);
+    atomicAdd(count + g, 1.f);
   }
 }
 
-// dlogits(bf16)[r, c] = g/count * (softmax - onehot) for scored rows, 0 elsewhere; columns [V, ld_d) zero-filled
+// dlogits(bf16)[r, c] = (g / G) / count[group] * (softmax - onehot) for scored rows, 0 elsewhere; columns [V, ld_d)
+// zero-filled
 __global__ void __launch_bounds__(256)
 xent_bwd_kernel(const float* __restrict__ logits, long long ld, const long long* __restrict__ labels,
                 const long long* __restrict__ vm, const float* __restrict__ lse_in, const float* __restrict__ count,
                 const float* __restrict__ gscale, bf16* __restrict__ dlogits, long long ld_d, int V, int target_mode,
-                long long ignore_index) {
+                long long ignore_index, int rows_per_group, int groups) {
   const int r = blockIdx.x;
   const long long lab = labels[r];
   bf16* drow = dlogits + (long long)r * ld_d;
@@ -296,11 +331,15 @@ xent_bwd_kernel(const float* __restrict__ logits, long long ld, const long long*
     for (int c = threadIdx.x; c < ld_d; c += blockDim.x) drow[c] = __float2bfloat16(0.f);
     return;
   }
+  const int grp = r / rows_per_group;
+  const long long off = target_mode == 1 ? (long long)grp * rows_per_group : 0;
   const float* row = logits + (long long)r * ld;
   const float vr = vm ? (vm[r] != 0 ? 1.f : 0.f) : 1.f;
+  if (vm) vm += off;
   const float lse = lse_in[r];
-  const float g = (gscale ? *gscale : 1.f) / *count;
-  const long long tgt = target_mode == 0 ? lab : r;
+  // (gscale / G) / count: the bits of the reference loop's (loss / G).backward() on this row's micro-batch alone
+  const float g = ((gscale ? *gscale : 1.f) / (float)groups) / count[grp];
+  const long long tgt = target_mode == 0 ? lab : r - off;
   for (int c = threadIdx.x; c < ld_d; c += blockDim.x) {
     float d = 0.f;
     if (c < V) {
@@ -312,9 +351,13 @@ xent_bwd_kernel(const float* __restrict__ logits, long long ld, const long long*
   }
 }
 
-__global__ void finalize_mean_kernel(const float* __restrict__ sum, const float* __restrict__ count,
+// mean over groups of sum[g] / count[g]; 0/0 -> NaN exactly like the reference's mean of an empty selection
+// (modeling.py:295-296), so a group without a scored row makes the loss NaN, as that micro-batch's loss would be
+__global__ void finalize_mean_kernel(const float* __restrict__ sum, const float* __restrict__ count, int groups,
                                      float* __restrict__ out) {
-  *out = *sum / *count;  // 0/0 -> NaN exactly like the reference's mean of an empty selection (modeling.py:295-296)
+  float acc = sum[0] / count[0];
+  for (int g = 1; g < groups; ++g) acc += sum[g] / count[g];
+  *out = groups > 1 ? acc / (float)groups : acc;
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -384,65 +427,93 @@ extern "C" int univl_meanpool_bwd(const float* dy, const float* y, const float* 
   UNIVL_CHECK_LAUNCH("meanpool_bwd");
   return UNIVL_OK;
 }
-extern "C" int univl_sim_matmul_fwd(const float* t, const float* v, float* sim, int Bt, int Bv, int H, void* stream) {
-  UNIVL_CHECK_ARG(t && v && sim && Bt > 0 && Bv > 0 && H > 0, "sim_matmul_fwd: bad arguments");
-  const long long threads = (long long)Bt * Bv * 32;
-  sim_fwd_kernel<<<(int)((threads + 255) / 256), 256, 0, (cudaStream_t)stream>>>(t, v, sim, Bt, Bv, H);
+extern "C" int univl_sim_matmul_fwd(const float* t, const float* v, float* sim, int Bt, int Bv, int H, int groups,
+                                    void* stream) {
+  UNIVL_CHECK_ARG(t && v && sim && Bt > 0 && Bv > 0 && H > 0 && groups > 0, "sim_matmul_fwd: bad arguments");
+  const long long threads = (long long)groups * Bt * Bv * 32;
+  sim_fwd_kernel<<<(int)((threads + 255) / 256), 256, 0, (cudaStream_t)stream>>>(t, v, sim, Bt, Bv, H, groups);
   UNIVL_CHECK_LAUNCH("sim_matmul_fwd");
   return UNIVL_OK;
 }
 extern "C" int univl_sim_matmul_bwd(const float* dsim, const float* t, const float* v, float* dt, float* dv, int Bt,
-                                    int Bv, int H, void* stream) {
-  UNIVL_CHECK_ARG(dsim && t && v && dt && dv && Bt > 0 && Bv > 0 && H > 0, "sim_matmul_bwd: bad arguments");
-  sim_bwd_kernel<<<Bt + Bv, 256, 0, (cudaStream_t)stream>>>(dsim, t, v, dt, dv, Bt, Bv, H);
+                                    int Bv, int H, int groups, void* stream) {
+  UNIVL_CHECK_ARG(dsim && t && v && dt && dv && Bt > 0 && Bv > 0 && H > 0 && groups > 0,
+                  "sim_matmul_bwd: bad arguments");
+  sim_bwd_kernel<<<groups * (Bt + Bv), 256, 0, (cudaStream_t)stream>>>(dsim, t, v, dt, dv, Bt, Bv, H);
   UNIVL_CHECK_LAUNCH("sim_matmul_bwd");
+  return UNIVL_OK;
+}
+// one CTA per group; G > 1 collects the group losses in scratch and averages them in group order
+template <typename Launch>
+static int group_loss(float* loss, int groups, cudaStream_t st, const char* name, Launch launch) {
+  if (groups == 1) {
+    launch(loss);
+    UNIVL_CHECK_LAUNCH(name);
+    return UNIVL_OK;
+  }
+  float* parts;
+  if (int rc = scratch_alloc((void**)&parts, (size_t)groups * sizeof(float), st)) return rc;
+  launch(parts);
+  group_mean_kernel<<<1, 1, 0, st>>>(parts, groups, loss);
+  const cudaError_t e = cudaGetLastError();
+  cudaFreeAsync(parts, st);
+  if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "%s launch: %s", name, cudaGetErrorString(e));
   return UNIVL_OK;
 }
 // n_pair <= 0 disables the block weighting (weights 1)
 extern "C" int univl_maxmargin_loss(const float* sim, float* loss, float* dsim, int B, float margin, int n_pair,
-                                    float w_same, float w_diff, void* stream) {
-  UNIVL_CHECK_ARG(sim && loss && dsim && B > 0 && B <= 4096, "maxmargin_loss: bad arguments");
-  maxmargin_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(sim, loss, dsim, B, margin, n_pair, w_same, w_diff);
-  UNIVL_CHECK_LAUNCH("maxmargin_loss");
-  return UNIVL_OK;
+                                    float w_same, float w_diff, int groups, void* stream) {
+  UNIVL_CHECK_ARG(sim && loss && dsim && B > 0 && B <= 4096 && groups > 0, "maxmargin_loss: bad arguments");
+  cudaStream_t st = (cudaStream_t)stream;
+  return group_loss(loss, groups, st, "maxmargin_loss", [&](float* out) {
+    maxmargin_kernel<<<groups, 256, 0, st>>>(sim, out, dsim, B, margin, n_pair, w_same, w_diff);
+  });
 }
-extern "C" int univl_crossen_loss(const float* sim, float* loss, float* dsim, int B, void* stream) {
-  UNIVL_CHECK_ARG(sim && loss && dsim && B > 0, "crossen_loss: bad arguments");
-  crossen_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(sim, loss, dsim, B);
-  UNIVL_CHECK_LAUNCH("crossen_loss");
-  return UNIVL_OK;
+extern "C" int univl_crossen_loss(const float* sim, float* loss, float* dsim, int B, int groups, void* stream) {
+  UNIVL_CHECK_ARG(sim && loss && dsim && B > 0 && groups > 0, "crossen_loss: bad arguments");
+  cudaStream_t st = (cudaStream_t)stream;
+  return group_loss(loss, groups, st, "crossen_loss", [&](float* out) {
+    crossen_kernel<<<groups, 256, 0, st>>>(sim, out, dsim, B);
+  });
 }
-extern "C" int univl_milnce_loss(const float* sim, float* loss, float* dsim, int batch_size, int n_pair,
+extern "C" int univl_milnce_loss(const float* sim, float* loss, float* dsim, int batch_size, int n_pair, int groups,
                                  void* stream) {
-  UNIVL_CHECK_ARG(sim && loss && dsim && batch_size > 0 && n_pair > 0, "milnce_loss: bad arguments");
-  milnce_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(sim, loss, dsim, batch_size, n_pair);
-  UNIVL_CHECK_LAUNCH("milnce_loss");
-  return UNIVL_OK;
+  UNIVL_CHECK_ARG(sim && loss && dsim && batch_size > 0 && n_pair > 0 && groups > 0, "milnce_loss: bad arguments");
+  cudaStream_t st = (cudaStream_t)stream;
+  return group_loss(loss, groups, st, "milnce_loss", [&](float* out) {
+    milnce_kernel<<<groups, 256, 0, st>>>(sim, out, dsim, batch_size, n_pair);
+  });
 }
-// loss = mean over scored rows of (logsumexp(row) - row[target]);  scratch: lse[T], sum_count[2] (zeroed here)
+// loss = mean over groups of the mean over the group's scored rows of (logsumexp(row) - row[target]);
+// scratch: lse[T], sum_count[2 * groups] (sums, then counts; zeroed here)
 extern "C" int univl_softmax_xent_fwd(const float* logits, long long ld, const long long* labels,
                                       const long long* pair_mask, float* lse, float* sum_count, float* loss, int T,
-                                      int V, int target_mode, long long ignore_index, void* stream) {
+                                      int V, int target_mode, long long ignore_index, int groups, void* stream) {
   UNIVL_CHECK_ARG(logits && labels && lse && sum_count && loss && T > 0 && V > 0 && ld >= V,
                   "softmax_xent_fwd: bad arguments");
   UNIVL_CHECK_ARG(target_mode == 0 || target_mode == 1, "softmax_xent_fwd: bad target_mode");
+  UNIVL_CHECK_ARG(groups > 0 && T % groups == 0, "softmax_xent_fwd: %d groups must divide T=%d", groups, T);
+  UNIVL_CHECK_ARG(target_mode == 0 || groups == 1 || V == T / groups,
+                  "softmax_xent_fwd: grouped target_mode 1 needs V = T / groups");
   cudaStream_t st = (cudaStream_t)stream;
-  cudaError_t e = cudaMemsetAsync(sum_count, 0, 2 * sizeof(float), st);
+  cudaError_t e = cudaMemsetAsync(sum_count, 0, 2 * (size_t)groups * sizeof(float), st);
   if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "softmax_xent_fwd memset: %s", cudaGetErrorString(e));
-  xent_fwd_kernel<<<T, 256, 0, st>>>(logits, ld, labels, pair_mask, lse, sum_count, sum_count + 1, V, target_mode,
-                                     ignore_index);
-  finalize_mean_kernel<<<1, 1, 0, st>>>(sum_count, sum_count + 1, loss);
+  xent_fwd_kernel<<<T, 256, 0, st>>>(logits, ld, labels, pair_mask, lse, sum_count, sum_count + groups, V, target_mode,
+                                     ignore_index, T / groups);
+  finalize_mean_kernel<<<1, 1, 0, st>>>(sum_count, sum_count + groups, groups, loss);
   UNIVL_CHECK_LAUNCH("softmax_xent_fwd");
   return UNIVL_OK;
 }
 extern "C" int univl_softmax_xent_bwd(const float* logits, long long ld, const long long* labels,
                                       const long long* pair_mask, const float* lse, const float* sum_count,
                                       const float* gscale, void* dlogits, long long ld_d, int T, int V,
-                                      int target_mode, long long ignore_index, void* stream) {
+                                      int target_mode, long long ignore_index, int groups, void* stream) {
   UNIVL_CHECK_ARG(logits && labels && lse && sum_count && dlogits && T > 0 && V > 0 && ld_d >= V,
                   "softmax_xent_bwd: bad arguments");
-  xent_bwd_kernel<<<T, 256, 0, (cudaStream_t)stream>>>(logits, ld, labels, pair_mask, lse, sum_count + 1, gscale,
-                                                       (bf16*)dlogits, ld_d, V, target_mode, ignore_index);
+  UNIVL_CHECK_ARG(groups > 0 && T % groups == 0, "softmax_xent_bwd: %d groups must divide T=%d", groups, T);
+  xent_bwd_kernel<<<T, 256, 0, (cudaStream_t)stream>>>(logits, ld, labels, pair_mask, lse, sum_count + groups, gscale,
+                                                       (bf16*)dlogits, ld_d, V, target_mode, ignore_index,
+                                                       T / groups, groups);
   UNIVL_CHECK_LAUNCH("softmax_xent_bwd");
   return UNIVL_OK;
 }

@@ -189,44 +189,47 @@ class UniVL(UniVLPreTrainedModel):
         """reference :315-325 (+ the pairing of :355-370) -> (hidden2d, n_seq, S)"""
         return self.cross.encode_pairs(seq2d, vis2d, attention_mask, video_mask, all_pairs)
 
-    def _cross_similarity(self, seq2d, vis2d, attention_mask, video_mask):
+    def _cross_similarity(self, seq2d, vis2d, attention_mask, video_mask, groups=1):
         """reference :341-375: every (text i, video j) pair through the cross encoder -> pooled -> similarity_dense.
         The reference walks text rows in chunks of 5 and `repeat`s both sides; here all B_t x B_v sequences go
-        through the layer kernels in one batch and the embedding kernel reads the un-repeated sources."""
+        through the layer kernels in one batch and the embedding kernel reads the un-repeated sources.  groups > 1:
+        only the pairs inside each micro-batch, G * Bg^2 sequences -> [G, Bg, Bg]."""
         bt, bv = attention_mask.shape[0], video_mask.shape[0]
         # only token 0 of the last cross layer feeds the pooler: the last layer computes just those rows
-        first, n_seq = self.cross.encode_pairs_first_token(seq2d, vis2d, attention_mask, video_mask, True)
+        first, n_seq = self.cross.encode_pairs_first_token(seq2d, vis2d, attention_mask, video_mask, groups)
         u = self.cross.pooler.pre_activation(first, n_seq, 1)
         logits = ops.PoolerSimFn.apply(u, self.similarity_dense.weight, self.similarity_dense.bias)
+        if groups > 1:
+            return logits.view(groups, bt // groups, bv // groups)
         return logits.view(bt, bv)
 
-    def _mean_pool_similarity(self, seq2d, vis2d, attention_mask, video_mask):
-        """reference :327-339 and :385-389"""
+    def _mean_pool_similarity(self, seq2d, vis2d, attention_mask, video_mask, groups=1):
+        """reference :327-339 and :385-389; groups > 1: the block diagonal [G, Bg, Bg]"""
         l2 = self.task_config.use_mil is False
         n_t, W = attention_mask.shape
         n_v, F = video_mask.shape
         text = ops.MeanPoolFn.apply(seq2d, attention_mask, n_t, W, True, False, l2)
         video = ops.MeanPoolFn.apply(vis2d, video_mask, n_v, F, False, True, l2)
-        return ops.SimMatmulFn.apply(text, video)
+        return ops.SimMatmulFn.apply(text, video, groups)
 
-    def _similarity(self, seq2d, vis2d, attention_mask, video_mask, _pretrain_joint=False):
+    def _similarity(self, seq2d, vis2d, attention_mask, video_mask, _pretrain_joint=False, groups=1):
         if (self._stage_two and _pretrain_joint is False) or self.train_sim_after_cross:
-            return self._cross_similarity(seq2d, vis2d, attention_mask, video_mask)
-        return self._mean_pool_similarity(seq2d, vis2d, attention_mask, video_mask)
+            return self._cross_similarity(seq2d, vis2d, attention_mask, video_mask, groups)
+        return self._mean_pool_similarity(seq2d, vis2d, attention_mask, video_mask, groups)
 
-    def _calculate_mlm_loss(self, cross2d, n_seq, S, W, token_labels):
+    def _calculate_mlm_loss(self, cross2d, n_seq, S, W, token_labels, groups=1):
         """reference :273-276 on the text half of the cross output"""
         text_rows = cross2d.view(n_seq, S, -1)[:, :W].reshape(n_seq * W, -1)
-        return self.cls.loss(text_rows, token_labels)
+        return self.cls.loss(text_rows, token_labels, groups=groups)
 
-    def _calculate_mfm_loss(self, cross2d, n_seq, S, W, video_norm, video_mask, video_labels_index):
-        """reference :278-297: NCE of every masked frame against all frames of the rank"""
+    def _calculate_mfm_loss(self, cross2d, n_seq, S, W, video_norm, video_mask, video_labels_index, groups=1):
+        """reference :278-297: NCE of every masked frame against all frames of the rank (of its micro-batch)"""
         F = S - W
         vis_rows = cross2d.view(n_seq, S, -1)[:, W:].reshape(n_seq * F, -1)
         scores = self.cls_visual.scores(vis_rows)
         frames = video_norm.reshape(n_seq * F, -1)
         return ops.ProjXentFn.apply(scores, frames, None, video_labels_index.reshape(-1).contiguous(),
-                                    video_mask.reshape(-1).contiguous(), 1, False, False)
+                                    video_mask.reshape(-1).contiguous(), 1, False, False, groups)
 
     def _decoder_hidden(self, seq2d, vis2d, attention_mask, video_mask, input_caption_ids, decoder_mask):
         """reference :393-407 up to the classifier"""
@@ -238,7 +241,16 @@ class UniVL(UniVLPreTrainedModel):
     # ------------------------------------------------------------------------------------------------------
     def forward(self, input_ids, token_type_ids, attention_mask, video, video_mask=None,
                 pairs_masked_text=None, pairs_token_labels=None, masked_video=None, video_labels_index=None,
-                input_caption_ids=None, decoder_mask=None, output_caption_ids=None):
+                input_caption_ids=None, decoder_mask=None, output_caption_ids=None, micro_batches=1):
+        """micro_batches = G > 1: the batch holds G consecutive micro-batches (rows [g b, (g+1) b) of the leading
+        dimension) of a gradient-accumulation window, run as one batch.  Returns (1/G) * sum_g L_g, L_g being the loss
+        of micro-batch g alone (its own similarity matrix, contrastive negatives, MLM / MFM / caption means), so one
+        backward() gives the window's accumulated gradient.  G = 1 is the plain call."""
+        G = micro_batches
+        if isinstance(G, bool) or not isinstance(G, int) or G < 1:
+            raise ValueError("micro_batches must be an integer >= 1, got %r" % (micro_batches,))
+        if G > 1 and input_ids.shape[0] % G:
+            raise ValueError("micro_batches=%d does not divide the batch of %d rows" % (G, input_ids.shape[0]))
         with rt.use_model(self, self._device()):
             input_ids, token_type_ids = _flat(input_ids), _flat(token_type_ids)
             attention_mask, video_mask = _flat(attention_mask), _flat(video_mask)
@@ -251,7 +263,7 @@ class UniVL(UniVLPreTrainedModel):
             cfg = self.task_config
             loss = 0.
             if self._stage_one:
-                sim = self._similarity(seq, vis, attention_mask, video_mask)
+                sim = self._similarity(seq, vis, attention_mask, video_mask, groups=G)
                 loss = loss + self.loss_fct(sim)
             if self._stage_two:
                 seq_a, vis_a = seq, vis
@@ -262,17 +274,17 @@ class UniVL(UniVLPreTrainedModel):
                     seq_a, vis_a = self._encode(masked_ids, token_type_ids, attention_mask, masked_video, video_mask)
                     cross2d, n_seq, S = self._cross_pairs(seq_a, vis_a, attention_mask, video_mask, False)
                     W = attention_mask.shape[-1]
-                    loss = loss + self._calculate_mlm_loss(cross2d, n_seq, S, W, token_labels)
+                    loss = loss + self._calculate_mlm_loss(cross2d, n_seq, S, W, token_labels, G)
                     loss = loss + self._calculate_mfm_loss(cross2d, n_seq, S, W, video, video_mask,
-                                                           video_labels_index)
-                    joint = self._similarity(seq, vis, attention_mask, video_mask, _pretrain_joint=True)
+                                                           video_labels_index, G)
+                    joint = self._similarity(seq, vis, attention_mask, video_mask, _pretrain_joint=True, groups=G)
                     loss = loss + self._pretrain_sim_loss_fct(joint)
                 if input_caption_ids is not None and (cfg.do_pretrain or cfg.task_type == "caption"):
                     hidden = self._decoder_hidden(seq_a, vis_a, attention_mask, video_mask, input_caption_ids,
                                                   decoder_mask)
-                    loss = loss + self.decoder.classifier.cls.loss(hidden, _flat(output_caption_ids))
+                    loss = loss + self.decoder.classifier.cls.loss(hidden, _flat(output_caption_ids), groups=G)
                 if cfg.do_pretrain or cfg.task_type == "retrieval":
-                    sim = self._similarity(seq_a, vis_a, attention_mask, video_mask)
+                    sim = self._similarity(seq_a, vis_a, attention_mask, video_mask, groups=G)
                     loss = loss + self.loss_fct(sim)
             return loss
 

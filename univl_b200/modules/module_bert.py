@@ -69,11 +69,12 @@ class BertOnlyMLMHead(nn.Module):
         super(BertOnlyMLMHead, self).__init__()
         self.predictions = BertLMPredictionHead(config, bert_model_embedding_weights)
 
-    def loss(self, hidden2d, labels, return_logits=False):
-        """CrossEntropy(ignore_index=-1) of the tied projection, fused (reference modeling.py:273-276)."""
+    def loss(self, hidden2d, labels, return_logits=False, groups=1):
+        """CrossEntropy(ignore_index=-1) of the tied projection, fused (reference modeling.py:273-276); groups > 1: the
+        mean over `groups` consecutive micro-batches of rows of each one's own mean."""
         t = self.predictions.transform.run(hidden2d)
         return ops.ProjXentFn.apply(t, self.predictions.decoder.weight, self.predictions.bias, labels.reshape(-1),
-                                    None, 0, True, return_logits)
+                                    None, 0, True, return_logits, groups)
 
     def logits(self, hidden2d):
         """[T, vocab] fp32 scores (inference: decoder_caption)."""

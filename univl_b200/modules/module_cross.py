@@ -51,6 +51,14 @@ class CrossEmbeddings(nn.Module):
                                     self.dropout.p, self.training)
 
 
+def _n_seq(Nt, Nv, groups):
+    """sequences of a pairing over `groups` groups (0 / False: aligned)"""
+    groups = int(groups)
+    if groups and (Nt % groups or Nv % groups):
+        raise ValueError("cross pairing: %d groups must divide %d text and %d video rows" % (groups, Nt, Nv))
+    return Nt * Nv // groups if groups else Nt
+
+
 class CrossModel(PreTrainedModel):
     """embeddings -> N fused encoder layers -> pooler (reference :355-394)."""
 
@@ -65,10 +73,11 @@ class CrossModel(PreTrainedModel):
     def encode_pairs(self, text2d, video2d, text_mask, video_mask, all_pairs, keep_all=False):
         """text2d [Nt*W, H], video2d [Nv*F, H]; sequence p = concat(text_i, video_j) with (i, j) = (p, p) or, if
         all_pairs, (p / Nv, p % Nv) — the B x B pairing of reference modeling.py:341-375 without `repeat` copies.
+        all_pairs = G > 1 pairs within G micro-batches only: G groups of (Nt/G) x (Nv/G) sequences, group after group.
         -> (hidden [n_seq*(W+F), H], n_seq, W+F)"""
         Nt, W = text_mask.shape
         Nv, F = video_mask.shape
-        n_seq = Nt * Nv if all_pairs else Nt
+        n_seq = _n_seq(Nt, Nv, all_pairs)
         x = self.embeddings.run(text2d, video2d, Nt, W, Nv, F, all_pairs)
         mask = ops.MaskSpec(text_mask, video_mask, all_pairs=all_pairs)
         return self.encoder.run(x, n_seq, W + F, mask, keep_all=keep_all), n_seq, W + F
@@ -79,7 +88,7 @@ class CrossModel(PreTrainedModel):
         the other W+F-1 tokens."""
         Nt, W = text_mask.shape
         Nv, F = video_mask.shape
-        n_seq = Nt * Nv if all_pairs else Nt
+        n_seq = _n_seq(Nt, Nv, all_pairs)
         x = self.embeddings.run(text2d, video2d, Nt, W, Nv, F, all_pairs)
         mask = ops.MaskSpec(text_mask, video_mask, all_pairs=all_pairs)
         return self.encoder.run_first_token(x, n_seq, W + F, mask), n_seq

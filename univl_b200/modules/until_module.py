@@ -136,12 +136,23 @@ class PreTrainedModel(nn.Module):
 
 
 # ---------------------------------------------------------------------------------------------------------
-# losses on the [B, B] similarity matrix
+# losses on the [B, B] similarity matrix, or on a [G, B, B] stack of one matrix per micro-batch: the mean over the G
+# group losses, each the reference loss of its own matrix (UniVL.forward(micro_batches=G))
 # ---------------------------------------------------------------------------------------------------------
+def _sim_input(sim_matrix, what, group_size=None):
+    _require_cuda(sim_matrix, what)
+    if sim_matrix.dim() == 3 and sim_matrix.shape[-1] != sim_matrix.shape[-2]:
+        raise ValueError("%s: expected [G, B, B] micro-batch similarity matrices, got %s"
+                         % (what, tuple(sim_matrix.shape)))
+    if sim_matrix.dim() == 3 and group_size is not None and sim_matrix.shape[-1] != group_size:
+        raise ValueError("%s: micro-batch similarity is %dx%d but the loss was built for batch_size * n_pair = %d"
+                         % (what, sim_matrix.shape[-1], sim_matrix.shape[-1], group_size))
+    return sim_matrix.float()
+
+
 class CrossEn(nn.Module):
     def forward(self, sim_matrix):
-        _require_cuda(sim_matrix, "CrossEn")
-        return ops.SimLossFn.apply(sim_matrix.float(), "crossen", None)
+        return ops.SimLossFn.apply(_sim_input(sim_matrix, "CrossEn"), "crossen", None)
 
 
 class MILNCELoss(nn.Module):
@@ -151,8 +162,8 @@ class MILNCELoss(nn.Module):
         self.n_pair = n_pair
 
     def forward(self, sim_matrix):
-        _require_cuda(sim_matrix, "MILNCELoss")
-        return ops.SimLossFn.apply(sim_matrix.float(), "milnce", (self.batch_size, self.n_pair))
+        sim = _sim_input(sim_matrix, "MILNCELoss", self.batch_size * self.n_pair)
+        return ops.SimLossFn.apply(sim, "milnce", (self.batch_size, self.n_pair))
 
 
 class MaxMarginRankingLoss(nn.Module):
@@ -173,6 +184,6 @@ class MaxMarginRankingLoss(nn.Module):
             self.w_same, self.w_diff = 1.0 * scale, alpha * scale
 
     def forward(self, x):
-        _require_cuda(x, "MaxMarginRankingLoss")
+        x = _sim_input(x, "MaxMarginRankingLoss", self.batch_size * self.n_pair)
         args = (self.margin, self.n_pair if self.weighted else 0, self.w_same, self.w_diff)
-        return ops.SimLossFn.apply(x.float(), "maxmargin", args)
+        return ops.SimLossFn.apply(x, "maxmargin", args)

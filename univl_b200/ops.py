@@ -143,12 +143,14 @@ def layernorm_bwd(dy, dy2, x, res, gamma, mean, rstd, p=0.0, mode=0, seed=0, str
 
 
 class MaskSpec:
-    """Key-padding description for attention: concat(mask_a[i, :Wa], mask_b[j, :Fb]); (i, j) per sequence."""
+    """Key-padding description for attention: concat(mask_a[i, :Wa], mask_b[j, :Fb]); (i, j) per sequence.
+    all_pairs: number of pairing groups (include/univl_b200.h): 0 / False = aligned (i = j = sequence), 1 / True = every
+    (i, j) pair, G = G micro-batches each pairing its own Na/G x Nb/G rows."""
 
     def __init__(self, mask_a=None, mask_b=None, all_pairs=False, causal=False):
         self.a = mask_a.contiguous() if mask_a is not None else None
         self.b = mask_b.contiguous() if mask_b is not None else None
-        self.all_pairs = bool(all_pairs)
+        self.all_pairs = int(all_pairs)
         self.causal = bool(causal)
         for m in (self.a, self.b):
             if m is not None and m.dtype != torch.int64:
@@ -533,7 +535,8 @@ class EmbedTextFn(torch.autograd.Function):
 
 class EmbedSrcFn(torch.autograd.Function):
     """activation rows + position (+ type) -> LayerNorm -> dropout; visual (module_visual.py:118-131) and cross
-    (module_cross.py:123-138) embeddings.  a: [Na*Wa, H] bf16, b: [Nb*Fb, H] bf16 or None."""
+    (module_cross.py:123-138) embeddings.  a: [Na*Wa, H] bf16, b: [Nb*Fb, H] bf16 or None.  all_pairs: pairing groups
+    as in MaskSpec (Na * Nb / G sequences for G >= 1)."""
 
     @staticmethod
     def forward(ctx, a, b, Na, Wa, Nb, Fb, all_pairs, pos, type_w, gamma, beta, p, training):
@@ -541,16 +544,17 @@ class EmbedSrcFn(torch.autograd.Function):
         H = a.shape[1]
         p = float(p) if training else 0.0
         stream = arena.next_stream()
-        n_seq = Na * Nb if (all_pairs and Fb > 0) else Na
+        all_pairs = int(all_pairs)
+        n_seq = Na * Nb // all_pairs if (all_pairs and Fb > 0) else Na
         rows = n_seq * (Wa + Fb)
         y = _empty((rows, H), BF16, a)
         mean = _empty((rows,), F32, a)
         rstd = _empty((rows,), F32, a)
         call("univl_embed_src_fwd", a.data_ptr(), ptr(b), pos.data_ptr(), ptr(type_w), gamma.data_ptr(),
-             beta.data_ptr(), y.data_ptr(), mean.data_ptr(), rstd.data_ptr(), Na, Wa, Nb, Fb, int(all_pairs), H,
+             beta.data_ptr(), y.data_ptr(), mean.data_ptr(), rstd.data_ptr(), Na, Wa, Nb, Fb, all_pairs, H,
              LN_EPS, p, arena.seed, stream)
         ctx.save_for_backward(a, b, pos, type_w, gamma, beta, mean, rstd)
-        ctx.cfg = (Na, Wa, Nb, Fb, int(all_pairs), H, p, arena.seed, stream)
+        ctx.cfg = (Na, Wa, Nb, Fb, all_pairs, H, p, arena.seed, stream)
         ctx.sink = GradSink()
         return y
 
@@ -694,25 +698,36 @@ class ProjXentFn(torch.autograd.Function):
     """loss = CrossEntropy(x W^T + bias, labels) without ever exposing logits to autograd: tied vocab projection
     (reference modules/module_bert.py:327-330) + CrossEntropyLoss(ignore_index=-1) (modeling.py:253, :275), or the MFM
     NCE (modeling.py:278-297) when `pair_mask` is given (W = all frames of the rank, diagonal targets).
-    w_is_param: W is an fp32 parameter [V, K] (bf16 copy from the arena); else W is a bf16 activation [V, K]."""
+    w_is_param: W is an fp32 parameter [V, K] (bf16 copy from the arena); else W is a bf16 activation [V, K].
+    groups: the T rows are `groups` consecutive micro-batches; the loss is the mean over groups of each group's mean.
+    Grouped NCE (target_mode 1) scores each group's rows against that group's own T / groups frames only: one
+    [T/G x T/G x K] logit GEMM per group, never the T x T matrix."""
 
     @staticmethod
-    def forward(ctx, x, W, bias, labels, pair_mask, target_mode, w_is_param, return_logits):
+    def forward(ctx, x, W, bias, labels, pair_mask, target_mode, w_is_param, return_logits, groups):
         arena = rt.current()
         w16 = arena.bf16(W) if w_is_param else W
         T, K = x.shape
-        V = w16.shape[0]
+        windowed = target_mode == 1 and groups > 1
+        if windowed and (w_is_param or w16.shape[0] != T or T % groups):
+            raise ValueError("grouped NCE needs one frame row per scored row and T divisible by the %d groups" % groups)
+        V = T // groups if windowed else w16.shape[0]
         ld = _ld_pad(V)
         logits = _empty((T, ld), F32, x)[:, :V]
-        gemm(x, w16, T, V, K, logits, epi=EPI_F32, bias=bias)
+        if windowed:
+            for g in range(groups):
+                rows = slice(g * V, (g + 1) * V)
+                gemm(x[rows], w16[rows], V, V, K, logits[rows], epi=EPI_F32, bias=bias)
+        else:
+            gemm(x, w16, T, V, K, logits, epi=EPI_F32, bias=bias)
         labels = labels.contiguous()
         lse = _empty((T,), F32, x)
-        sc = _empty((2,), F32, x)
+        sc = _empty((2 * groups,), F32, x)
         loss = _empty((), F32, x)
         call("univl_softmax_xent_fwd", logits.data_ptr(), logits.stride(0), labels.data_ptr(), ptr(pair_mask),
-             lse.data_ptr(), sc.data_ptr(), loss.data_ptr(), T, V, target_mode, -1)
+             lse.data_ptr(), sc.data_ptr(), loss.data_ptr(), T, V, target_mode, -1, groups)
         ctx.save_for_backward(x, w16, logits, labels, pair_mask, lse, sc, W if w_is_param else None, bias)
-        ctx.cfg = (target_mode, w_is_param, bias is not None)
+        ctx.cfg = (target_mode, w_is_param, bias is not None, groups, windowed)
         ctx.sink = GradSink()
         if return_logits:
             return loss, logits
@@ -721,16 +736,29 @@ class ProjXentFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g, *unused):
         x, w16, logits, labels, pair_mask, lse, sc, W, bias = ctx.saved_tensors
-        target_mode, w_is_param, has_bias = ctx.cfg
+        target_mode, w_is_param, has_bias, groups, windowed = ctx.cfg
         T, K = x.shape
-        V = w16.shape[0]
+        V = logits.shape[1]
         ld = _ld_pad(V)
         g = g.contiguous().to(F32)
         dl = _empty((T, ld), BF16, x)
         call("univl_softmax_xent_bwd", logits.data_ptr(), logits.stride(0), labels.data_ptr(), ptr(pair_mask),
-             lse.data_ptr(), sc.data_ptr(), g.data_ptr(), dl.data_ptr(), ld, T, V, target_mode, -1)
+             lse.data_ptr(), sc.data_ptr(), g.data_ptr(), dl.data_ptr(), ld, T, V, target_mode, -1, groups)
         dlv = dl[:, :V]
         dx = _empty((T, K), BF16, x)
+        if windowed:
+            dW = _empty((T, K), BF16, x)
+            tmp = _zeros((T, K), F32, x)
+            for gi in range(groups):
+                rows = slice(gi * V, (gi + 1) * V)
+                gemm(dlv[rows], w16[rows], V, K, V, dx[rows], b_mn=True)
+                gemm(dl[rows], x[rows], V, K, V, tmp[rows], epi=EPI_ATOMIC, a_mn=True, b_mn=True)
+            call("univl_cast_f32_to_bf16", tmp.data_ptr(), dW.data_ptr(), tmp.numel())
+            db = None
+            if has_bias:
+                dbbuf, db = ctx.sink.one(bias)
+                colsum(dlv, dbbuf)
+            return dx, dW, db, None, None, None, None, None, None
         gemm(dlv, w16, T, K, V, dx, b_mn=True)
         if w_is_param:
             dWbuf, dW = ctx.sink.one(W)
@@ -744,7 +772,7 @@ class ProjXentFn(torch.autograd.Function):
         if has_bias:
             dbbuf, db = ctx.sink.one(bias)
             colsum(dlv, dbbuf)
-        return dx, dW, db, None, None, None, None, None
+        return dx, dW, db, None, None, None, None, None, None
 
 
 class MeanPoolFn(torch.autograd.Function):
@@ -774,47 +802,52 @@ class MeanPoolFn(torch.autograd.Function):
 
 
 class SimMatmulFn(torch.autograd.Function):
-    """sim = T V^T (reference modules/modeling.py:389)."""
+    """sim = T V^T (reference modules/modeling.py:389); groups > 1: the block diagonal [G, Bt/G, Bv/G], one similarity
+    matrix per micro-batch."""
 
     @staticmethod
-    def forward(ctx, t, v):
-        sim = _empty((t.shape[0], v.shape[0]), F32, t)
-        call("univl_sim_matmul_fwd", t.data_ptr(), v.data_ptr(), sim.data_ptr(), t.shape[0], v.shape[0], t.shape[1])
+    def forward(ctx, t, v, groups):
+        bt, bv = t.shape[0] // groups, v.shape[0] // groups
+        sim = _empty((t.shape[0], v.shape[0]) if groups == 1 else (groups, bt, bv), F32, t)
+        call("univl_sim_matmul_fwd", t.data_ptr(), v.data_ptr(), sim.data_ptr(), bt, bv, t.shape[1], groups)
         ctx.save_for_backward(t, v)
+        ctx.groups = groups
         return sim
 
     @staticmethod
     def backward(ctx, ds):
         t, v = ctx.saved_tensors
+        G = ctx.groups
         dt = _empty(t.shape, F32, t)
         dv = _empty(v.shape, F32, t)
         ds = ds.contiguous()
         call("univl_sim_matmul_bwd", ds.data_ptr(), t.data_ptr(), v.data_ptr(), dt.data_ptr(), dv.data_ptr(),
-             t.shape[0], v.shape[0], t.shape[1])
-        return dt, dv
+             t.shape[0] // G, v.shape[0] // G, t.shape[1], G)
+        return dt, dv, None
 
 
 class SimLossFn(torch.autograd.Function):
-    """scalar loss on a square similarity matrix; kind: 'maxmargin' | 'crossen' | 'milnce'
-    (reference modules/until_module.py:182-251)."""
+    """scalar loss on a square similarity matrix [B, B], or the mean over groups of the loss of each matrix of a
+    [G, B, B] stack; kind: 'maxmargin' | 'crossen' | 'milnce' (reference modules/until_module.py:182-251)."""
 
     @staticmethod
     def forward(ctx, sim, kind, args):
         sim = sim.contiguous()
-        B = sim.shape[0]
+        B = sim.shape[-1]
+        G = sim.shape[0] if sim.dim() == 3 else 1
         loss = _empty((), F32, sim)
         dsim = _empty(sim.shape, F32, sim)
         if kind == "maxmargin":
             margin, n_pair, w_same, w_diff = args
             call("univl_maxmargin_loss", sim.data_ptr(), loss.data_ptr(), dsim.data_ptr(), B, float(margin), n_pair,
-                 float(w_same), float(w_diff))
+                 float(w_same), float(w_diff), G)
         elif kind == "crossen":
-            call("univl_crossen_loss", sim.data_ptr(), loss.data_ptr(), dsim.data_ptr(), B)
+            call("univl_crossen_loss", sim.data_ptr(), loss.data_ptr(), dsim.data_ptr(), B, G)
         elif kind == "milnce":
             bs, n_pair = args
             if bs * n_pair != B:
                 raise RuntimeError("MILNCELoss: sim matrix is %dx%d but batch_size*n_pair = %d" % (B, B, bs * n_pair))
-            call("univl_milnce_loss", sim.data_ptr(), loss.data_ptr(), dsim.data_ptr(), bs, n_pair)
+            call("univl_milnce_loss", sim.data_ptr(), loss.data_ptr(), dsim.data_ptr(), bs, n_pair, G)
         else:
             raise ValueError(kind)
         ctx.save_for_backward(dsim)
