@@ -123,6 +123,20 @@ int univl_attention_long_bwd(const void* q, long long ldq, const void* k, long l
                              int n_seq, int heads, int Sq, int Sk, int causal, float scale, float p_drop,
                              const unsigned long long* rng_state, unsigned long long stream_id, int rng_layout,
                              float* dbq, float* dbk, float* dbv, void* stream);
+/* Forward only, no dropout: the attention core of the Na x Nb sequences concat(a_i, b_j), p = i * Nb + j (all_pairs
+ * = 1 above), with Q/K/V read from per-source projections instead of per-pair copies.  Row r < Wa of sequence p reads
+ * row i * Wa + r of (qa, ka, va); row r >= Wa reads row j * Fb + (r - Wa) of (qb, kb, vb).  The cross encoder's eval
+ * similarity (modeling.py:355-373 under model.eval() / no_grad) computes its first layer's projections once per text
+ * row and once per video row and scores every pair through this entry.  Sq = Wa + Fb (every query row) or 1 (token 0
+ * only, from a_i); the context is [Na * Nb * Sq, heads * 64] as univl_attention_fwd writes it; lse is nullable.  Masks
+ * as above (both parts needed when Fb > 0); 12 heads, 0 < Wa + Fb <= 1024; row strides multiples of 8 and 16-byte
+ * aligned q/k/v.  Runs univl_attention_fwd's kernel up to 256 tokens and univl_attention_long_fwd's above, and gives
+ * the same bits as they do on the materialised per-pair q/k/v. */
+int univl_attention_pair_fwd(const void* qa, long long ldqa, const void* ka, long long ldka, const void* va,
+                             long long ldva, const void* qb, long long ldqb, const void* kb, long long ldkb,
+                             const void* vb, long long ldvb, void* o, long long ldo, float* lse,
+                             const long long* mask_a, const long long* mask_b, int Na, int Wa, int Nb, int Fb,
+                             int heads, int Sq, float scale, void* stream);
 /* ---- fused QKV projection + self-attention, forward (wgmma / TMA; module_bert.py:171-197 as ONE kernel) --------------
  * ctx[T,H] = merge_heads(dropout(softmax((x Wq^T + bq)(x Wk^T + bk)^T * scale + mask)) (x Wv^T + bv)), T = n_seq * S,
  * H = heads * 64 = 768.  wqkv: bf16 [3H, H] (query | key | value rows), bias fp32 [3H].  The [T,3H] projections and the

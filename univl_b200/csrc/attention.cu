@@ -51,9 +51,10 @@ __device__ __forceinline__ void tile_rng_rowmajor(const AttnParams& p, long long
 // ------------------------------------------------------------------------------------------------------------
 // NKB > 0: the whole score row (<= NKB 16-key blocks) stays in registers — one QK^T pass, exact softmax, 2 * NKB
 // independent accumulator chains for the tensor pipe.  NKB == 0: 16-key chunks with a stats pre-pass (any Sk <= 256).
-template <int NKB>
+// PAIR: the Q/K/V rows come from two sources (load_pair_tile; univl_attention_pair_fwd).
+template <int NKB, bool PAIR>
 __global__ void __launch_bounds__(ATT_FWD_WARPS * 32)  // (capping S=96 at 112 registers for 3 CTAs/SM measured 6% slower)
-attention_fwd_kernel(const AttnParams p_in) {
+attention_fwd_kernel(const AttnParams p_in, const PairSrc pb) {
   pdl_trigger();
   pdl_wait();
   AttnParams p = p_in;
@@ -73,9 +74,15 @@ attention_fwd_kernel(const AttnParams p_in) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
 
-  load_head_tile(sQ, p.q + (long long)seq * p.Sq * p.ldq + h * HD, p.ldq, p.Sq, Sq16);
-  load_head_tile(sK, p.k + (long long)seq * p.Sk * p.ldk + h * HD, p.ldk, p.Sk, Sk16);
-  load_head_tile(sV, p.v + (long long)seq * p.Sk * p.ldv + h * HD, p.ldv, p.Sk, Sk16);
+  if constexpr (PAIR) {
+    load_pair_tile(sQ, p.q, p.ldq, pb.q, pb.ldq, p, seq, h, 0, p.Sq, Sq16);
+    load_pair_tile(sK, p.k, p.ldk, pb.k, pb.ldk, p, seq, h, 0, p.Sk, Sk16);
+    load_pair_tile(sV, p.v, p.ldv, pb.v, pb.ldv, p, seq, h, 0, p.Sk, Sk16);
+  } else {
+    load_head_tile(sQ, p.q + (long long)seq * p.Sq * p.ldq + h * HD, p.ldq, p.Sq, Sq16);
+    load_head_tile(sK, p.k + (long long)seq * p.Sk * p.ldk + h * HD, p.ldk, p.Sk, Sk16);
+    load_head_tile(sV, p.v + (long long)seq * p.Sk * p.ldv + h * HD, p.ldv, p.Sk, Sk16);
+  }
   build_key_mask(madd, p, seq, Sk16);
   cp_async_wait_all();
   __syncthreads();
@@ -595,6 +602,39 @@ attention_bwd_kernel(const AttnParams p_in) {
   }
 }
 
+int attention_fwd_launch(const AttnParams& p, bool pair, const PairSrc& pb, cudaStream_t stream) {
+  const int Sq16 = (p.Sq + 15) & ~15, Sk16 = (p.Sk + 15) & ~15;
+  const size_t smem = (size_t)(Sq16 + 2 * Sk16) * LDS * 2 + (size_t)Sk16 * 4;
+  const int nkb = Sk16 / 16;
+  void (*kern)(const AttnParams, const PairSrc);
+  if (pair)
+    kern = nkb <= 3 ? attention_fwd_kernel<3, true>
+           : nkb <= 6 ? attention_fwd_kernel<6, true>
+           : nkb <= 8 ? attention_fwd_kernel<8, true> : attention_fwd_kernel<0, true>;
+  else
+    kern = nkb <= 3 ? attention_fwd_kernel<3, false>
+           : nkb <= 6 ? attention_fwd_kernel<6, false>
+           : nkb <= 8 ? attention_fwd_kernel<8, false> : attention_fwd_kernel<0, false>;
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "attention_fwd smem attribute: %s", cudaGetErrorString(e));
+  // warps per CTA: one per 16-row task up to 3, else two tasks per warp — smaller CTAs, more of them resident per SM, so
+  // the load phase of one overlaps the math of the others (S = 96: 3-warp CTAs measured +0.8% on the whole step)
+  const int fwd_tasks = Sq16 / 16;
+  int fwd_warps = fwd_tasks <= 3 ? fwd_tasks : (fwd_tasks + 1) / 2;
+  if (fwd_warps > ATT_FWD_WARPS) fwd_warps = ATT_FWD_WARPS;
+  {
+    static int cap = -1;  // tuning: UNIVL_ATT_FWD_WARPS=n caps the warps per CTA (more, smaller CTAs per SM)
+    if (cap < 0) {
+      const char* e = getenv("UNIVL_ATT_FWD_WARPS");
+      cap = e ? atoi(e) : 0;
+    }
+    if (cap > 0 && fwd_warps > cap) fwd_warps = cap;
+  }
+  launch_kernel(kern, dim3(p.n_seq * p.heads), dim3(fwd_warps * 32), smem, stream, p, pb);
+  UNIVL_CHECK_LAUNCH("attention_fwd");
+  return UNIVL_OK;
+}
+
 }  // namespace univl
 
 using namespace univl;
@@ -614,30 +654,7 @@ extern "C" int univl_attention_fwd(const void* q, long long ldq, const void* k, 
   UNIVL_CHECK_ARG(o != nullptr && (ldo % 2) == 0, "attention_fwd: bad output");
   if (n_seq == 0) return UNIVL_OK;
   p.o = (bf16*)o; p.ldo = ldo; p.lse = lse;
-  const int Sq16 = (Sq + 15) & ~15, Sk16 = (Sk + 15) & ~15;
-  const size_t smem = (size_t)(Sq16 + 2 * Sk16) * LDS * 2 + (size_t)Sk16 * 4;
-  const int nkb = Sk16 / 16;
-  void (*kern)(const AttnParams) = nkb <= 3 ? attention_fwd_kernel<3>
-                                   : nkb <= 6 ? attention_fwd_kernel<6>
-                                   : nkb <= 8 ? attention_fwd_kernel<8> : attention_fwd_kernel<0>;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "attention_fwd smem attribute: %s", cudaGetErrorString(e));
-  // warps per CTA: one per 16-row task up to 3, else two tasks per warp — smaller CTAs, more of them resident per SM, so
-  // the load phase of one overlaps the math of the others (S = 96: 3-warp CTAs measured +0.8% on the whole step)
-  const int fwd_tasks = Sq16 / 16;
-  int fwd_warps = fwd_tasks <= 3 ? fwd_tasks : (fwd_tasks + 1) / 2;
-  if (fwd_warps > ATT_FWD_WARPS) fwd_warps = ATT_FWD_WARPS;
-  {
-    static int cap = -1;  // tuning: UNIVL_ATT_FWD_WARPS=n caps the warps per CTA (more, smaller CTAs per SM)
-    if (cap < 0) {
-      const char* e = getenv("UNIVL_ATT_FWD_WARPS");
-      cap = e ? atoi(e) : 0;
-    }
-    if (cap > 0 && fwd_warps > cap) fwd_warps = cap;
-  }
-  launch_kernel(kern, dim3(n_seq * heads), dim3(fwd_warps * 32), smem, (cudaStream_t)stream, p);
-  UNIVL_CHECK_LAUNCH("attention_fwd");
-  return UNIVL_OK;
+  return attention_fwd_launch(p, false, PairSrc{}, (cudaStream_t)stream);
 }
 
 extern "C" int univl_attention_bwd(const void* q, long long ldq, const void* k, long long ldk, const void* v,

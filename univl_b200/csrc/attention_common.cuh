@@ -37,6 +37,13 @@ struct AttnParams {
   float *dbq, *dbk, *dbv;  // backward, optional: projection-bias gradients += column sums of dq / dk / dv  [heads*64]
 };
 
+// The pair forward's second source (univl_attention_pair_fwd): its q/k/v projections, read for sequence rows >= Wa.  A
+// kernel argument of its own, so AttnParams and the kernels that do not read it keep their layout.
+struct PairSrc {
+  const bf16 *q, *k, *v;
+  long long ldq, ldk, ldv;
+};
+
 __device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
                : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
@@ -61,6 +68,24 @@ __device__ __forceinline__ void load_head_tile(bf16* dst, const bf16* src, long 
     const int r = idx >> 3, c = idx & 7;
     bf16* d = dst + r * LDS + c * 8;
     if (r < rows) cp_async16(d, src + (long long)r * ld + c * 8);
+    else *reinterpret_cast<uint4*>(d) = make_uint4(0, 0, 0, 0);
+  }
+}
+
+// load_head_tile for the pair forward: rows [r0, r0 + rows) of sequence `seq` = concat(text i, video j) (all-pairs
+// pairing), whose row s is row i * Wa + s of the first source a (s < Wa) or row j * Fb + s - Wa of the second source b.
+// a / b point at column 0 of the q, k or v projections of each source.
+__device__ __forceinline__ void load_pair_tile(bf16* dst, const bf16* a, long long lda, const bf16* b, long long ldb,
+                                               const AttnParams& p, int seq, int h, int r0, int rows, int rows16) {
+  long long i, j;
+  pair_sources(seq, 1, p.n_seq, p.Nb, i, j);
+  const bf16* ra = a + i * p.Wa * lda + h * HD;
+  const bf16* rb = b + j * p.Fb * ldb + h * HD;
+  for (int idx = threadIdx.x; idx < rows16 * 8; idx += blockDim.x) {
+    const int r = idx >> 3, c = idx & 7;
+    const int s = r0 + r;
+    bf16* d = dst + r * LDS + c * 8;
+    if (r < rows) cp_async16(d, (s < p.Wa ? ra + (long long)s * lda : rb + (long long)(s - p.Wa) * ldb) + c * 8);
     else *reinterpret_cast<uint4*>(d) = make_uint4(0, 0, 0, 0);
   }
 }
@@ -177,5 +202,11 @@ static inline int fill_common(AttnParams& p, const void* q, long long ldq, const
   p.seed = 0; p.stream = stream_id; p.rng = rng_state;
   return UNIVL_OK;
 }
+
+// Launch the forward kernels for a filled AttnParams (o, lse and the shape set, n_seq > 0).  pair: read Q/K/V through
+// load_pair_tile from p's q/k/v and pb (univl_attention_pair_fwd); pb is ignored otherwise.
+// attention.cu: Sq, Sk <= 256; attention_long.cu: Sq, Sk <= 1024 and 12 heads.
+int attention_fwd_launch(const AttnParams& p, bool pair, const PairSrc& pb, cudaStream_t stream);
+int attention_long_fwd_launch(const AttnParams& p, bool pair, const PairSrc& pb, cudaStream_t stream);
 
 }  // namespace univl

@@ -69,10 +69,12 @@ __device__ __forceinline__ void write_partial_row(const float* slots, int nwarps
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// forward
+// forward (PAIR: the Q/K/V rows come from two sources through load_pair_tile, univl_attention_pair_fwd; a key tile
+// may straddle the boundary between them)
 // ------------------------------------------------------------------------------------------------------------
+template <bool PAIR>
 __global__ void __launch_bounds__(LONG_WARPS * 32)
-attention_long_fwd_kernel(const AttnParams p_in) {
+attention_long_fwd_kernel(const AttnParams p_in, const PairSrc pb) {
   pdl_trigger();
   pdl_wait();
   AttnParams p = p_in;
@@ -94,10 +96,16 @@ attention_long_fwd_kernel(const AttnParams p_in) {
   auto load_kv = [&](int tile, int stage) {
     const int k0 = tile * LT;
     bf16* sK = sKV + stage * 2 * LT * LDS;
-    load_head_tile(sK, p.k + ((long long)seq * p.Sk + k0) * p.ldk + h * HD, p.ldk, min(LT, p.Sk - k0), LT);
-    load_head_tile(sK + LT * LDS, p.v + ((long long)seq * p.Sk + k0) * p.ldv + h * HD, p.ldv, min(LT, p.Sk - k0), LT);
+    if constexpr (PAIR) {
+      load_pair_tile(sK, p.k, p.ldk, pb.k, pb.ldk, p, seq, h, k0, min(LT, p.Sk - k0), LT);
+      load_pair_tile(sK + LT * LDS, p.v, p.ldv, pb.v, pb.ldv, p, seq, h, k0, min(LT, p.Sk - k0), LT);
+    } else {
+      load_head_tile(sK, p.k + ((long long)seq * p.Sk + k0) * p.ldk + h * HD, p.ldk, min(LT, p.Sk - k0), LT);
+      load_head_tile(sK + LT * LDS, p.v + ((long long)seq * p.Sk + k0) * p.ldv + h * HD, p.ldv, min(LT, p.Sk - k0), LT);
+    }
   };
-  load_head_tile(sQ, p.q + ((long long)seq * p.Sq + qbase) * p.ldq + h * HD, p.ldq, qrows, qrows16);
+  if constexpr (PAIR) load_pair_tile(sQ, p.q, p.ldq, pb.q, pb.ldq, p, seq, h, qbase, qrows, qrows16);
+  else load_head_tile(sQ, p.q + ((long long)seq * p.Sq + qbase) * p.ldq + h * HD, p.ldq, qrows, qrows16);
   build_key_mask(madd, p, seq, Sk16);
   load_kv(0, 0);
   cp_async_commit();
@@ -503,6 +511,19 @@ attention_long_bwd_dkdv_kernel(const AttnParams p_in, const float* __restrict__ 
   }
 }
 
+int attention_long_fwd_launch(const AttnParams& p, bool pair, const PairSrc& pb, cudaStream_t stream) {
+  const int Sq16 = (p.Sq + 15) & ~15, Sk16 = (p.Sk + 15) & ~15;
+  const size_t smem = (size_t)(LB + 4 * LT) * LDS * 2 + (size_t)Sk16 * 4;
+  void (*kern)(const AttnParams, const PairSrc) =
+      pair ? attention_long_fwd_kernel<true> : attention_long_fwd_kernel<false>;
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "attention_long_fwd smem attribute: %s", cudaGetErrorString(e));
+  const int warps = Sq16 / 16 < LONG_WARPS ? Sq16 / 16 : LONG_WARPS;
+  launch_kernel(kern, dim3(p.n_seq * p.heads, (Sq16 + LB - 1) / LB), dim3(warps * 32), smem, stream, p, pb);
+  UNIVL_CHECK_LAUNCH("attention_long_fwd");
+  return UNIVL_OK;
+}
+
 }  // namespace univl
 
 using namespace univl;
@@ -521,15 +542,7 @@ extern "C" int univl_attention_long_fwd(const void* q, long long ldq, const void
   UNIVL_CHECK_ARG(o != nullptr && (ldo % 2) == 0, "attention_long_fwd: bad output");
   if (n_seq == 0) return UNIVL_OK;
   p.o = (bf16*)o; p.ldo = ldo; p.lse = lse;
-  const int Sq16 = (Sq + 15) & ~15, Sk16 = (Sk + 15) & ~15;
-  const size_t smem = (size_t)(LB + 4 * LT) * LDS * 2 + (size_t)Sk16 * 4;
-  cudaError_t e = cudaFuncSetAttribute(attention_long_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "attention_long_fwd smem attribute: %s", cudaGetErrorString(e));
-  const int warps = Sq16 / 16 < LONG_WARPS ? Sq16 / 16 : LONG_WARPS;
-  launch_kernel(attention_long_fwd_kernel, dim3(n_seq * heads, (Sq16 + LB - 1) / LB), dim3(warps * 32), smem,
-                (cudaStream_t)stream, p);
-  UNIVL_CHECK_LAUNCH("attention_long_fwd");
-  return UNIVL_OK;
+  return attention_long_fwd_launch(p, false, PairSrc{}, (cudaStream_t)stream);
 }
 
 // As univl_attention_bwd, for 0 < Sq, Sk <= 1024, 12 heads and rng_layout 0 (the forward was univl_attention_long_fwd

@@ -1,0 +1,47 @@
+// univl_b200 — attention core over (text, video) pair sequences, Q/K/V rows read from per-source projections.
+//
+// In evaluation (no dropout) the first cross layer's Q/K/V projections act on each token alone, and the token's input
+// (the CrossEmbeddings LayerNorm of text i's or video j's row) does not depend on the pair.  So the projections are
+// computed once per source row, and this entry reads them in place: sequence p = i * Nb + j (the all-pairs pairing of
+// common.cuh pair_sources) takes rows r < Wa from the text source at row i * Wa + r and rows r >= Wa from the video
+// source at row j * Fb + r - Wa.  The kernels are attention.cu's (S <= 256) and attention_long.cu's (S <= 1024) forward
+// kernels with the pair row addressing (load_pair_tile) as a compile-time variant, so the context equals that of
+// univl_attention_fwd / univl_attention_long_fwd on the materialised per-pair q/k/v bit for bit.
+#include <climits>
+
+#include "attention_common.cuh"
+
+using namespace univl;
+
+extern "C" int univl_attention_pair_fwd(const void* qa, long long ldqa, const void* ka, long long ldka, const void* va,
+                                        long long ldva, const void* qb, long long ldqb, const void* kb, long long ldkb,
+                                        const void* vb, long long ldvb, void* o, long long ldo, float* lse,
+                                        const long long* mask_a, const long long* mask_b, int Na, int Wa, int Nb,
+                                        int Fb, int heads, int Sq, float scale, void* stream) {
+  UNIVL_CHECK_ARG(Na >= 0 && Wa > 0 && Nb > 0 && Fb >= 0,
+                  "attention_pair_fwd: bad source shape Na=%d Wa=%d Nb=%d Fb=%d", Na, Wa, Nb, Fb);
+  UNIVL_CHECK_ARG(heads == 12, "attention_pair_fwd: heads must be 12 (got %d)", heads);
+  const int S = Wa + Fb;
+  UNIVL_CHECK_ARG(Sq == 1 || Sq == S, "attention_pair_fwd: Sq must be 1 or Wa + Fb = %d (got %d)", S, Sq);
+  UNIVL_CHECK_ARG((long long)Na * Nb * heads <= INT_MAX, "attention_pair_fwd: too many pairs (%d x %d)", Na, Nb);
+  UNIVL_CHECK_ARG(Fb == 0 || (mask_a != nullptr && mask_b != nullptr),
+                  "attention_pair_fwd: both mask parts are needed when Fb > 0");
+  if (Fb > 0) {
+    UNIVL_CHECK_ARG(qb && kb && vb, "attention_pair_fwd: null second-source q/k/v");
+    UNIVL_CHECK_ARG((ldqb % 8) == 0 && (ldkb % 8) == 0 && (ldvb % 8) == 0,
+                    "attention_pair_fwd: second-source row strides must be multiples of 8");
+    UNIVL_CHECK_ARG(((uintptr_t)qb & 15) == 0 && ((uintptr_t)kb & 15) == 0 && ((uintptr_t)vb & 15) == 0,
+                    "attention_pair_fwd: second-source q/k/v must be 16-byte aligned");
+  }
+  const int n_seq = Na * Nb;
+  AttnParams p = {};
+  if (int rc = fill_common(p, qa, ldqa, ka, ldka, va, ldva, mask_a, mask_b, Wa, Fb, Nb, 1, n_seq, heads, Sq, S, 0,
+                           scale, 0.f, nullptr, 0, 1024))
+    return rc;
+  UNIVL_CHECK_ARG(o != nullptr && (ldo % 2) == 0, "attention_pair_fwd: bad output");
+  if (n_seq == 0) return UNIVL_OK;
+  const PairSrc pb{(const bf16*)qb, (const bf16*)kb, (const bf16*)vb, ldqb, ldkb, ldvb};
+  p.o = (bf16*)o; p.ldo = ldo; p.lse = lse;
+  if (S <= 256) return attention_fwd_launch(p, true, pb, (cudaStream_t)stream);
+  return attention_long_fwd_launch(p, true, pb, (cudaStream_t)stream);
+}

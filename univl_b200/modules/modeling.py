@@ -7,6 +7,7 @@ drivers (main_task_retrieval.py / main_task_caption.py / main_pretrain.py) load 
 observe: hidden states are bf16 (the kernels' activation type); everything needs a CUDA device; there is no CPU path.
 """
 import logging
+import math
 
 import torch
 from torch import nn
@@ -20,6 +21,12 @@ from .module_visual import VisualConfig, VisualModel, VisualOnlyMLMHead
 from .until_module import CrossEn, LayerNorm, MaxMarginRankingLoss, MILNCELoss, PreTrainedModel
 
 logger = logging.getLogger(__name__)
+
+# Pair tokens (pairs x (W + F)) per tile of the cross-encoder similarity in evaluation (UniVL._cross_similarity_eval).
+# A tile's memory grows linearly with it.  At this value, W = F = 48 and two cross layers, a tile's peak was 5.2 GiB of
+# torch allocations (measured on an H100 80GB HBM3 at a 400 W power limit, scripts/bench_retrieval_eval.py); the eval
+# path draws no stream-ordered kernel scratch.
+EVAL_PAIR_TOKENS = 1 << 18
 
 
 class UniVLPreTrainedModel(PreTrainedModel, nn.Module):
@@ -95,6 +102,15 @@ def check_attr(target_name, task_config):
 
 def _flat(t):
     return t.reshape(-1, t.shape[-1]).contiguous()
+
+
+def _eval_tile(Nt, Nv, S, budget):
+    """(text rows, video rows) of one tile of the eval similarity: about square, at most `budget` pair tokens (at
+    least one pair)"""
+    pairs = max(1, budget // S)
+    bv = min(Nv, max(1, math.isqrt(pairs)))
+    bt = min(Nt, max(1, pairs // bv))
+    return bt, min(Nv, max(1, pairs // bt))
 
 
 class UniVL(UniVLPreTrainedModel):
@@ -192,8 +208,15 @@ class UniVL(UniVLPreTrainedModel):
     def _cross_similarity(self, seq2d, vis2d, attention_mask, video_mask, groups=1):
         """reference :341-375: every (text i, video j) pair through the cross encoder -> pooled -> similarity_dense.
         The reference walks text rows in chunks of 5 and `repeat`s both sides; here all B_t x B_v sequences go
-        through the layer kernels in one batch and the embedding kernel reads the un-repeated sources.  groups > 1:
+        through the layer kernels in one batch and the embedding kernel reads the un-repeated sources, except in
+        evaluation without gradients, which scores them in bounded tiles (_cross_similarity_eval).  groups > 1:
         only the pairs inside each micro-batch, G * Bg^2 sequences -> [G, Bg, Bg]."""
+        if groups == 1 and not self.training and not torch.is_grad_enabled():
+            return self._cross_similarity_eval(seq2d, vis2d, attention_mask, video_mask)
+        return self._cross_similarity_all_pairs(seq2d, vis2d, attention_mask, video_mask, groups)
+
+    def _cross_similarity_all_pairs(self, seq2d, vis2d, attention_mask, video_mask, groups=1):
+        """_cross_similarity as one batch of all the pair sequences (training, and any call with gradients)"""
         bt, bv = attention_mask.shape[0], video_mask.shape[0]
         # only token 0 of the last cross layer feeds the pooler: the last layer computes just those rows
         first, n_seq = self.cross.encode_pairs_first_token(seq2d, vis2d, attention_mask, video_mask, groups)
@@ -202,6 +225,31 @@ class UniVL(UniVLPreTrainedModel):
         if groups > 1:
             return logits.view(groups, bt // groups, bv // groups)
         return logits.view(bt, bv)
+
+    def _cross_similarity_eval(self, seq2d, vis2d, attention_mask, video_mask):
+        """_cross_similarity in evaluation (model.eval() under torch.no_grad(), as the reference's eval_epoch calls
+        it), in memory bounded by EVAL_PAIR_TOKENS whatever the batch: the Nt x Nv pairs are scored in tiles of
+        (text block x video block) into one fp32 [Nt, Nv] result.  With dropout off, the first cross layer's Q/K/V
+        projections of a pair's token depend on its text or video row alone, so they are computed once per source row
+        (CrossModel.first_layer_source_qkv) and every tile reads them in place.  Every other stage is row- or
+        sequence-local, so a pair's logit does not depend on the tiling."""
+        Nt, W = attention_mask.shape
+        Nv, F = video_mask.shape
+        qkv = self.cross.first_layer_source_qkv(seq2d, vis2d, Nt, W, Nv, F)
+        qkv_t, qkv_v = qkv[:Nt * W], qkv[Nt * W:]
+        logits = torch.empty((Nt, Nv), dtype=torch.float32, device=seq2d.device)
+        bt, bv = _eval_tile(Nt, Nv, W + F, EVAL_PAIR_TOKENS)
+        for t0 in range(0, Nt, bt):
+            t1 = min(Nt, t0 + bt)
+            for v0 in range(0, Nv, bv):
+                v1 = min(Nv, v0 + bv)
+                first = self.cross.encode_pairs_first_token_eval(
+                    seq2d[t0 * W:t1 * W], vis2d[v0 * F:v1 * F], attention_mask[t0:t1], video_mask[v0:v1],
+                    qkv_t[t0 * W:t1 * W], qkv_v[v0 * F:v1 * F])
+                u = self.cross.pooler.pre_activation(first, (t1 - t0) * (v1 - v0), 1)
+                tile = ops.PoolerSimFn.apply(u, self.similarity_dense.weight, self.similarity_dense.bias)
+                logits[t0:t1, v0:v1] = tile.view(t1 - t0, v1 - v0)
+        return logits
 
     def _mean_pool_similarity(self, seq2d, vis2d, attention_mask, video_mask, groups=1):
         """reference :327-339 and :385-389; groups > 1: the block diagonal [G, Bg, Bg]"""

@@ -7,7 +7,7 @@ from torch import nn
 
 from .. import ops
 from .. import runtime as rt
-from .transformer import EncoderStack, Pooler, check_config, hidden_list
+from .transformer import EncoderStack, Pooler, _layer_params, check_config, hidden_list
 from .until_config import PretrainedConfig
 from .until_module import LayerNorm, PreTrainedModel
 
@@ -92,6 +92,36 @@ class CrossModel(PreTrainedModel):
         x = self.embeddings.run(text2d, video2d, Nt, W, Nv, F, all_pairs)
         mask = ops.MaskSpec(text_mask, video_mask, all_pairs=all_pairs)
         return self.encoder.run_first_token(x, n_seq, W + F, mask), n_seq
+
+    def first_layer_source_qkv(self, text2d, video2d, Nt, W, Nv, F):
+        """Evaluation only: the first layer's Q/K/V projections of every text row and every video row, once per source
+        row -> [Nt*W + Nv*F, 3H], text rows first.  With dropout off, a pair's first-layer input row is the embedding
+        LayerNorm of its text or video row alone (position and type rows are the same for every pair), so these are
+        the projections every pair sequence would compute for itself."""
+        emb = self.embeddings
+        pos, typ = emb.position_embeddings.weight, emb.token_type_embeddings.weight
+        gamma, beta = emb.LayerNorm.weight, emb.LayerNorm.bias
+        rows_t = Nt * W
+        x = torch.empty((rows_t + Nv * F, text2d.shape[1]), dtype=torch.bfloat16, device=text2d.device)
+        ops.embed_src_rows_eval(text2d, Nt, W, pos, typ, gamma, beta, x[:rows_t])
+        ops.embed_src_rows_eval(video2d, Nv, F, pos[W:], typ[1:], gamma, beta, x[rows_t:])  # video rows: s >= W, type 1
+        a = self.encoder.layer[0].attention.self
+        wqkv = rt.current().bf16_qkv(a.query.weight, a.key.weight, a.value.weight)
+        return ops.linear_fwd(x, wqkv, rt.packed_bias(a.query.bias, a.key.bias, a.value.bias))
+
+    def encode_pairs_first_token_eval(self, text2d, video2d, text_mask, video_mask, qkv_t, qkv_v):
+        """encode_pairs_first_token over all Nt x Nv pairs in evaluation, with the first layer's Q/K/V projections read
+        from qkv_t [Nt*W, 3H] and qkv_v [Nv*F, 3H] (rows of first_layer_source_qkv) -> [Nt*Nv, H]"""
+        Nt, W = text_mask.shape
+        Nv, F = video_mask.shape
+        S = W + F
+        x = self.embeddings.run(text2d, video2d, Nt, W, Nv, F, 1)  # the first layer's residual input
+        mask = ops.MaskSpec(text_mask, video_mask, all_pairs=1)
+        layers = self.encoder.layer
+        x = ops.pair_layer_eval(x, qkv_t, qkv_v, Nt, Nv, S, mask, _layer_params(layers[0]), len(layers) == 1)
+        if len(layers) == 1:
+            return x
+        return self.encoder.run_first_token(x, Nt * Nv, S, mask, start=1)
 
     def forward(self, concat_input, concat_type=None, attention_mask=None, output_all_encoded_layers=True):
         """API-parity entry: `concat_type` must be the reference's layout (0s for the text part then 1s)."""

@@ -127,10 +127,11 @@ class EncoderStack(nn.Module):
                 outs.append(x2d)
         return outs if keep_all else x2d
 
-    def run_first_token(self, x2d, n_seq, S, mask):
+    def run_first_token(self, x2d, n_seq, S, mask, start=0):
         """-> [n_seq, H]: token 0 of the last layer's output, for consumers that read nothing else (pooler).  All layers
-        but the last run in full; the last one computes only what token 0 needs (ops.EncoderLayerClsFn)."""
-        for layer in self.layer[:-1]:
+        but the last run in full; the last one computes only what token 0 needs (ops.EncoderLayerClsFn).  start: x2d
+        is the output of layer start - 1 (the layers before it ran elsewhere)."""
+        for layer in self.layer[start:-1]:
             x2d = layer.run(x2d, n_seq, S, mask)
         last = self.layer[-1]
         return ops.EncoderLayerClsFn.apply(x2d, n_seq, S, mask, last.attention.output.dropout.p,

@@ -237,6 +237,49 @@ def attention_bwd(q, k, v, o, lse, d_o, dq, dk, dv, n_seq, Sq, Sk, mask, p=0.0, 
          stream, int(rng_layout), ptr(dbq), ptr(dbk), ptr(dbv))
 
 
+def attention_pair_fwd(qkv_a, qkv_b, Na, Nb, Sq, mask):
+    """Attention core of the Na x Nb sequences concat(a_i, b_j), p = i * Nb + j, reading Q/K/V from per-source
+    projections (csrc/attention_pair.cu): qkv_a [Na*Wa, 3H] and qkv_b [Nb*Fb, 3H] hold q | k | v of every source row.
+    Sq = Wa + Fb, or 1 for token 0 only.  No dropout.  -> ctx [Na*Nb*Sq, H]"""
+    H = HEADS * 64
+    o = _empty((Na * Nb * Sq, H), BF16, qkv_a)
+    call("univl_attention_pair_fwd", qkv_a.data_ptr(), qkv_a.stride(0), qkv_a[:, H:].data_ptr(), qkv_a.stride(0),
+         qkv_a[:, 2 * H:].data_ptr(), qkv_a.stride(0), qkv_b.data_ptr(), qkv_b.stride(0), qkv_b[:, H:].data_ptr(),
+         qkv_b.stride(0), qkv_b[:, 2 * H:].data_ptr(), qkv_b.stride(0), o.data_ptr(), o.stride(0), None, ptr(mask.a),
+         ptr(mask.b), Na, mask.Wa, Nb, mask.Fb, HEADS, Sq, 1.0 / math.sqrt(64.0))
+    return o
+
+
+def embed_src_rows_eval(a, N, W, pos, type_w, gamma, beta, out):
+    """LayerNorm(a + pos[s] + type[0]) of every row of one source alone (aligned univl_embed_src_fwd, no dropout) into
+    out [N*W, H].  With pos / type_w offset by the rows that precede the source in the pair sequence, these are exactly
+    the source's rows of the all-pairs embedding, since that LayerNorm reads the row alone."""
+    mean = _empty((N * W,), F32, a)
+    rstd = _empty((N * W,), F32, a)
+    call("univl_embed_src_fwd", a.data_ptr(), None, pos.data_ptr(), type_w.data_ptr(), gamma.data_ptr(),
+         beta.data_ptr(), out.data_ptr(), mean.data_ptr(), rstd.data_ptr(), N, W, 0, 0, 0, a.shape[1], LN_EPS, 0.0,
+         None, 0)
+    return out
+
+
+def pair_layer_eval(x, qkv_a, qkv_b, Na, Nb, S, mask, params, first_token):
+    """An encoder layer over the Na x Nb pair sequences in evaluation (no dropout, no autograd) whose Q/K/V
+    projections are given per source row, computed once per text row and once per video row instead of once per pair.
+    x: the pair inputs [Na*Nb*S, H] (the residual of the attention block); params as EncoderLayerFn.  first_token: the
+    layer is the stack's last and produces token 0 of every sequence only, as EncoderLayerClsFn -> [Na*Nb, H].
+    Same arithmetic as EncoderLayerFn / EncoderLayerClsFn on the QKV-GEMM + attention-core path."""
+    arena = rt.current()
+    wa = dict(zip(ATT_KEYS, params[:10]))
+    wf = dict(zip(FFN_KEYS, params[10:16]))
+    drop = _Drop(0.0, 0.0, False)
+    n_seq = Na * Nb
+    ctx = attention_pair_fwd(qkv_a, qkv_b, Na, Nb, 1 if first_token else S, mask)
+    xq = x.view(n_seq, S, -1)[:, 0].contiguous() if first_token else x
+    ao = linear_fwd(ctx, arena.bf16(wa["o"]), wa["bo"])
+    y, _, _ = layernorm_fwd(ao, xq, wa["gamma"], wa["beta"], 0.0, 1, drop.seed, drop.stream())
+    return ffn_block_fwd(y, wf, drop)[0]
+
+
 # ---------------------------------------------------------------------------------------------------------
 # transformer blocks (forward keeps a dict of saved tensors; backward consumes it)
 # ---------------------------------------------------------------------------------------------------------
