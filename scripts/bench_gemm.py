@@ -1,4 +1,4 @@
-"""Time every GEMM of one FT-Align cross-encoder layer, and the 1536-row text / visual GEMMs, through ops.gemm.
+"""Time every GEMM of the FT-Align cross encoder, and the 1536-row text / visual GEMMs, through ops.gemm.
 
 Each row is one GEMM as ops.py issues it (attn_block_fwd / attn_block_bwd / ffn_block_fwd / ffn_block_bwd): its
 operand majors, epilogue, bias, aux_in / aux_out and automatic tile-width / split-K plan.  The FT-Align cross encoder
@@ -52,6 +52,10 @@ CROSS = {
     "cross_attn_out_dgrad": (T_CROSS, "dgrad", H, H, ops.EPI_BIAS, False),
     "cross_qkv_wgrad": (T_CROSS, "wgrad", 3 * H, H, ops.EPI_ATOMIC, False),
     "cross_qkv_dgrad_add": (T_CROSS, "dgrad", 3 * H, H, ops.EPI_ADD, False),
+    # the first-token cross layer (layer 2) projects K / V of all T rows (its queries are one row per pair)
+    "cross2_kv_fwd": (T_CROSS, "fwd", 2 * H, H, ops.EPI_BIAS, True),
+    "cross2_kv_dgrad": (T_CROSS, "dgrad", 2 * H, H, ops.EPI_BIAS, False),
+    "cross2_kv_wgrad": (T_CROSS, "wgrad", 2 * H, H, ops.EPI_ATOMIC, False),
 }
 TEXT = {
     "text_qkv_fwd": (T_TEXT, "fwd", 3 * H, H, ops.EPI_BIAS, True),

@@ -336,6 +336,10 @@ __device__ __forceinline__ void regs_alloc() {
 __device__ __forceinline__ void named_bar(int id, int count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
+// arrive on a named barrier without waiting: releases the threads that bar.sync on it (count includes both)
+__device__ __forceinline__ void named_bar_arrive(int id, int count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
 
 // Shared-memory matrix descriptor of a 128B-swizzled operand (sm_90 GmmaDescriptor): start address, leading / stride
 // byte offsets in 16-byte units, layout type 1 = SWIZZLE_128B.  K-major: SBO = 1024 (8 rows of 128 B), LBO unused.

@@ -12,10 +12,19 @@
 //
 // Structure (per CTA, 384 threads, 128 x BLOCK_N output tiles, optional split-K):
 //   warpgroup 0      TMA producer : one thread streams 2D boxes (128B swizzle) into a STAGES-deep mbarrier ring
-//   warpgroups 1, 2  consumers    : each owns 64 rows of the tile, issues m64 x BLOCK_N x k16 wgmma on the shared stage
-//                                   and runs the fused epilogue straight from its accumulator registers
+//   warpgroups 1, 2  consumers    : issue wgmma on the stage and run the fused epilogue straight from their
+//                                   accumulator registers, in one of two schedules chosen by the tile width:
+//     BLOCK_N = 256       cooperative: both warpgroups work on every tile, each on 64 of its 128 rows
+//                         (m64 x 256 x k16 per k16 step); the tensor cores idle while the two run the epilogue.
+//     BLOCK_N = 64 / 128  ping-pong: each warpgroup owns whole tiles, the two alternating the CTA's tiles, and issues
+//                         two m64 x BLOCK_N x k16 wgmma per k16 step (rows 0-63 and 64-127).  A pair of named barriers
+//                         hands the tensor cores from one warpgroup's mainloop to the other's in tile order, so one
+//                         warpgroup's epilogue runs while the other's MMAs do.  (256 accumulator floats per warpgroup
+//                         would not fit in registers, so the 256-wide tile stays cooperative.)
 // grid = min(#work items, #SMs); each CTA walks work items round-robin in the order decode_work() defines, and the
-// producer's ring runs continuously across tiles, so the next tile's operands load while the epilogue runs.
+// producer's ring runs continuously across tiles, so the next tile's operands load while the epilogue runs.  Both
+// schedules give every output element the same chain of k16 wgmmas in the same k order and the same epilogue, so the
+// tile width does not change a bit of the result.
 #include "common.cuh"
 #include "tmap.cuh"
 #include "wgmma.cuh"
@@ -46,6 +55,7 @@ struct GemmParams {
   bf16* aux_out;
   long long ld_aux_out;
   int vec2;  // 1 = every epilogue operand takes 2-element vector accesses (aligned base, even leading dimension)
+  int vec8;  // 1 = the bf16 outputs (out, aux_out) take 16-byte stores of 8 columns (16-byte aligned base, ld % 8 == 0)
   float* part;  // EPI_ATOMIC_F32 with split-K: [splits][M][N] partial sums, else null
 };
 
@@ -174,25 +184,61 @@ __device__ __forceinline__ void epi_pair(const GemmParams& p, int split, int row
 // flight; every instance compiles without spills under regs_alloc<232> (check with -Xptxas -v when changing it)
 constexpr int EPI_CHUNK = 8;
 
+// 4 x 4 transpose of 32-bit words across the four lanes of a quad (q = lane % 4): on entry w[k] is this lane's word of
+// 8-column group k (columns 2 q, 2 q + 1 of the group); on return the four words of group q, word k from lane k, which
+// is the group's 8 columns in order.  Two butterfly stages; the whole warp must call it.
+__device__ __forceinline__ uint4 quad_transpose(uint32_t w0, uint32_t w1, uint32_t w2, uint32_t w3, int q) {
+  const bool odd = q & 1;
+  uint32_t r0 = __shfl_xor_sync(0xffffffffu, odd ? w0 : w1, 1);
+  uint32_t r1 = __shfl_xor_sync(0xffffffffu, odd ? w2 : w3, 1);
+  if (odd) {
+    w0 = r0;
+    w2 = r1;
+  } else {
+    w1 = r0;
+    w3 = r1;
+  }
+  const bool hi = q & 2;
+  r0 = __shfl_xor_sync(0xffffffffu, hi ? w0 : w2, 2);
+  r1 = __shfl_xor_sync(0xffffffffu, hi ? w1 : w3, 2);
+  if (hi) {
+    w0 = r0;
+    w1 = r1;
+  } else {
+    w2 = r0;
+    w3 = r1;
+  }
+  return make_uint4(w0, w1, w2, w3);
+}
+
 // Unchecked epilogue of a work item whose 128 x BLOCK_N tile lies wholly inside M x N, with p.vec2 set (and, for
 // split-K partials, N even): no bounds checks, every access a 2-element vector.  The epilogue is a template argument,
 // so the fragment walk is straight-line code.  It runs in chunks of EPI_CHUNK 8-column groups.  Each chunk's global
 // loads (bias, aux_in, the accumulated output) are issued together, and before the previous chunk's arithmetic, so
 // their latencies overlap each other and that arithmetic instead of adding up.  Loading ahead of the previous chunk's
-// stores is safe for the exact in-place use epi_pair allows (aux_in == out, same leading dimension): each element is
-// read and written by the same thread, and a chunk's loads never touch the elements of an earlier chunk.
+// stores is safe for the exact in-place use epi_pair allows (aux_in == out, same leading dimension): a chunk's loads
+// never touch the elements of an earlier chunk, and within a chunk every element's load is consumed by the arithmetic
+// before its result is stored (by the same thread, or with WIDE by a lane of the same quad after the shuffles).
 // It computes exactly what epi_pair computes: the same fp32 operations in the same order, with __fmul_rn / __fadd_rn
 // so that alpha * acc and the add after it stay two roundings and are not contracted to an FFMA.
 // BIAS: p.bias is set (bias epilogues); PART: p.part is set (EPI_ATOMIC_F32 with split-K).
-template <int EPI, bool BIAS, bool PART, int BLOCK_N>
+// WIDE (p.vec8, bf16 outputs): the four lanes of a quad, which hold 2 columns each of the same 8-column groups,
+// exchange their packed results (quad_transpose) so that each lane stores one group whole, 16 bytes.  A warp's store
+// then covers 64 contiguous bytes (two full 32-byte sectors) of each of its 8 rows, with a quarter of the store
+// instructions, where the 4-byte stores cover 16 bytes (half a sector) of each row.
+template <int EPI, bool BIAS, bool PART, int BLOCK_N, bool WIDE = false>
 __device__ __forceinline__ void epi_tile(const GemmParams& p, int split, int row, int col0,
                                          const float (&acc)[BLOCK_N / 2]) {
   constexpr int GROUPS = BLOCK_N / 8;
-  constexpr int CHUNK = GROUPS < EPI_CHUNK ? GROUPS : EPI_CHUNK;
+  // WIDE holds a quad's results for the shuffles: half-size chunks keep the 256-wide tile free of spills
+  constexpr int CHUNK = WIDE ? 4 : (GROUPS < EPI_CHUNK ? GROUPS : EPI_CHUNK);
+  static_assert(CHUNK % 4 == 0, "a chunk holds whole quads of 8-column groups");
   constexpr bool AUX = EPI == EPI_GELU_BWD_BF16 || EPI == EPI_ADD_BF16;
   constexpr bool OUT_F32 = EPI == EPI_BIAS_F32 || EPI == EPI_ATOMIC_F32;
+  static_assert(!(WIDE && OUT_F32), "16-byte stores are for the bf16 outputs");
   constexpr bool ACCUM = EPI == EPI_ATOMIC_F32 && !PART;  // one split: out += alpha * acc
   const float alpha = p.alpha;
+  const int q = threadIdx.x & 3;
   const float* bias = p.bias + col0;
   const bf16* ax = p.aux_in + (long long)row * p.ld_aux_in + col0;
   const long long ax8 = 8 * p.ld_aux_in;
@@ -228,50 +274,130 @@ __device__ __forceinline__ void epi_tile(const GemmParams& p, int split, int row
     const int s = (j0 / CHUNK) & 1;
     if (j0 + CHUNK < GROUPS) load(j0 + CHUNK, s ^ 1);
 #pragma unroll
-    for (int j = 0; j < CHUNK; ++j) {
-      const int c = (j0 + j) * 8;
+    for (int jq = 0; jq < CHUNK; jq += 4) {  // one quad of 8-column groups
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        float v0 = __fmul_rn(acc[4 * (j0 + j) + 2 * h], alpha);
-        float v1 = __fmul_rn(acc[4 * (j0 + j) + 2 * h + 1], alpha);
-        if constexpr (BIAS) {
-          v0 = __fadd_rn(v0, b[s][j][0]);
-          v1 = __fadd_rn(v1, b[s][j][1]);
-        }
-        if constexpr (AUX) {
-          const float2 f = unpack_bf16x2(x[s][j][h]);
-          if constexpr (EPI == EPI_GELU_BWD_BF16) {
-            v0 = __fmul_rn(v0, gelu_erf_grad(f.x));
-            v1 = __fmul_rn(v1, gelu_erf_grad(f.y));
+      for (int h = 0; h < 2; ++h) {  // rows row, row + 8
+        uint32_t wo[4], wa[4];       // WIDE: packed out / aux_out words of the quad's groups in this row
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+          const int j = jq + jj;
+          const int c = (j0 + j) * 8;
+          float v0 = __fmul_rn(acc[4 * (j0 + j) + 2 * h], alpha);
+          float v1 = __fmul_rn(acc[4 * (j0 + j) + 2 * h + 1], alpha);
+          if constexpr (BIAS) {
+            v0 = __fadd_rn(v0, b[s][j][0]);
+            v1 = __fadd_rn(v1, b[s][j][1]);
+          }
+          if constexpr (AUX) {
+            const float2 f = unpack_bf16x2(x[s][j][h]);
+            if constexpr (EPI == EPI_GELU_BWD_BF16) {
+              v0 = __fmul_rn(v0, gelu_erf_grad(f.x));
+              v1 = __fmul_rn(v1, gelu_erf_grad(f.y));
+            } else {
+              v0 = __fadd_rn(v0, f.x);
+              v1 = __fadd_rn(v1, f.y);
+            }
+          }
+          if constexpr (OUT_F32) {
+            if constexpr (ACCUM) {
+              v0 = __fadd_rn(a[s][j][h].x, v0);
+              v1 = __fadd_rn(a[s][j][h].y, v1);
+            }
+            *reinterpret_cast<float2*>(of + h * o8 + c) = make_float2(v0, v1);
           } else {
-            v0 = __fadd_rn(v0, f.x);
-            v1 = __fadd_rn(v1, f.y);
+            if constexpr (EPI == EPI_BIAS_GELU_BF16) {
+              const uint32_t w = pack_bf16x2(v0, v1);
+              if constexpr (WIDE) wa[jj] = w;
+              else *reinterpret_cast<uint32_t*>(ao + h * ao8 + c) = w;
+              v0 = gelu_erf(v0);
+              v1 = gelu_erf(v1);
+            }
+            const uint32_t w = pack_bf16x2(v0, v1);
+            if constexpr (WIDE) wo[jj] = w;
+            else *reinterpret_cast<uint32_t*>(ob + h * o8 + c) = w;
           }
         }
-        if constexpr (OUT_F32) {
-          if constexpr (ACCUM) {
-            v0 = __fadd_rn(a[s][j][h].x, v0);
-            v1 = __fadd_rn(a[s][j][h].y, v1);
-          }
-          *reinterpret_cast<float2*>(of + h * o8 + c) = make_float2(v0, v1);
-        } else {
-          if constexpr (EPI == EPI_BIAS_GELU_BF16) {
-            *reinterpret_cast<uint32_t*>(ao + h * ao8 + c) = pack_bf16x2(v0, v1);
-            v0 = gelu_erf(v0);
-            v1 = gelu_erf(v1);
-          }
-          *reinterpret_cast<uint32_t*>(ob + h * o8 + c) = pack_bf16x2(v0, v1);
+        if constexpr (WIDE) {
+          // this lane stores group j0 + jq + q whole: 8 (j0 + jq) + 6 q columns from col0 = 2 q
+          const int c = (j0 + jq) * 8 + 6 * q;
+          if constexpr (EPI == EPI_BIAS_GELU_BF16)
+            *reinterpret_cast<uint4*>(ao + h * ao8 + c) = quad_transpose(wa[0], wa[1], wa[2], wa[3], q);
+          *reinterpret_cast<uint4*>(ob + h * o8 + c) = quad_transpose(wo[0], wo[1], wo[2], wo[3], q);
         }
       }
     }
   }
 }
 
+// fused epilogue of one warpgroup's 64 x BLOCK_N accumulator block.  accumulator fragment: warp w holds rows
+// 16 w + lane / 4 (+ 8); register 4 j + {0, 1} (+ {2, 3} for row + 8) are columns 8 j + 2 (lane % 4) + {0, 1}.
+// The epilogue is chosen once per work item (inside: its whole tile lies in the output): tiles wholly inside the
+// output take the unchecked epi_tile, edge tiles and launches without 2-element vector access the checked per-pair
+// epi_pair.
+template <int BLOCK_N>
+__device__ __forceinline__ void epilogue_block(const GemmParams& p, bool inside, int split, int n0, int row, int col0,
+                                               const float (&acc)[BLOCK_N / 2]) {
+  if (inside) {
+    const bool bias = p.bias != nullptr;
+    const bool wide = p.vec8;
+    switch (p.epilogue) {
+      case EPI_BIAS_BF16:
+        if (wide) {
+          if (bias) epi_tile<EPI_BIAS_BF16, true, false, BLOCK_N, true>(p, split, row, col0, acc);
+          else epi_tile<EPI_BIAS_BF16, false, false, BLOCK_N, true>(p, split, row, col0, acc);
+        } else {
+          if (bias) epi_tile<EPI_BIAS_BF16, true, false, BLOCK_N>(p, split, row, col0, acc);
+          else epi_tile<EPI_BIAS_BF16, false, false, BLOCK_N>(p, split, row, col0, acc);
+        }
+        break;
+      case EPI_BIAS_GELU_BF16:
+        if (wide) {
+          if (bias) epi_tile<EPI_BIAS_GELU_BF16, true, false, BLOCK_N, true>(p, split, row, col0, acc);
+          else epi_tile<EPI_BIAS_GELU_BF16, false, false, BLOCK_N, true>(p, split, row, col0, acc);
+        } else {
+          if (bias) epi_tile<EPI_BIAS_GELU_BF16, true, false, BLOCK_N>(p, split, row, col0, acc);
+          else epi_tile<EPI_BIAS_GELU_BF16, false, false, BLOCK_N>(p, split, row, col0, acc);
+        }
+        break;
+      case EPI_GELU_BWD_BF16:
+        if (wide) epi_tile<EPI_GELU_BWD_BF16, false, false, BLOCK_N, true>(p, split, row, col0, acc);
+        else epi_tile<EPI_GELU_BWD_BF16, false, false, BLOCK_N>(p, split, row, col0, acc);
+        break;
+      case EPI_ADD_BF16:
+        if (wide) epi_tile<EPI_ADD_BF16, false, false, BLOCK_N, true>(p, split, row, col0, acc);
+        else epi_tile<EPI_ADD_BF16, false, false, BLOCK_N>(p, split, row, col0, acc);
+        break;
+      case EPI_BIAS_F32:
+        if (bias) epi_tile<EPI_BIAS_F32, true, false, BLOCK_N>(p, split, row, col0, acc);
+        else epi_tile<EPI_BIAS_F32, false, false, BLOCK_N>(p, split, row, col0, acc);
+        break;
+      default:
+        if (p.part != nullptr) epi_tile<EPI_ATOMIC_F32, false, true, BLOCK_N>(p, split, row, col0, acc);
+        else epi_tile<EPI_ATOMIC_F32, false, false, BLOCK_N>(p, split, row, col0, acc);
+    }
+  } else {
+#pragma unroll
+    for (int j = 0; j < BLOCK_N / 8; ++j) {
+      if (n0 + j * 8 >= p.N) break;  // warp-uniform
+      epi_pair(p, split, row, col0 + j * 8, acc[4 * j], acc[4 * j + 1]);
+      epi_pair(p, split, row + 8, col0 + j * 8, acc[4 * j + 2], acc[4 * j + 3]);
+    }
+  }
+}
+
+__device__ __forceinline__ bool tile_inside(const GemmParams& p, const WorkItem& wi, int bn) {
+  return p.vec2 && wi.m0 + BLOCK_M <= p.M && wi.n0 + bn <= p.N && (p.part == nullptr || (p.N & 1) == 0);
+}
+
+// named barriers of the ping-pong hand-off: consumer warpgroup c waits on TURN_BAR + c for its turn at the MMAs
+constexpr int TURN_BAR = 1;
+
 template <int BLOCK_N, int STAGES, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                   const GemmParams p, const int num_work) {
   using L = GemmSmem<BLOCK_N, STAGES>;
+  constexpr bool PING = BLOCK_N <= 128;  // ping-pong schedule (else cooperative), see the top of this file
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -289,7 +415,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     tma_prefetch_desc(&tmap_b);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 2);  // one arrival per consumer warpgroup
+      mbar_init(&empty_bar[s], PING ? 1 : 2);  // one arrival per consumer warpgroup that reads the stage
     }
     fence_mbar_init();
   }
@@ -328,8 +454,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         }
       }
     }
-  } else {
-    // ------------------------------ consumers ------------------------------
+  } else if constexpr (!PING) {
+    // ------------------------------ cooperative consumers ------------------------------
     regs_alloc<232>();
     const int c = wg - 1;  // rows [64 c, 64 c + 64) of every tile
     const int t = threadIdx.x & 127;
@@ -368,48 +494,75 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       wgmma_wait<0>();
       fence_regs(acc);
       if (t == 0) mbar_arrive(&empty_bar[prev_s]);
-      // accumulator fragment: warp w holds rows 16 w + lane / 4 (+ 8); register 4 j + {0, 1} (+ {2, 3} for row + 8) are
-      // columns 8 j + 2 (lane % 4) + {0, 1}
       const int row = wi.m0 + c * 64 + warp * 16 + (lane >> 2);
       const int col0 = wi.n0 + 2 * (lane & 3);
-      const int split = wi.kb_begin / kb_per;
-      // the epilogue is chosen once per work item: tiles wholly inside the output take the unchecked epi_tile, edge
-      // tiles and launches without 2-element vector access the checked per-pair epi_pair
-      const bool inside = p.vec2 && wi.m0 + BLOCK_M <= p.M && wi.n0 + BLOCK_N <= p.N &&
-                          (p.part == nullptr || (p.N & 1) == 0);
-      if (inside) {
-        const bool bias = p.bias != nullptr;
-        switch (p.epilogue) {
-          case EPI_BIAS_BF16:
-            if (bias) epi_tile<EPI_BIAS_BF16, true, false, BLOCK_N>(p, split, row, col0, acc);
-            else epi_tile<EPI_BIAS_BF16, false, false, BLOCK_N>(p, split, row, col0, acc);
-            break;
-          case EPI_BIAS_GELU_BF16:
-            if (bias) epi_tile<EPI_BIAS_GELU_BF16, true, false, BLOCK_N>(p, split, row, col0, acc);
-            else epi_tile<EPI_BIAS_GELU_BF16, false, false, BLOCK_N>(p, split, row, col0, acc);
-            break;
-          case EPI_GELU_BWD_BF16:
-            epi_tile<EPI_GELU_BWD_BF16, false, false, BLOCK_N>(p, split, row, col0, acc);
-            break;
-          case EPI_ADD_BF16:
-            epi_tile<EPI_ADD_BF16, false, false, BLOCK_N>(p, split, row, col0, acc);
-            break;
-          case EPI_BIAS_F32:
-            if (bias) epi_tile<EPI_BIAS_F32, true, false, BLOCK_N>(p, split, row, col0, acc);
-            else epi_tile<EPI_BIAS_F32, false, false, BLOCK_N>(p, split, row, col0, acc);
-            break;
-          default:
-            if (p.part != nullptr) epi_tile<EPI_ATOMIC_F32, false, true, BLOCK_N>(p, split, row, col0, acc);
-            else epi_tile<EPI_ATOMIC_F32, false, false, BLOCK_N>(p, split, row, col0, acc);
-        }
-      } else {
-#pragma unroll
-        for (int j = 0; j < BLOCK_N / 8; ++j) {
-          if (wi.n0 + j * 8 >= p.N) break;  // warp-uniform
-          epi_pair(p, split, row, col0 + j * 8, acc[4 * j], acc[4 * j + 1]);
-          epi_pair(p, split, row + 8, col0 + j * 8, acc[4 * j + 2], acc[4 * j + 3]);
-        }
+      epilogue_block<BLOCK_N>(p, tile_inside(p, wi, BLOCK_N), wi.kb_begin / kb_per, wi.n0, row, col0, acc);
+    }
+  } else {
+    // ------------------------------ ping-pong consumers ------------------------------
+    // Warpgroup c owns the CTA's items j = c, c + 2, c + 4, ...: all 128 rows of each.  Its mainloop of item j starts
+    // only once the other warpgroup has issued its last MMA of item j - 1 (TURN_BAR + c), and it hands over the same
+    // way when it has issued its own, so the two mainloops take turns in item order and each warpgroup's epilogue runs
+    // under the other's MMAs.  The hand-off is also what makes the ring safe: every k-block before item j has passed
+    // its full_bar wait when item j starts, so no full_bar wait runs more than one phase ahead of the barrier, where
+    // its parity would match a phase that has already completed and it would read a stage before its load lands.
+    regs_alloc<232>();
+    const int c = wg - 1;
+    const int t = threadIdx.x & 127;
+    const int warp = t >> 5, lane = t & 31;
+    uint32_t it = 0;  // ring position: advances over the other warpgroup's k-blocks as well as this one's
+    int j = 0;
+    for (int w = blockIdx.x; w < num_work; w += gridDim.x, ++j) {
+      const WorkItem wi = decode_work(w, m_tiles, n_tiles, total_kb, kb_per, BLOCK_N);
+      if ((j & 1) != c) {  // the other warpgroup's item (num_kb differs between items under split-K)
+        it += wi.num_kb;
+        continue;
       }
+      float acc[2][BLOCK_N / 2];  // rows 0-63 and 64-127 of the tile
+#pragma unroll
+      for (int e = 0; e < BLOCK_N / 2; ++e) acc[0][e] = acc[1][e] = 0.f;
+      if (j > 0) named_bar(TURN_BAR + c, 256);
+      int prev_s = -1;
+      for (int i = 0; i < wi.num_kb; ++i, ++it) {
+        const int s = it % STAGES;
+        const uint32_t ph = (it / STAGES) & 1;
+        mbar_wait(&full_bar[s], ph);
+        // rows 64-127 of A start 8 KB into the stage in both layouts, as in the cooperative schedule
+        const uint32_t sa = smem_u32(smem + s * L::STAGE_BYTES);
+        const uint32_t sb = sa + L::A_BYTES;
+        wgmma_fence();
+        fence_regs(acc[0]);
+        fence_regs(acc[1]);
+#pragma unroll
+        for (int k = 0; k < BLOCK_K / 16; ++k) {
+          const uint64_t db = B_MN ? make_smem_desc_sw128(sb + k * 2048, BLOCK_K * 128, 1024)
+                                   : make_smem_desc_sw128(sb + k * 32, 16, 1024);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const uint32_t sah = sa + h * (64 * 128);
+            const uint64_t da = A_MN ? make_smem_desc_sw128(sah + k * 2048, BLOCK_K * 128, 1024)
+                                     : make_smem_desc_sw128(sah + k * 32, 16, 1024);
+            WgmmaSS<BLOCK_N>::template mma<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc[h], da, db, (i > 0 || k > 0) ? 1 : 0);
+          }
+        }
+        wgmma_commit();
+        fence_regs(acc[0]);
+        fence_regs(acc[1]);
+        wgmma_wait<1>();  // the previous k-block's MMAs have read their stage
+        if (prev_s >= 0 && t == 0) mbar_arrive(&empty_bar[prev_s]);
+        prev_s = s;
+      }
+      if (w + (int)gridDim.x < num_work) named_bar_arrive(TURN_BAR + (c ^ 1), 256);  // the next item's turn
+      wgmma_wait<0>();
+      fence_regs(acc[0]);
+      fence_regs(acc[1]);
+      if (t == 0) mbar_arrive(&empty_bar[prev_s]);
+      const bool inside = tile_inside(p, wi, BLOCK_N);
+      const int split = wi.kb_begin / kb_per;
+      const int row = wi.m0 + warp * 16 + (lane >> 2);
+      const int col0 = wi.n0 + 2 * (lane & 3);
+      epilogue_block<BLOCK_N>(p, inside, split, wi.n0, row, col0, acc[0]);
+      epilogue_block<BLOCK_N>(p, inside, split, wi.n0, row + 64, col0, acc[1]);
     }
   }
 }
@@ -458,10 +611,22 @@ int plan_gemm(int M, int N, int Kc, int epilogue, int block_n, int split_k, Gemm
   int bn = block_n;
   if (bn == 0) {
     bn = 256;
-    // without split-K the tile count alone must fill the SMs; with the atomic epilogue split-K supplies the
-    // parallelism, so keep the widest (most operand-bandwidth-efficient) tile
-    if (epilogue != EPI_ATOMIC_F32)
-      while (bn > 64 && (long long)m_tiles * ((N + bn - 1) / bn) < PLAN_SMS) bn >>= 1;
+    // Without split-K the tile count alone must fill the SMs.  256 -> 128 below two work items per SM: the 128-wide
+    // ping-pong tiles then keep both warpgroups of a CTA busy, where a 256-wide grid of 1.1 waves leaves most SMs idle
+    // for its second wave (1536 x 3072 x 768, bias + GELU: 0.036 against 0.044 ms).  128 -> 64 only below one item
+    // per SM (the caption step, whose 4096-row GEMMs of 768 columns then go to 64, ran 2.6 % slower when they
+    // narrowed at two items per SM as well).  A problem with thousands of tiles keeps the cooperative
+    // 256-wide tile: it loads the fewest operand bytes per MMA, and on an H100 SXM at a 400 W power limit the
+    // 98304-row GEMMs, which run at that cap, were up to 16 % slower with 128-wide ping-pong tiles (a lower SM clock
+    // for the same work; the bias + GELU forward was 2 % faster).
+    // The fp32 weight gradients keep 256 and take their parallelism from split-K (cross-encoder wgrads, K = 98304:
+    // 256 is 20-45 % faster than 128 or 64).  Their split count follows from the tile count, and it sets the order in
+    // which the partial sums are added, so a different tile width would change their bits.
+    if (epilogue != EPI_ATOMIC_F32) {
+      const auto tiles = [&](int w) { return (long long)m_tiles * ((N + w - 1) / w); };
+      if (tiles(256) < 2 * PLAN_SMS) bn = 128;
+      if (tiles(128) < PLAN_SMS) bn = 64;
+    }
     if (N <= 64) bn = 64;
     else if (N <= 128 && bn > 128) bn = 128;
   }
@@ -542,6 +707,10 @@ extern "C" int univl_gemm_bf16(const void* A, long long lda, int a_mn_major, con
   if (aux_in != nullptr) vec2 = vec2 && ((uintptr_t)aux_in % 4) == 0 && (ld_aux_in % 2) == 0;
   if (aux_out != nullptr) vec2 = vec2 && ((uintptr_t)aux_out % 4) == 0 && (ld_aux_out % 2) == 0;
   p.vec2 = vec2 ? 1 : 0;
+  // 16-byte stores of the bf16 outputs: 8-column groups start at multiples of 8 columns from a 16-byte aligned base
+  bool vec8 = !out_f32 && ((uintptr_t)out % 16) == 0 && (ldo % 8) == 0;
+  if (aux_out != nullptr) vec8 = vec8 && ((uintptr_t)aux_out % 16) == 0 && (ld_aux_out % 8) == 0;
+  p.vec8 = vec8 ? 1 : 0;
   p.part = nullptr;
   if (plan.splits > 1)
     if ((rc = scratch_alloc((void**)&p.part, (size_t)plan.splits * M * N * sizeof(float), stream))) return rc;
