@@ -49,6 +49,25 @@ int univl_gemm_bf16(const void* A, long long lda, int a_mn_major, const void* B,
  * function of its arguments (measurement aid: bench.py attributes launch times to the dominant kernel with it) */
 int univl_gemm_plan(int M, int N, int Kc, int epilogue, int block_n, int split_k);
 
+/* ---- FP8 (e4m3) forward GEMM with block scaling (cross-encoder evaluation) ------------------------------------
+ * A block of e4m3 codes q with its fp32 scale s stands for q * s.  s = 2^ceil(log2(amax / 448)) of the block's largest
+ * magnitude (1 for an all-zero block, at least 2^-126); codes round to nearest even and saturate at +-448.
+ * univl_quantize_e4m3_rows:   x bf16 [M, K] (ldx) -> q e4m3 [M, K] (ldq), scale fp32 [K/128, M]: 1 x 128 blocks.
+ * univl_quantize_e4m3_blocks: w fp32 [N, K] (ldw) -> q e4m3 [N, K] (ldq), scale fp32 [N/128, K/128]: 128 x 128 blocks.
+ * univl_gemm_fp8: D[M,N] = epilogue(sum_kb a_scale[kb, m] b_scale[n/128, kb] sum_{k in kb} A(m,k) B(n,k)),
+ *   A e4m3 [M, Kc] (lda) with a_scale [Kc/128, M], B e4m3 [N, Kc] (ldb) with b_scale [N/128, Kc/128], both K-major;
+ *   Kc and N multiples of 128; each 128-wide K block accumulates apart and is added in fp32 with its two scales.
+ *   epilogue 0: out bf16 [M, ldo] = D + bias      (module_bert.py:208 attention output, :247 FFN output, K/V)
+ *            1: out e4m3 [M, ldo] with out_scale [N/128, M] = gelu_erf(D + bias) quantized per (row, 128 columns)
+ *               (module_bert.py:234 intermediate; no pre-activation is written: forward only) */
+int univl_quantize_e4m3_rows(const void* x, long long ldx, void* q, long long ldq, float* scale, int M, int K,
+                             void* stream);
+int univl_quantize_e4m3_blocks(const float* w, long long ldw, void* q, long long ldq, float* scale, int N, int K,
+                               void* stream);
+int univl_gemm_fp8(const void* A, long long lda, const float* a_scale, const void* B, long long ldb,
+                   const float* b_scale, int M, int N, int Kc, int epilogue, const float* bias, void* out,
+                   long long ldo, float* out_scale, void* stream);
+
 /* ---- LayerNorm family (until_module.py:49-53; eps inside sqrt) ---------------------------------------------
  * drop_mode 1: y = LN(dropout(x) + res)   (module_bert.py:207-211, :246-250)
  * drop_mode 2: y = dropout(LN(x + res))   (embeddings; head transforms use p = 0) */

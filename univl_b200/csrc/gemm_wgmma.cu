@@ -26,10 +26,12 @@
 // schedules give every output element the same chain of k16 wgmmas in the same k order and the same epilogue, so the
 // tile width does not change a bit of the result.
 #include "common.cuh"
+#include "fp8.cuh"
 #include "tmap.cuh"
 #include "wgmma.cuh"
 
 #include <stdio.h>
+#include <type_traits>
 
 namespace univl {
 
@@ -392,6 +394,44 @@ __device__ __forceinline__ bool tile_inside(const GemmParams& p, const WorkItem&
 // named barriers of the ping-pong hand-off: consumer warpgroup c waits on TURN_BAR + c for its turn at the MMAs
 constexpr int TURN_BAR = 1;
 
+// TMA producer (one thread): streams the k-blocks of the CTA's work items, in order, into the STAGES-deep ring.
+// ELEM: operand bytes per element (2 = bf16, 1 = e4m3).  A k-block is 128 bytes of K whatever the type (64 bf16 or
+// 128 e4m3), so the stage bytes, the 128B swizzle and the box shapes are the same for both; only the k coordinate
+// of a block differs.
+template <int BLOCK_N, int STAGES, bool A_MN, bool B_MN, int ELEM = 2>
+__device__ __forceinline__ void produce_ring(const CUtensorMap* tmap_a, const CUtensorMap* tmap_b, uint8_t* smem,
+                                             uint64_t* full_bar, uint64_t* empty_bar, int num_work, int m_tiles,
+                                             int n_tiles, int total_kb, int kb_per) {
+  using L = GemmSmem<BLOCK_N, STAGES>;
+  uint32_t it = 0;
+  for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
+    const WorkItem wi = decode_work(w, m_tiles, n_tiles, total_kb, kb_per, BLOCK_N);
+    for (int i = 0; i < wi.num_kb; ++i, ++it) {
+      const int s = it % STAGES;
+      const uint32_t ph = (it / STAGES) & 1;
+      mbar_wait(&empty_bar[s], ph ^ 1);
+      uint8_t* sa = smem + s * L::STAGE_BYTES;
+      uint8_t* sb = sa + L::A_BYTES;
+      mbar_arrive_expect_tx(&full_bar[s], L::STAGE_BYTES);
+      const int k_elem = (wi.kb_begin + i) * (128 / ELEM);
+      if (!A_MN) {
+        tma_load_2d(sa, tmap_a, &full_bar[s], k_elem, wi.m0);  // box {128 B of k, 128 rows}
+      } else {
+#pragma unroll
+        for (int c = 0; c < BLOCK_M / 64; ++c)  // box {64 m, 64 k-rows}
+          tma_load_2d(sa + c * (BLOCK_K * 128), tmap_a, &full_bar[s], wi.m0 + c * 64, k_elem);
+      }
+      if (!B_MN) {
+        tma_load_2d(sb, tmap_b, &full_bar[s], k_elem, wi.n0);  // box {128 B of k, BLOCK_N rows}
+      } else {
+#pragma unroll
+        for (int c = 0; c < BLOCK_N / 64; ++c)
+          tma_load_2d(sb + c * (BLOCK_K * 128), tmap_b, &full_bar[s], wi.n0 + c * 64, k_elem);
+      }
+    }
+  }
+}
+
 template <int BLOCK_N, int STAGES, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
@@ -425,35 +465,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   if (wg == 0) {
     // ------------------------------ TMA producer ------------------------------
     regs_dealloc<40>();
-    if (threadIdx.x == 0) {
-      uint32_t it = 0;
-      for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
-        const WorkItem wi = decode_work(w, m_tiles, n_tiles, total_kb, kb_per, BLOCK_N);
-        for (int i = 0; i < wi.num_kb; ++i, ++it) {
-          const int s = it % STAGES;
-          const uint32_t ph = (it / STAGES) & 1;
-          mbar_wait(&empty_bar[s], ph ^ 1);
-          uint8_t* sa = smem + s * L::STAGE_BYTES;
-          uint8_t* sb = sa + L::A_BYTES;
-          mbar_arrive_expect_tx(&full_bar[s], L::STAGE_BYTES);
-          const int k_elem = (wi.kb_begin + i) * BLOCK_K;
-          if (!A_MN) {
-            tma_load_2d(sa, &tmap_a, &full_bar[s], k_elem, wi.m0);  // box {64 k, 128 rows}
-          } else {
-#pragma unroll
-            for (int c = 0; c < BLOCK_M / 64; ++c)  // box {64 m, 64 k-rows}
-              tma_load_2d(sa + c * (BLOCK_K * 128), &tmap_a, &full_bar[s], wi.m0 + c * 64, k_elem);
-          }
-          if (!B_MN) {
-            tma_load_2d(sb, &tmap_b, &full_bar[s], k_elem, wi.n0);  // box {64 k, BLOCK_N rows}
-          } else {
-#pragma unroll
-            for (int c = 0; c < BLOCK_N / 64; ++c)
-              tma_load_2d(sb + c * (BLOCK_K * 128), &tmap_b, &full_bar[s], wi.n0 + c * 64, k_elem);
-          }
-        }
-      }
-    }
+    if (threadIdx.x == 0)
+      produce_ring<BLOCK_N, STAGES, A_MN, B_MN>(&tmap_a, &tmap_b, smem, full_bar, empty_bar, num_work, m_tiles, n_tiles,
+                                                total_kb, kb_per);
   } else if constexpr (!PING) {
     // ------------------------------ cooperative consumers ------------------------------
     regs_alloc<232>();
@@ -595,6 +609,204 @@ static int dispatch_major(bool a_mn, bool b_mn, const CUtensorMap& ta, const CUt
   return launch_gemm<BLOCK_N, STAGES, true, false>(ta, tb, p, splits, stream);
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// FP8 (e4m3 x e4m3) GEMM with fine-grained scaling, forward only:
+//   D[M,N] = epilogue( sum_kb  sa[kb, m] * sb[n / 128, kb] * sum_{k in block kb} A(m,k) B(n,k) )
+// A [M,K] e4m3 with one scale per (row, 128-column block), sa laid out [K/128, M]; B [N,K] e4m3 with one scale per
+// 128 x 128 block, sb [N/128, K/128].  Both K-major (8-bit wgmma takes no other layout).
+// The producer, ring, work decoding and descriptors are the bf16 kernel's: a k-block is 128 e4m3 = 128 bytes, one
+// stage holds the same bytes with the same swizzle, and a k32 step advances the descriptors by the same 32 bytes.
+// The consumers run the cooperative schedule on 128 x 128 tiles (each warpgroup 64 rows).  Every k-block is one
+// scaling block: its four k32 wgmmas accumulate into a temporary, which is then promoted into the fp32 accumulator
+// with one FMA by sa * sb (a product of two powers of two, exact).  So the tensor cores' in-instruction accumulation,
+// whose precision is not specified for 8-bit inputs, only ever sums 128 products.  The accumulator and two
+// temporaries (3 x 64 floats per thread) fit in registers without spills, which the 256-wide tile (3 x 128) would not.
+// Epilogues: FP8_EPI_BIAS_BF16  out(bf16) = acc + bias (the bf16 kernel's unchecked / checked epilogue code)
+//            FP8_EPI_GELU_E4M3  out(e4m3), out_scale = gelu_erf(acc + bias) quantized per (row, 128-column block), the
+//                               scale found from the accumulator fragment with two quad shuffles
+enum Fp8Epilogue : int { FP8_EPI_BIAS_BF16 = 0, FP8_EPI_GELU_E4M3 = 1 };
+
+struct Fp8Params {
+  const float* a_scale;  // [K/128, M]
+  const float* b_scale;  // [N/128, K/128]
+  uint8_t* out_q;        // FP8_EPI_GELU_E4M3: e4m3 [M, ldo]
+  float* out_scale;      // FP8_EPI_GELU_E4M3: [N/128, M]
+};
+
+constexpr int FP8_BLOCK_N = 128;
+constexpr int FP8_STAGES = 6;
+
+template <int EPI, bool PAIRS>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                const GemmParams p, const Fp8Params f, const int num_work) {
+  using L = GemmSmem<FP8_BLOCK_N, FP8_STAGES>;
+  pdl_trigger();
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFFSET);
+  uint64_t* empty_bar = full_bar + FP8_STAGES;
+
+  const int wg = threadIdx.x >> 7;
+  const int m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M;
+  const int n_tiles = p.N / FP8_BLOCK_N;
+  const int total_kb = p.Kc / 128;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmap_a);
+    tma_prefetch_desc(&tmap_b);
+    for (int s = 0; s < FP8_STAGES; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 2);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  pdl_wait();
+
+  if (wg == 0) {
+    regs_dealloc<40>();
+    if (threadIdx.x == 0)
+      produce_ring<FP8_BLOCK_N, FP8_STAGES, false, false, 1>(&tmap_a, &tmap_b, smem, full_bar, empty_bar, num_work,
+                                                              m_tiles, n_tiles, total_kb, total_kb);
+    return;
+  }
+  regs_alloc<232>();
+  const int c = wg - 1;  // rows [64 c, 64 c + 64) of every tile
+  const int t = threadIdx.x & 127;
+  const int warp = t >> 5, lane = t & 31;
+  const int M = p.M;
+  uint32_t it = 0;
+  for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
+    const WorkItem wi = decode_work(w, m_tiles, n_tiles, total_kb, total_kb, FP8_BLOCK_N);
+    const int row = wi.m0 + c * 64 + warp * 16 + (lane >> 2);  // and row + 8
+    const bool in0 = row < M, in1 = row + 8 < M;
+    const float* sa = f.a_scale + row;
+    const float* sb = f.b_scale + (long long)(wi.n0 / FP8_BLOCK_N) * total_kb;
+    float acc[FP8_BLOCK_N / 2];
+#pragma unroll
+    for (int e = 0; e < FP8_BLOCK_N / 2; ++e) acc[e] = 0.f;
+    // Block kb's four wgmmas go into a temporary (issue), which is then added into acc with the block's scales
+    // (promote, after waiting until at most `newer` younger wgmma groups are in flight).  With an even number of
+    // blocks (PAIRS) two temporaries alternate, so that the MMAs of block kb + 1 run while block kb is promoted; the
+    // wgmmas and waits sit in straight-line code and a loop, never under a data-dependent branch, which would make
+    // ptxas serialize them.  An odd number of blocks takes one temporary and waits for each block's MMAs.
+    auto issue = [&](float (&tmp)[FP8_BLOCK_N / 2], int kb) {
+      const uint32_t r = it + kb;
+      const int s = r % FP8_STAGES;
+      mbar_wait(&full_bar[s], (r / FP8_STAGES) & 1);
+      const uint32_t a_s = smem_u32(smem + s * L::STAGE_BYTES) + c * (64 * 128);
+      const uint32_t b_s = smem_u32(smem + s * L::STAGE_BYTES) + L::A_BYTES;
+      wgmma_fence();
+      fence_regs(tmp);
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        WgmmaSSE4M3N128::mma(tmp, make_smem_desc_sw128(a_s + k * 32, 16, 1024),
+                             make_smem_desc_sw128(b_s + k * 32, 16, 1024), k > 0 ? 1 : 0);
+      wgmma_commit();
+      fence_regs(tmp);
+    };
+    auto promote = [&](auto newer, float (&tmp)[FP8_BLOCK_N / 2], int kb) {
+      // the block's scales, loaded before the wait so their latency hides under it
+      const float bs = __ldg(sb + kb);
+      const float s0 = in0 ? __ldg(sa + (long long)kb * M) : 0.f;
+      const float s1 = in1 ? __ldg(sa + (long long)kb * M + 8) : 0.f;
+      wgmma_wait<decltype(newer)::value>();
+      fence_regs(tmp);
+      if (t == 0) mbar_arrive(&empty_bar[(it + kb) % FP8_STAGES]);
+      const float f0 = s0 * bs, f1 = s1 * bs;
+#pragma unroll
+      for (int j = 0; j < FP8_BLOCK_N / 8; ++j) {
+        acc[4 * j] = __fmaf_rn(tmp[4 * j], f0, acc[4 * j]);
+        acc[4 * j + 1] = __fmaf_rn(tmp[4 * j + 1], f0, acc[4 * j + 1]);
+        acc[4 * j + 2] = __fmaf_rn(tmp[4 * j + 2], f1, acc[4 * j + 2]);
+        acc[4 * j + 3] = __fmaf_rn(tmp[4 * j + 3], f1, acc[4 * j + 3]);
+      }
+    };
+    using One = std::integral_constant<int, 1>;
+    using None = std::integral_constant<int, 0>;
+    float ta[FP8_BLOCK_N / 2];
+    if constexpr (PAIRS) {
+      float tb[FP8_BLOCK_N / 2];
+      issue(ta, 0);
+      issue(tb, 1);
+      int kb = 0;
+      for (; kb + 2 < total_kb; kb += 2) {
+        promote(One(), ta, kb);
+        issue(ta, kb + 2);
+        promote(One(), tb, kb + 1);
+        issue(tb, kb + 3);
+      }
+      promote(One(), ta, kb);
+      promote(None(), tb, kb + 1);
+    } else {
+      for (int kb = 0; kb < total_kb; ++kb) {
+        issue(ta, kb);
+        promote(None(), ta, kb);
+      }
+    }
+    it += total_kb;
+    const int col0 = wi.n0 + 2 * (lane & 3);
+    if constexpr (EPI == FP8_EPI_BIAS_BF16) {
+      if (tile_inside(p, wi, FP8_BLOCK_N)) {
+        if (p.vec8) epi_tile<EPI_BIAS_BF16, true, false, FP8_BLOCK_N, true>(p, 0, row, col0, acc);
+        else epi_tile<EPI_BIAS_BF16, true, false, FP8_BLOCK_N>(p, 0, row, col0, acc);
+      } else {
+#pragma unroll
+        for (int j = 0; j < FP8_BLOCK_N / 8; ++j) {
+          epi_pair(p, 0, row, col0 + j * 8, acc[4 * j], acc[4 * j + 1]);
+          epi_pair(p, 0, row + 8, col0 + j * 8, acc[4 * j + 2], acc[4 * j + 3]);
+        }
+      }
+    } else {
+      // the tile's 128 columns are one scaling block: a row's amax is the max over its quad's fragments
+      const float* bias = p.bias + col0;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {  // rows row, row + 8
+        float amax = 0.f;
+#pragma unroll
+        for (int j = 0; j < FP8_BLOCK_N / 8; ++j) {
+          const float v0 = gelu_erf(__fadd_rn(acc[4 * j + 2 * h], __ldg(bias + 8 * j)));
+          const float v1 = gelu_erf(__fadd_rn(acc[4 * j + 2 * h + 1], __ldg(bias + 8 * j + 1)));
+          acc[4 * j + 2 * h] = v0;
+          acc[4 * j + 2 * h + 1] = v1;
+          amax = fmaxf(amax, fmaxf(fabsf(v0), fabsf(v1)));
+        }
+        amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
+        amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 2));
+        const float sc = e4m3_scale(amax);
+        const float inv = e4m3_inv_scale(sc);
+        const int r = row + 8 * h;
+        if (r < M) {
+          uint8_t* q = f.out_q + (long long)r * p.ldo + col0;
+#pragma unroll
+          for (int j = 0; j < FP8_BLOCK_N / 8; ++j)
+            *reinterpret_cast<uint16_t*>(q + 8 * j) =
+                e4m3x2(__fmul_rn(acc[4 * j + 2 * h], inv), __fmul_rn(acc[4 * j + 2 * h + 1], inv));
+          if ((lane & 3) == 0) f.out_scale[(long long)(wi.n0 / FP8_BLOCK_N) * M + r] = sc;
+        }
+      }
+    }
+  }
+}
+
+template <int EPI, bool PAIRS>
+static int launch_gemm_fp8(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, const Fp8Params& f,
+                           cudaStream_t stream) {
+  using L = GemmSmem<FP8_BLOCK_N, FP8_STAGES>;
+  auto kern = gemm_fp8_kernel<EPI, PAIRS>;
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::DYN_BYTES);
+  if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "univl_gemm_fp8 smem attribute: %s", cudaGetErrorString(e));
+  const long long work = (long long)((p.M + BLOCK_M - 1) / BLOCK_M) * (p.N / FP8_BLOCK_N);
+  if (work > 0x7fffffffLL) return set_error(UNIVL_ERR_ARG, "univl_gemm_fp8: too many tiles");
+  const int sms = usable_sms();
+  const int grid = (int)(work < sms ? work : sms);
+  e = launch_kernel(kern, dim3(grid), dim3(GEMM_THREADS), (size_t)L::DYN_BYTES, stream, ta, tb, p, f, (int)work);
+  if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "univl_gemm_fp8 launch: %s", cudaGetErrorString(e));
+  UNIVL_CHECK_LAUNCH("gemm_fp8");
+  return UNIVL_OK;
+}
+
 }  // namespace univl
 
 using namespace univl;
@@ -721,4 +933,58 @@ extern "C" int univl_gemm_bf16(const void* A, long long lda, int a_mn_major, con
   else rc = dispatch_major<64, 8>(amn, bmn, ta, tb, p, plan.splits, stream);
   if (rc != UNIVL_OK || p.part == nullptr) return rc;
   return partials_reduce(p.part, plan.splits, M, N, reinterpret_cast<float*>(out), ldo, stream);
+}
+
+// FP8 GEMM (see gemm_fp8_kernel).  epilogue 0: out bf16 [M, ldo] = acc + bias; 1: out e4m3 [M, ldo] with out_scale
+// [N/128, M] = gelu_erf(acc + bias) quantized per (row, 128-column block).
+extern "C" int univl_gemm_fp8(const void* A, long long lda, const float* a_scale, const void* B, long long ldb,
+                              const float* b_scale, int M, int N, int Kc, int epilogue, const float* bias, void* out,
+                              long long ldo, float* out_scale, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  UNIVL_CHECK_ARG(M > 0 && N > 0 && Kc > 0, "univl_gemm_fp8: empty problem M=%d N=%d K=%d", M, N, Kc);
+  UNIVL_CHECK_ARG(Kc % 128 == 0, "univl_gemm_fp8: K=%d must be a multiple of 128 (one scale per 128 columns)", Kc);
+  UNIVL_CHECK_ARG(N % 128 == 0, "univl_gemm_fp8: N=%d must be a multiple of 128 (one scale per 128 x 128 block)", N);
+  UNIVL_CHECK_ARG(epilogue == FP8_EPI_BIAS_BF16 || epilogue == FP8_EPI_GELU_E4M3,
+                  "univl_gemm_fp8: unknown epilogue %d", epilogue);
+  UNIVL_CHECK_ARG(A && B && a_scale && b_scale && bias && out, "univl_gemm_fp8: null operand, scale, bias or output");
+  UNIVL_CHECK_ARG(lda >= Kc && ldb >= Kc && (lda % 16) == 0 && (ldb % 16) == 0,
+                  "univl_gemm_fp8: lda/ldb must be >= K and multiples of 16 (got %lld, %lld, K=%d)", lda, ldb, Kc);
+  UNIVL_CHECK_ARG(((uintptr_t)A & 15) == 0 && ((uintptr_t)B & 15) == 0,
+                  "univl_gemm_fp8: A and B must be 16-byte aligned");
+  UNIVL_CHECK_ARG(ldo >= N, "univl_gemm_fp8: ldo=%lld must be >= N=%d", ldo, N);
+  if (epilogue == FP8_EPI_GELU_E4M3) {
+    UNIVL_CHECK_ARG(out_scale != nullptr, "univl_gemm_fp8: the GELU epilogue needs out_scale");
+    UNIVL_CHECK_ARG(((uintptr_t)out & 15) == 0 && (ldo % 16) == 0,
+                    "univl_gemm_fp8: the e4m3 output must be 16-byte aligned with ldo a multiple of 16 (got %lld)",
+                    ldo);
+  }
+
+  CUtensorMap ta, tb;
+  int rc;
+  if ((rc = make_tmap(&ta, A, M, Kc, lda, BLOCK_M, true))) return rc;
+  if ((rc = make_tmap(&tb, B, N, Kc, ldb, FP8_BLOCK_N, true))) return rc;
+
+  GemmParams p;
+  p.M = M; p.N = N; p.Kc = Kc;
+  p.k_blocks_per_split = Kc / 128;
+  p.epilogue = EPI_BIAS_BF16;
+  p.alpha = 1.f;
+  p.out = out; p.ldo = ldo;
+  p.bias = bias;
+  p.aux_in = nullptr; p.ld_aux_in = 0;
+  p.aux_out = nullptr; p.ld_aux_out = 0;
+  p.vec2 = (((uintptr_t)out % 4) == 0 && (ldo % 2) == 0) ? 1 : 0;
+  p.vec8 = (((uintptr_t)out % 16) == 0 && (ldo % 8) == 0) ? 1 : 0;
+  p.part = nullptr;
+  Fp8Params f;
+  f.a_scale = a_scale;
+  f.b_scale = b_scale;
+  f.out_q = reinterpret_cast<uint8_t*>(out);
+  f.out_scale = out_scale;
+  const bool pairs = (Kc / 128) % 2 == 0;
+  if (epilogue == FP8_EPI_BIAS_BF16)
+    return pairs ? launch_gemm_fp8<FP8_EPI_BIAS_BF16, true>(ta, tb, p, f, stream)
+                 : launch_gemm_fp8<FP8_EPI_BIAS_BF16, false>(ta, tb, p, f, stream);
+  return pairs ? launch_gemm_fp8<FP8_EPI_GELU_E4M3, true>(ta, tb, p, f, stream)
+               : launch_gemm_fp8<FP8_EPI_GELU_E4M3, false>(ta, tb, p, f, stream);
 }

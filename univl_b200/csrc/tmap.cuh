@@ -22,16 +22,19 @@ static inline EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-// 2D bf16 tensor map over a row-major [rows, cols] matrix with leading dimension ld (elements);
-// box = {64 cols (128 B, swizzled), box_rows}.
-static inline int make_tmap(CUtensorMap* tm, const void* ptr, long long rows, long long cols, long long ld, int box_rows) {
+// 2D bf16 (or, with e4m3, 1-byte) tensor map over a row-major [rows, cols] matrix with leading dimension ld
+// (elements); box = {128 B of columns (64 bf16 or 128 e4m3, swizzled), box_rows}.
+static inline int make_tmap(CUtensorMap* tm, const void* ptr, long long rows, long long cols, long long ld, int box_rows,
+                            bool e4m3 = false) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) return set_error(UNIVL_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable");
+  const int esize = e4m3 ? 1 : 2;
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {64, (cuuint32_t)box_rows};
+  cuuint64_t strides[1] = {(cuuint64_t)ld * esize};
+  cuuint32_t box[2] = {(cuuint32_t)(128 / esize), (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
+  CUresult r = fn(tm, e4m3 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
+                  const_cast<void*>(ptr), dims, strides, box, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)

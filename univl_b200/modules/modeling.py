@@ -8,6 +8,7 @@ observe: hidden states are bf16 (the kernels' activation type); everything needs
 """
 import logging
 import math
+import os
 
 import torch
 from torch import nn
@@ -27,6 +28,18 @@ logger = logging.getLogger(__name__)
 # torch allocations (measured on an H100 80GB HBM3 at a 400 W power limit, scripts/bench_retrieval_eval.py); the eval
 # path draws no stream-ordered kernel scratch.
 EVAL_PAIR_TOKENS = 1 << 18
+
+EVAL_PRECISIONS = ("bf16", "fp8")
+
+
+def eval_precision():
+    """UNIVL_EVAL_PRECISION, read on every tiled evaluation call: "bf16" (default) or "fp8", which runs the cross
+    layers' dense GEMMs over the pair tokens as block-scaled e4m3 GEMMs (CrossModel.encode_pairs_first_token_eval_fp8).
+    An environment variable, so that evaluation drivers pick it up unchanged."""
+    value = os.environ.get("UNIVL_EVAL_PRECISION", "bf16")
+    if value not in EVAL_PRECISIONS:
+        raise ValueError("UNIVL_EVAL_PRECISION must be one of %s, got %r" % ("/".join(EVAL_PRECISIONS), value))
+    return value
 
 
 class UniVLPreTrainedModel(PreTrainedModel, nn.Module):
@@ -232,9 +245,12 @@ class UniVL(UniVLPreTrainedModel):
         (text block x video block) into one fp32 [Nt, Nv] result.  With dropout off, the first cross layer's Q/K/V
         projections of a pair's token depend on its text or video row alone, so they are computed once per source row
         (CrossModel.first_layer_source_qkv) and every tile reads them in place.  Every other stage is row- or
-        sequence-local, so a pair's logit does not depend on the tiling."""
+        sequence-local, so a pair's logit does not depend on the tiling.  UNIVL_EVAL_PRECISION=fp8 (eval_precision)
+        runs the cross layers' dense GEMMs over the pair tokens in FP8, with weights quantized once per call."""
         Nt, W = attention_mask.shape
         Nv, F = video_mask.shape
+        fp8 = eval_precision() == "fp8" and len(self.cross.encoder.layer) > 1
+        qw = self.cross.fp8_eval_weights() if fp8 else None
         qkv = self.cross.first_layer_source_qkv(seq2d, vis2d, Nt, W, Nv, F)
         qkv_t, qkv_v = qkv[:Nt * W], qkv[Nt * W:]
         logits = torch.empty((Nt, Nv), dtype=torch.float32, device=seq2d.device)
@@ -243,9 +259,12 @@ class UniVL(UniVLPreTrainedModel):
             t1 = min(Nt, t0 + bt)
             for v0 in range(0, Nv, bv):
                 v1 = min(Nv, v0 + bv)
-                first = self.cross.encode_pairs_first_token_eval(
-                    seq2d[t0 * W:t1 * W], vis2d[v0 * F:v1 * F], attention_mask[t0:t1], video_mask[v0:v1],
-                    qkv_t[t0 * W:t1 * W], qkv_v[v0 * F:v1 * F])
+                tile_args = (seq2d[t0 * W:t1 * W], vis2d[v0 * F:v1 * F], attention_mask[t0:t1], video_mask[v0:v1],
+                             qkv_t[t0 * W:t1 * W], qkv_v[v0 * F:v1 * F])
+                if fp8:
+                    first = self.cross.encode_pairs_first_token_eval_fp8(*tile_args, qw)
+                else:
+                    first = self.cross.encode_pairs_first_token_eval(*tile_args)
                 u = self.cross.pooler.pre_activation(first, (t1 - t0) * (v1 - v0), 1)
                 tile = ops.PoolerSimFn.apply(u, self.similarity_dense.weight, self.similarity_dense.bias)
                 logits[t0:t1, v0:v1] = tile.view(t1 - t0, v1 - v0)

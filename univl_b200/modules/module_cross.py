@@ -123,6 +123,32 @@ class CrossModel(PreTrainedModel):
             return x
         return self.encoder.run_first_token(x, Nt * Nv, S, mask, start=1)
 
+    def fp8_eval_weights(self):
+        """Per layer, the e4m3 weights encode_pairs_first_token_eval_fp8 reads, quantized now from the fp32 parameters
+        (nothing is cached, so in-place weight edits and replicas are always current).  Needs >= 2 layers."""
+        layers = self.encoder.layer
+        out = []
+        for i, layer in enumerate(layers):
+            names = ("kv",) if i == len(layers) - 1 else ("o", "w1", "w2") if i == 0 else ("qkv", "o", "w1", "w2")
+            out.append(ops.fp8_layer_weights(_layer_params(layer), names))
+        return out
+
+    def encode_pairs_first_token_eval_fp8(self, text2d, video2d, text_mask, video_mask, qkv_t, qkv_v, qw):
+        """encode_pairs_first_token_eval with the dense GEMMs over the pair tokens in FP8 (qw = fp8_eval_weights()):
+        the first layer's attention output and FFN, the middle layers' Q/K/V projection, attention output and FFN, and
+        the last layer's K/V projection.  Needs >= 2 layers (with one, only token-0 rows remain, which stay bf16)."""
+        Nt, W = text_mask.shape
+        Nv, F = video_mask.shape
+        S = W + F
+        n_seq = Nt * Nv
+        x = self.embeddings.run(text2d, video2d, Nt, W, Nv, F, 1)
+        mask = ops.MaskSpec(text_mask, video_mask, all_pairs=1)
+        layers = self.encoder.layer
+        x = ops.pair_layer_eval_fp8(x, qkv_t, qkv_v, Nt, Nv, S, mask, _layer_params(layers[0]), qw[0])
+        for i in range(1, len(layers) - 1):
+            x = ops.encoder_layer_eval_fp8(x, n_seq, S, mask, _layer_params(layers[i]), qw[i])
+        return ops.cls_layer_eval_fp8(x, n_seq, S, mask, _layer_params(layers[-1]), qw[-1])
+
     def forward(self, concat_input, concat_type=None, attention_mask=None, output_all_encoded_layers=True):
         """API-parity entry: `concat_type` must be the reference's layout (0s for the text part then 1s)."""
         N, S, _ = concat_input.shape

@@ -281,6 +281,124 @@ def pair_layer_eval(x, qkv_a, qkv_b, Na, Nb, S, mask, params, first_token):
 
 
 # ---------------------------------------------------------------------------------------------------------
+# FP8 evaluation (include/univl_b200.h: e4m3 codes with power-of-two block scales, forward only)
+# ---------------------------------------------------------------------------------------------------------
+E4M3 = torch.float8_e4m3fn
+FP8_EPI_BIAS, FP8_EPI_GELU = 0, 1
+
+
+def quantize_e4m3_rows(x):
+    """bf16 [M, K] -> (e4m3 [M, K], fp32 scales [K/128, M]), one scale per (row, 128-column block)"""
+    _check2d(x, "quantize_e4m3_rows x")
+    M, K = x.shape
+    q = _empty((M, K), E4M3, x)
+    s = _empty((K // 128, M), F32, x)
+    call("univl_quantize_e4m3_rows", x.data_ptr(), x.stride(0), q.data_ptr(), q.stride(0), s.data_ptr(), M, K)
+    return q, s
+
+
+def quantize_e4m3_blocks(w, q=None, s=None):
+    """fp32 [N, K] -> (e4m3 [N, K], fp32 scales [N/128, K/128]), one scale per 128 x 128 block; q / s: optional
+    outputs (row slices of larger buffers)"""
+    _check2d(w, "quantize_e4m3_blocks w")
+    N, K = w.shape
+    q = _empty((N, K), E4M3, w) if q is None else q
+    s = _empty((N // 128, K // 128), F32, w) if s is None else s
+    call("univl_quantize_e4m3_blocks", w.data_ptr(), w.stride(0), q.data_ptr(), q.stride(0), s.data_ptr(), N, K)
+    return q, s
+
+
+def gemm_fp8(a, a_scale, b, b_scale, bias, gelu=False):
+    """a e4m3 [M, K] with a_scale [K/128, M], b e4m3 [N, K] with b_scale [N/128, K/128] ->
+    bf16 [M, N] = a b^T + bias, or with gelu (e4m3 [M, N], scales [N/128, M]) of gelu_erf(a b^T + bias)"""
+    _check2d(a, "gemm_fp8 A"); _check2d(b, "gemm_fp8 B")
+    M, K = a.shape
+    N = b.shape[0]
+    if gelu:
+        out = _empty((M, N), E4M3, a)
+        out_s = _empty((N // 128, M), F32, a)
+    else:
+        out = _empty((M, N), BF16, a)
+        out_s = None
+    call("univl_gemm_fp8", a.data_ptr(), a.stride(0), a_scale.data_ptr(), b.data_ptr(), b.stride(0),
+         b_scale.data_ptr(), M, N, K, FP8_EPI_GELU if gelu else FP8_EPI_BIAS, bias.data_ptr(), out.data_ptr(),
+         out.stride(0), ptr(out_s))
+    return (out, out_s) if gelu else out
+
+
+def fp8_layer_weights(params, names):
+    """The e4m3 weights (with their block scales) of one encoder layer's FP8 GEMMs, quantized from the fp32 parameters
+    (params as EncoderLayerFn) -> {name: (codes, scales)} for the names asked for: "qkv" (Q/K/V projection), "kv" (the
+    last layer's K/V projection), "o" (attention output), "w1", "w2" (FFN)."""
+    wa = dict(zip(ATT_KEYS, params[:10]))
+    wf = dict(zip(FFN_KEYS, params[10:16]))
+    H = wa["q"].shape[1]
+
+    def stacked(ws):
+        q = _empty((len(ws) * H, H), E4M3, ws[0])
+        s = _empty((len(ws) * H // 128, H // 128), F32, ws[0])
+        for i, w in enumerate(ws):
+            quantize_e4m3_blocks(w, q[i * H:(i + 1) * H], s[i * H // 128:(i + 1) * H // 128])
+        return q, s
+
+    make = {"qkv": lambda: stacked((wa["q"], wa["k"], wa["v"])), "kv": lambda: stacked((wa["k"], wa["v"])),
+            "o": lambda: quantize_e4m3_blocks(wa["o"]), "w1": lambda: quantize_e4m3_blocks(wf["w1"]),
+            "w2": lambda: quantize_e4m3_blocks(wf["w2"])}
+    return {n: make[n]() for n in names}
+
+
+def _fp8_layer_tail(ctx, x, params, qw):
+    """attention output dense + LayerNorm(x) and the FFN block of an encoder layer in evaluation, the three dense GEMMs
+    in FP8: ctx the attention context [T, H], x the layer input (the attention block's residual)"""
+    wa = dict(zip(ATT_KEYS, params[:10]))
+    wf = dict(zip(FFN_KEYS, params[10:16]))
+    drop = _Drop(0.0, 0.0, False)
+    ao = gemm_fp8(*quantize_e4m3_rows(ctx), *qw["o"], wa["bo"])
+    y, _, _ = layernorm_fwd(ao, x, wa["gamma"], wa["beta"], 0.0, 1, drop.seed, drop.stream())
+    h, hs = gemm_fp8(*quantize_e4m3_rows(y), *qw["w1"], wf["b1"], gelu=True)
+    fo = gemm_fp8(h, hs, *qw["w2"], wf["b2"])
+    out, _, _ = layernorm_fwd(fo, y, wf["gamma"], wf["beta"], 0.0, 1, drop.seed, drop.stream())
+    return out
+
+
+def pair_layer_eval_fp8(x, qkv_a, qkv_b, Na, Nb, S, mask, params, qw):
+    """pair_layer_eval for a layer that is not the stack's last, its dense GEMMs over the pair tokens in FP8
+    (qw holds "o", "w1", "w2" of fp8_layer_weights).  The attention core and the LayerNorms stay bf16."""
+    ctx = attention_pair_fwd(qkv_a, qkv_b, Na, Nb, S, mask)
+    return _fp8_layer_tail(ctx, x, params, qw)
+
+
+def encoder_layer_eval_fp8(x, n_seq, S, mask, params, qw):
+    """EncoderLayerFn in evaluation with the Q/K/V projection, attention output and FFN GEMMs in FP8 (qw holds "qkv",
+    "o", "w1", "w2" of fp8_layer_weights)"""
+    wa = dict(zip(ATT_KEYS, params[:10]))
+    H = x.shape[1]
+    qkv = gemm_fp8(*quantize_e4m3_rows(x), *qw["qkv"], rt.packed_bias(wa["bq"], wa["bk"], wa["bv"]))
+    drop = _Drop(0.0, 0.0, False)
+    ctx, _ = attention_fwd(qkv[:, :H], qkv[:, H:2 * H], qkv[:, 2 * H:], n_seq, S, S, mask, 0.0, drop.seed,
+                           drop.stream())
+    return _fp8_layer_tail(ctx, x, params, qw)
+
+
+def cls_layer_eval_fp8(x, n_seq, S, mask, params, qw):
+    """EncoderLayerClsFn in evaluation with the K/V projection of all n_seq * S rows in FP8 (qw holds "kv" of
+    fp8_layer_weights); everything on the n_seq token-0 rows (Q, attention output, FFN) stays bf16
+    -> [n_seq, H]"""
+    arena = rt.current()
+    wa = dict(zip(ATT_KEYS, params[:10]))
+    wf = dict(zip(FFN_KEYS, params[10:16]))
+    drop = _Drop(0.0, 0.0, False)
+    H = x.shape[1]
+    x0 = x.view(n_seq, S, H)[:, 0].contiguous()
+    kv = gemm_fp8(*quantize_e4m3_rows(x), *qw["kv"], rt.packed_bias(wa["bk"], wa["bv"]))
+    q = linear_fwd(x0, arena.bf16_qkv(wa["q"], wa["k"], wa["v"])[:H], wa["bq"])
+    ctx, _ = attention_fwd(q, kv[:, :H], kv[:, H:], n_seq, 1, S, mask, 0.0, drop.seed, drop.stream())
+    ao = linear_fwd(ctx, arena.bf16(wa["o"]), wa["bo"])
+    y, _, _ = layernorm_fwd(ao, x0, wa["gamma"], wa["beta"], 0.0, 1, drop.seed, drop.stream())
+    return ffn_block_fwd(y, wf, drop)[0]
+
+
+# ---------------------------------------------------------------------------------------------------------
 # transformer blocks (forward keeps a dict of saved tensors; backward consumes it)
 # ---------------------------------------------------------------------------------------------------------
 class _Drop:
