@@ -1,16 +1,18 @@
-"""Time every GEMM of the FT-Align cross encoder, and the 1536-row text / visual GEMMs, through ops.gemm.
+"""Time every GEMM of the FT-Align cross encoder, the 1536-row text / visual GEMMs and the small-K weight gradients,
+through ops.gemm.
 
 Each row is one GEMM as ops.py issues it (attn_block_fwd / attn_block_bwd / ffn_block_fwd / ffn_block_bwd): its
 operand majors, epilogue, bias, aux_in / aux_out and automatic tile-width / split-K plan.  The FT-Align cross encoder
 runs T = 98304 rows (32 x 32 all-pairs sequences of 96 tokens); its self-attention takes the fused QKV-projection +
 attention kernel, so the only QKV GEMMs of a cross layer are in the backward.  The text and visual stacks run 1536
-rows (batch 32 x 48 tokens).
+rows (batch 32 x 48 tokens); the first-token cross layer's query, output and FFN weights see 1024 rows (one per
+pair).  `--rows text` runs these small-K rows.
 
 Prints one JSON line per GEMM: ms (CUDA events over enough launches for >= --min_s seconds, after a warm-up),
 TFLOP/s (2 M N K), and the hardware bound max(FLOPs / 989 TFLOP/s, HBM bytes / 3.35 TB/s) — the H100 SXM data sheet's
 dense bf16 rate and HBM3 bandwidth (700 W figures) — naming which of the two it is and the share of it reached.  HBM
 bytes are the least the GEMM must move: A and B read once, the output written once (read and written for the
-accumulating epilogue), aux_in read, aux_out written; the split-K partial buffer is not counted.  The card's name,
+accumulating epilogue), aux_in read, aux_out written.  The card's name,
 power limit and maximum SM clock are printed first, and the SM clock is read again after every row.
 
 usage: python scripts/bench_gemm.py [--min_s 0.5] [--rows cross|text|all]
@@ -32,7 +34,7 @@ from univl_b200 import ops  # noqa: E402
 PEAK_FLOPS = 989e12
 PEAK_BYTES = 3.35e12
 H, I = 768, 3072
-T_CROSS, T_TEXT = 98304, 1536
+T_CROSS, T_TEXT, T_PAIRS = 98304, 1536, 1024
 EPI_NAME = {ops.EPI_BIAS: "bias", ops.EPI_GELU: "bias_gelu", ops.EPI_GELU_BWD: "gelu_bwd", ops.EPI_ADD: "add",
             ops.EPI_F32: "bias_f32", ops.EPI_ATOMIC: "atomic_f32"}
 
@@ -64,9 +66,17 @@ TEXT = {
     "text_ffn2_fwd": (T_TEXT, "fwd", H, I, ops.EPI_BIAS, True),
     "text_ffn2_dgrad_gelu_bwd": (T_TEXT, "dgrad", H, I, ops.EPI_GELU_BWD, False),
     "text_qkv_dgrad_add": (T_TEXT, "dgrad", 3 * H, H, ops.EPI_ADD, False),
+    "text_ffn2_wgrad": (T_TEXT, "wgrad", H, I, ops.EPI_ATOMIC, False),
     "text_ffn1_wgrad": (T_TEXT, "wgrad", I, H, ops.EPI_ATOMIC, False),
     "text_attn_out_wgrad": (T_TEXT, "wgrad", H, H, ops.EPI_ATOMIC, False),
+    "text_qkv_wgrad": (T_TEXT, "wgrad", 3 * H, H, ops.EPI_ATOMIC, False),
     "visual_in_fwd": (T_TEXT, "fwd", H, 1024, ops.EPI_BIAS, True),
+    "visual_in_wgrad": (T_TEXT, "wgrad", H, 1024, ops.EPI_ATOMIC, False),
+    # the first-token cross layer's query, output and FFN weights see one row per pair (32 x 32)
+    "cross2_q_wgrad": (T_PAIRS, "wgrad", H, H, ops.EPI_ATOMIC, False),
+    "cross2_attn_out_wgrad": (T_PAIRS, "wgrad", H, H, ops.EPI_ATOMIC, False),
+    "cross2_ffn1_wgrad": (T_PAIRS, "wgrad", I, H, ops.EPI_ATOMIC, False),
+    "cross2_ffn2_wgrad": (T_PAIRS, "wgrad", H, I, ops.EPI_ATOMIC, False),
 }
 
 

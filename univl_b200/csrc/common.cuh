@@ -268,6 +268,16 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 
 // ----------------------------------------------------------------------------
+// GPU-scope publication of data between CTAs (the GEMM's split-K fix-up)
+// ----------------------------------------------------------------------------
+__device__ __forceinline__ void fence_acq_rel_gpu() { asm volatile("fence.acq_rel.gpu;" ::: "memory"); }
+__device__ __forceinline__ unsigned atom_add_acq_rel_gpu(unsigned* addr, unsigned v) {
+  unsigned old;
+  asm volatile("atom.add.acq_rel.gpu.global.u32 %0, [%1], %2;" : "=r"(old) : "l"(addr), "r"(v) : "memory");
+  return old;
+}
+
+// ----------------------------------------------------------------------------
 // TMA (cp.async.bulk.tensor) — 2D tiled loads into shared memory
 // ----------------------------------------------------------------------------
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {

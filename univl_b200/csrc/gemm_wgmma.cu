@@ -25,6 +25,13 @@
 // producer's ring runs continuously across tiles, so the next tile's operands load while the epilogue runs.  Both
 // schedules give every output element the same chain of k16 wgmmas in the same k order and the same epilogue, so the
 // tile width does not change a bit of the result.
+// Split-K (fp32 weight gradients, EPI_ATOMIC_F32, K >= SPLIT_MIN_K or a forced split_k): a work item is a (tile,
+// split) pair.  Its epilogue stores alpha * acc into a scratch slot of its own, and the last of a tile's items to
+// arrive (per warp, counted on a zeroed counter) adds every split's slot in split order and then into the output —
+// in the owning warpgroup's epilogue, so under the ping-pong schedule it overlaps the other warpgroup's MMAs
+// (splitk_fixup).  No item waits for another.  Below SPLIT_MIN_K the automatic plan's splits are instead summed in
+// registers by one unsplit 64-wide work item per tile (GemmParams::kb_seg): the same segments, the same order, the
+// same bits.
 #include "common.cuh"
 #include "fp8.cuh"
 #include "tmap.cuh"
@@ -58,13 +65,23 @@ struct GemmParams {
   long long ld_aux_out;
   int vec2;  // 1 = every epilogue operand takes 2-element vector accesses (aligned base, even leading dimension)
   int vec8;  // 1 = the bf16 outputs (out, aux_out) take 16-byte stores of 8 columns (16-byte aligned base, ld % 8 == 0)
-  float* part;  // EPI_ATOMIC_F32 with split-K: [splits][M][N] partial sums, else null
+  // EPI_ATOMIC_F32 with splits > 1 (else null): the split-K fix-up's slots, [tiles][splits][2 halves][64 x BLOCK_N]
+  // floats in accumulator-fragment order, and its arrival counters, [tiles][2 halves][4 warps], zero at launch
+  float* slots;
+  unsigned* arrived;
+  int splits;
+  // EPI_ATOMIC_F32 on the 64-wide tile: a work item of more k-blocks than this sums its k range in segments of
+  // kb_seg k-blocks, t = 0, t += alpha * segment in k order, then out += t — the bits of a split-K plan with kb_seg
+  // k-blocks per split, without its scratch memory
+  int kb_seg;
 };
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;  // 64 bf16 = 128 bytes = one swizzle row
 constexpr int GEMM_THREADS = 384;
 constexpr int PLAN_SMS = 132;  // H100 SXM: the tile-width / split-K plan is a pure function of the problem
+// below it, an automatic split-K plan runs unsplit with in-register k-segment sums (see plan_gemm)
+constexpr int SPLIT_MIN_K = 4096;
 
 template <int BLOCK_N, int STAGES>
 struct GemmSmem {
@@ -104,31 +121,22 @@ __device__ __forceinline__ WorkItem decode_work(int w, int m_tiles, int n_tiles,
   return it;
 }
 
-// fused epilogue of the accumulator values of columns (col, col + 1) of one row; col is even.  split: the work item's
-// split-K index
-__device__ __forceinline__ void epi_pair(const GemmParams& p, int split, int row, int col, float v0, float v1) {
+// fused epilogue of the accumulator values of columns (col, col + 1) of one row; col is even.  alpha: the scale of
+// the accumulator values (p.alpha, or 1 for the split-K sums, which carry it already)
+__device__ __forceinline__ void epi_pair(const GemmParams& p, float alpha, int row, int col, float v0, float v1) {
   if (row >= p.M || col >= p.N) return;
   const bool two = col + 1 < p.N;
   const bool vec = two && p.vec2;
   const int epi = p.epilogue;
-  v0 *= p.alpha;
-  v1 *= p.alpha;
+  v0 *= alpha;
+  v1 *= alpha;
   if (p.bias != nullptr && (epi == EPI_BIAS_BF16 || epi == EPI_BIAS_GELU_BF16 || epi == EPI_BIAS_F32)) {
     v0 += __ldg(p.bias + col);
     if (two) v1 += __ldg(p.bias + col + 1);
   }
-  if (epi == EPI_ATOMIC_F32 && p.part != nullptr) {  // this split's partial sums (partials_reduce adds them in order)
-    float* o = p.part + ((long long)split * p.M + row) * p.N + col;
-    if (two && (p.N & 1) == 0) *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
-    else {
-      o[0] = v0;
-      if (two) o[1] = v1;
-    }
-    return;
-  }
   if (epi == EPI_ATOMIC_F32 || epi == EPI_BIAS_F32) {
     float* o = reinterpret_cast<float*>(p.out) + (long long)row * p.ldo + col;
-    if (epi == EPI_ATOMIC_F32) {  // one split: this thread is the element's only writer in the launch
+    if (epi == EPI_ATOMIC_F32) {  // this thread is the element's only writer in the launch (split-K: the last arriver's)
       if (vec) {
         float2 a = *reinterpret_cast<float2*>(o);
         *reinterpret_cast<float2*>(o) = make_float2(a.x + v0, a.y + v1);
@@ -213,8 +221,8 @@ __device__ __forceinline__ uint4 quad_transpose(uint32_t w0, uint32_t w1, uint32
   return make_uint4(w0, w1, w2, w3);
 }
 
-// Unchecked epilogue of a work item whose 128 x BLOCK_N tile lies wholly inside M x N, with p.vec2 set (and, for
-// split-K partials, N even): no bounds checks, every access a 2-element vector.  The epilogue is a template argument,
+// Unchecked epilogue of a work item whose 128 x BLOCK_N tile lies wholly inside M x N, with p.vec2 set: no bounds
+// checks, every access a 2-element vector.  The epilogue is a template argument,
 // so the fragment walk is straight-line code.  It runs in chunks of EPI_CHUNK 8-column groups.  Each chunk's global
 // loads (bias, aux_in, the accumulated output) are issued together, and before the previous chunk's arithmetic, so
 // their latencies overlap each other and that arithmetic instead of adding up.  Loading ahead of the previous chunk's
@@ -223,13 +231,13 @@ __device__ __forceinline__ uint4 quad_transpose(uint32_t w0, uint32_t w1, uint32
 // before its result is stored (by the same thread, or with WIDE by a lane of the same quad after the shuffles).
 // It computes exactly what epi_pair computes: the same fp32 operations in the same order, with __fmul_rn / __fadd_rn
 // so that alpha * acc and the add after it stay two roundings and are not contracted to an FFMA.
-// BIAS: p.bias is set (bias epilogues); PART: p.part is set (EPI_ATOMIC_F32 with split-K).
+// BIAS: p.bias is set (bias epilogues).  alpha: as in epi_pair.
 // WIDE (p.vec8, bf16 outputs): the four lanes of a quad, which hold 2 columns each of the same 8-column groups,
 // exchange their packed results (quad_transpose) so that each lane stores one group whole, 16 bytes.  A warp's store
 // then covers 64 contiguous bytes (two full 32-byte sectors) of each of its 8 rows, with a quarter of the store
 // instructions, where the 4-byte stores cover 16 bytes (half a sector) of each row.
-template <int EPI, bool BIAS, bool PART, int BLOCK_N, bool WIDE = false>
-__device__ __forceinline__ void epi_tile(const GemmParams& p, int split, int row, int col0,
+template <int EPI, bool BIAS, int BLOCK_N, bool WIDE = false>
+__device__ __forceinline__ void epi_tile(const GemmParams& p, float alpha, int row, int col0,
                                          const float (&acc)[BLOCK_N / 2]) {
   constexpr int GROUPS = BLOCK_N / 8;
   // WIDE holds a quad's results for the shuffles: half-size chunks keep the 256-wide tile free of spills
@@ -238,19 +246,16 @@ __device__ __forceinline__ void epi_tile(const GemmParams& p, int split, int row
   constexpr bool AUX = EPI == EPI_GELU_BWD_BF16 || EPI == EPI_ADD_BF16;
   constexpr bool OUT_F32 = EPI == EPI_BIAS_F32 || EPI == EPI_ATOMIC_F32;
   static_assert(!(WIDE && OUT_F32), "16-byte stores are for the bf16 outputs");
-  constexpr bool ACCUM = EPI == EPI_ATOMIC_F32 && !PART;  // one split: out += alpha * acc
-  const float alpha = p.alpha;
+  constexpr bool ACCUM = EPI == EPI_ATOMIC_F32;  // out += alpha * acc
   const int q = threadIdx.x & 3;
   const float* bias = p.bias + col0;
   const bf16* ax = p.aux_in + (long long)row * p.ld_aux_in + col0;
   const long long ax8 = 8 * p.ld_aux_in;
   bf16* ao = p.aux_out + (long long)row * p.ld_aux_out + col0;
   const long long ao8 = 8 * p.ld_aux_out;
-  const long long ld = PART ? (long long)p.N : p.ldo;
-  const long long o8 = 8 * ld;
-  float* of = PART ? p.part + ((long long)split * p.M + row) * p.N + col0
-                   : reinterpret_cast<float*>(p.out) + (long long)row * ld + col0;
-  bf16* ob = reinterpret_cast<bf16*>(p.out) + (long long)row * ld + col0;
+  const long long o8 = 8 * p.ldo;
+  float* of = reinterpret_cast<float*>(p.out) + (long long)row * p.ldo + col0;
+  bf16* ob = reinterpret_cast<bf16*>(p.out) + (long long)row * p.ldo + col0;
   // two load buffers, alternating between chunks
   float b[2][CHUNK][2];
   uint32_t x[2][CHUNK][2];
@@ -337,58 +342,141 @@ __device__ __forceinline__ void epi_tile(const GemmParams& p, int split, int row
 // output take the unchecked epi_tile, edge tiles and launches without 2-element vector access the checked per-pair
 // epi_pair.
 template <int BLOCK_N>
-__device__ __forceinline__ void epilogue_block(const GemmParams& p, bool inside, int split, int n0, int row, int col0,
-                                               const float (&acc)[BLOCK_N / 2]) {
+__device__ __forceinline__ void epilogue_block(const GemmParams& p, bool inside, float alpha, int n0, int row,
+                                               int col0, const float (&acc)[BLOCK_N / 2]) {
   if (inside) {
     const bool bias = p.bias != nullptr;
     const bool wide = p.vec8;
     switch (p.epilogue) {
       case EPI_BIAS_BF16:
         if (wide) {
-          if (bias) epi_tile<EPI_BIAS_BF16, true, false, BLOCK_N, true>(p, split, row, col0, acc);
-          else epi_tile<EPI_BIAS_BF16, false, false, BLOCK_N, true>(p, split, row, col0, acc);
+          if (bias) epi_tile<EPI_BIAS_BF16, true, BLOCK_N, true>(p, alpha, row, col0, acc);
+          else epi_tile<EPI_BIAS_BF16, false, BLOCK_N, true>(p, alpha, row, col0, acc);
         } else {
-          if (bias) epi_tile<EPI_BIAS_BF16, true, false, BLOCK_N>(p, split, row, col0, acc);
-          else epi_tile<EPI_BIAS_BF16, false, false, BLOCK_N>(p, split, row, col0, acc);
+          if (bias) epi_tile<EPI_BIAS_BF16, true, BLOCK_N>(p, alpha, row, col0, acc);
+          else epi_tile<EPI_BIAS_BF16, false, BLOCK_N>(p, alpha, row, col0, acc);
         }
         break;
       case EPI_BIAS_GELU_BF16:
         if (wide) {
-          if (bias) epi_tile<EPI_BIAS_GELU_BF16, true, false, BLOCK_N, true>(p, split, row, col0, acc);
-          else epi_tile<EPI_BIAS_GELU_BF16, false, false, BLOCK_N, true>(p, split, row, col0, acc);
+          if (bias) epi_tile<EPI_BIAS_GELU_BF16, true, BLOCK_N, true>(p, alpha, row, col0, acc);
+          else epi_tile<EPI_BIAS_GELU_BF16, false, BLOCK_N, true>(p, alpha, row, col0, acc);
         } else {
-          if (bias) epi_tile<EPI_BIAS_GELU_BF16, true, false, BLOCK_N>(p, split, row, col0, acc);
-          else epi_tile<EPI_BIAS_GELU_BF16, false, false, BLOCK_N>(p, split, row, col0, acc);
+          if (bias) epi_tile<EPI_BIAS_GELU_BF16, true, BLOCK_N>(p, alpha, row, col0, acc);
+          else epi_tile<EPI_BIAS_GELU_BF16, false, BLOCK_N>(p, alpha, row, col0, acc);
         }
         break;
       case EPI_GELU_BWD_BF16:
-        if (wide) epi_tile<EPI_GELU_BWD_BF16, false, false, BLOCK_N, true>(p, split, row, col0, acc);
-        else epi_tile<EPI_GELU_BWD_BF16, false, false, BLOCK_N>(p, split, row, col0, acc);
+        if (wide) epi_tile<EPI_GELU_BWD_BF16, false, BLOCK_N, true>(p, alpha, row, col0, acc);
+        else epi_tile<EPI_GELU_BWD_BF16, false, BLOCK_N>(p, alpha, row, col0, acc);
         break;
       case EPI_ADD_BF16:
-        if (wide) epi_tile<EPI_ADD_BF16, false, false, BLOCK_N, true>(p, split, row, col0, acc);
-        else epi_tile<EPI_ADD_BF16, false, false, BLOCK_N>(p, split, row, col0, acc);
+        if (wide) epi_tile<EPI_ADD_BF16, false, BLOCK_N, true>(p, alpha, row, col0, acc);
+        else epi_tile<EPI_ADD_BF16, false, BLOCK_N>(p, alpha, row, col0, acc);
         break;
       case EPI_BIAS_F32:
-        if (bias) epi_tile<EPI_BIAS_F32, true, false, BLOCK_N>(p, split, row, col0, acc);
-        else epi_tile<EPI_BIAS_F32, false, false, BLOCK_N>(p, split, row, col0, acc);
+        if (bias) epi_tile<EPI_BIAS_F32, true, BLOCK_N>(p, alpha, row, col0, acc);
+        else epi_tile<EPI_BIAS_F32, false, BLOCK_N>(p, alpha, row, col0, acc);
         break;
       default:
-        if (p.part != nullptr) epi_tile<EPI_ATOMIC_F32, false, true, BLOCK_N>(p, split, row, col0, acc);
-        else epi_tile<EPI_ATOMIC_F32, false, false, BLOCK_N>(p, split, row, col0, acc);
+        epi_tile<EPI_ATOMIC_F32, false, BLOCK_N>(p, alpha, row, col0, acc);
     }
   } else {
 #pragma unroll
     for (int j = 0; j < BLOCK_N / 8; ++j) {
       if (n0 + j * 8 >= p.N) break;  // warp-uniform
-      epi_pair(p, split, row, col0 + j * 8, acc[4 * j], acc[4 * j + 1]);
-      epi_pair(p, split, row + 8, col0 + j * 8, acc[4 * j + 2], acc[4 * j + 3]);
+      epi_pair(p, alpha, row, col0 + j * 8, acc[4 * j], acc[4 * j + 1]);
+      epi_pair(p, alpha, row + 8, col0 + j * 8, acc[4 * j + 2], acc[4 * j + 3]);
     }
   }
 }
 
 __device__ __forceinline__ bool tile_inside(const GemmParams& p, const WorkItem& wi, int bn) {
-  return p.vec2 && wi.m0 + BLOCK_M <= p.M && wi.n0 + bn <= p.N && (p.part == nullptr || (p.N & 1) == 0);
+  return p.vec2 && wi.m0 + BLOCK_M <= p.M && wi.n0 + bn <= p.N;
+}
+
+// In-kernel split-K fix-up of one warp's share (16 rows x BLOCK_N) of a tile half (rows 64 half .. 64 half + 63).
+// The work item stores alpha * acc into its slot, in fragment order (float4 j of warpgroup thread t at j * 128 + t,
+// so every thread later reads back exactly the values it wrote, 16 bytes at a time), and publishes it: a release
+// fence by every lane, then one acq_rel add on the warp's counter.  The item whose add brings the counter to
+// p.splits is the last arriver: it returns true with acc = t, where t = 0, t += alpha * acc_s for s = 0 .. splits - 1
+// in split order (its own split from its registers, the others from their slots) — the order partials_reduce adds
+// rows in, so the sum does not depend on which item arrives last.  Every other item returns false and is done.  No
+// warp ever waits for another, so the kernel cannot deadlock however few of its CTAs are resident.
+template <int BLOCK_N>
+__device__ __forceinline__ bool splitk_fixup(const GemmParams& p, int tile, int half, int split, float alpha,
+                                             float (&acc)[BLOCK_N / 2]) {
+  constexpr int V = BLOCK_N / 8;  // float4 per thread
+  // float4 loads in flight per slot: 8 spills the 256-wide tile's 128 accumulator registers (check with -Xptxas -v)
+  constexpr int CHUNK = BLOCK_N == 256 ? 4 : 8;
+  const int t = threadIdx.x & 127;
+  const int lane = t & 31;
+  const long long slot = 64LL * BLOCK_N;  // floats per (tile, split, half)
+  float4* base = reinterpret_cast<float4*>(p.slots + ((long long)tile * p.splits * 2 + half) * slot) + t;
+  float4* mine = base + split * (2 * slot / 4);
+#pragma unroll
+  for (int j = 0; j < V; ++j) {
+#pragma unroll
+    for (int e = 0; e < 4; ++e) acc[4 * j + e] = __fmul_rn(acc[4 * j + e], alpha);
+    __stcg(mine + j * 128, make_float4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]));
+  }
+  fence_acq_rel_gpu();
+  __syncwarp();
+  unsigned before = 0;
+  if (lane == 0) before = atom_add_acq_rel_gpu(p.arrived + (tile * 2 + half) * 4 + (t >> 5), 1u);
+  before = __shfl_sync(0xffffffffu, before, 0);
+  if (before != (unsigned)p.splits - 1) return false;
+  fence_acq_rel_gpu();
+#pragma unroll
+  for (int j0 = 0; j0 < V; j0 += CHUNK) {
+    float4 s4[CHUNK];
+#pragma unroll
+    for (int j = 0; j < CHUNK; ++j) s4[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int s = 0; s < p.splits; ++s) {
+      float4 v[CHUNK];
+      if (s == split) {
+#pragma unroll
+        for (int j = 0; j < CHUNK; ++j) {
+          const int a = 4 * (j0 + j);
+          v[j] = make_float4(acc[a], acc[a + 1], acc[a + 2], acc[a + 3]);
+        }
+      } else {
+        const float4* src = base + s * (2 * slot / 4);
+#pragma unroll
+        for (int j = 0; j < CHUNK; ++j) v[j] = __ldcg(src + (j0 + j) * 128);
+      }
+#pragma unroll
+      for (int j = 0; j < CHUNK; ++j) {
+        s4[j].x = __fadd_rn(s4[j].x, v[j].x);
+        s4[j].y = __fadd_rn(s4[j].y, v[j].y);
+        s4[j].z = __fadd_rn(s4[j].z, v[j].z);
+        s4[j].w = __fadd_rn(s4[j].w, v[j].w);
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < CHUNK; ++j) {
+      const int a = 4 * (j0 + j);
+      acc[a] = s4[j].x;
+      acc[a + 1] = s4[j].y;
+      acc[a + 2] = s4[j].z;
+      acc[a + 3] = s4[j].w;
+    }
+  }
+  return true;
+}
+
+// the split-K fix-up (when p.slots is set) and then the epilogue of one tile half; a split-K item that is not its
+// tile's last arriver has no epilogue.  alpha: the scale of acc (1 for in-register k-segment sums, which carry it)
+template <int BLOCK_N>
+__device__ __forceinline__ void finish_block(const GemmParams& p, const WorkItem& wi, int n_tiles, int kb_per,
+                                             bool inside, float alpha, int half, int row, int col0,
+                                             float (&acc)[BLOCK_N / 2]) {
+  if (p.slots != nullptr) {
+    const int tile = (wi.m0 / BLOCK_M) * n_tiles + wi.n0 / BLOCK_N;
+    if (!splitk_fixup<BLOCK_N>(p, tile, half, wi.kb_begin / kb_per, alpha, acc)) return;
+    alpha = 1.f;  // t carries it
+  }
+  epilogue_block<BLOCK_N>(p, inside, alpha, wi.n0, row, col0, acc);
 }
 
 // named barriers of the ping-pong hand-off: consumer warpgroup c waits on TURN_BAR + c for its turn at the MMAs
@@ -438,6 +526,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
                   const GemmParams p, const int num_work) {
   using L = GemmSmem<BLOCK_N, STAGES>;
   constexpr bool PING = BLOCK_N <= 128;  // ping-pong schedule (else cooperative), see the top of this file
+  // in-register k-segment sums (p.kb_seg): the 64-wide tile has the registers for a second accumulator set
+  constexpr bool FOLD = BLOCK_N == 64;
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -510,7 +600,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       if (t == 0) mbar_arrive(&empty_bar[prev_s]);
       const int row = wi.m0 + c * 64 + warp * 16 + (lane >> 2);
       const int col0 = wi.n0 + 2 * (lane & 3);
-      epilogue_block<BLOCK_N>(p, tile_inside(p, wi, BLOCK_N), wi.kb_begin / kb_per, wi.n0, row, col0, acc);
+      finish_block<BLOCK_N>(p, wi, n_tiles, kb_per, tile_inside(p, wi, BLOCK_N), p.alpha, c, row, col0, acc);
     }
   } else {
     // ------------------------------ ping-pong consumers ------------------------------
@@ -535,48 +625,81 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       float acc[2][BLOCK_N / 2];  // rows 0-63 and 64-127 of the tile
 #pragma unroll
       for (int e = 0; e < BLOCK_N / 2; ++e) acc[0][e] = acc[1][e] = 0.f;
+      // k-segments (see GemmParams::kb_seg): the MMAs restart from zero at each segment, and sum += alpha * acc
+      // after it, in k order
+      const bool fold = FOLD && p.kb_seg < wi.num_kb;
+      const int seg = fold ? p.kb_seg : wi.num_kb;
+      float sum[2][FOLD ? BLOCK_N / 2 : 1];
+      if constexpr (FOLD) {
+#pragma unroll
+        for (int e = 0; e < BLOCK_N / 2; ++e) sum[0][e] = sum[1][e] = 0.f;
+      }
       if (j > 0) named_bar(TURN_BAR + c, 256);
-      int prev_s = -1;
-      for (int i = 0; i < wi.num_kb; ++i, ++it) {
-        const int s = it % STAGES;
-        const uint32_t ph = (it / STAGES) & 1;
-        mbar_wait(&full_bar[s], ph);
-        // rows 64-127 of A start 8 KB into the stage in both layouts, as in the cooperative schedule
-        const uint32_t sa = smem_u32(smem + s * L::STAGE_BYTES);
-        const uint32_t sb = sa + L::A_BYTES;
-        wgmma_fence();
+      for (int i0 = 0; i0 < wi.num_kb; i0 += seg) {
+        const int i1 = min(wi.num_kb, i0 + seg);
+        int prev_s = -1;
+        for (int i = i0; i < i1; ++i, ++it) {
+          const int s = it % STAGES;
+          const uint32_t ph = (it / STAGES) & 1;
+          mbar_wait(&full_bar[s], ph);
+          // rows 64-127 of A start 8 KB into the stage in both layouts, as in the cooperative schedule
+          const uint32_t sa = smem_u32(smem + s * L::STAGE_BYTES);
+          const uint32_t sb = sa + L::A_BYTES;
+          wgmma_fence();
+          fence_regs(acc[0]);
+          fence_regs(acc[1]);
+#pragma unroll
+          for (int k = 0; k < BLOCK_K / 16; ++k) {
+            const uint64_t db = B_MN ? make_smem_desc_sw128(sb + k * 2048, BLOCK_K * 128, 1024)
+                                     : make_smem_desc_sw128(sb + k * 32, 16, 1024);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const uint32_t sah = sa + h * (64 * 128);
+              const uint64_t da = A_MN ? make_smem_desc_sw128(sah + k * 2048, BLOCK_K * 128, 1024)
+                                       : make_smem_desc_sw128(sah + k * 32, 16, 1024);
+              WgmmaSS<BLOCK_N>::template mma<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc[h], da, db,
+                                                                          (i > i0 || k > 0) ? 1 : 0);
+            }
+          }
+          wgmma_commit();
+          fence_regs(acc[0]);
+          fence_regs(acc[1]);
+          wgmma_wait<1>();  // the previous k-block's MMAs have read their stage
+          if (prev_s >= 0 && t == 0) mbar_arrive(&empty_bar[prev_s]);
+          prev_s = s;
+        }
+        if (i1 == wi.num_kb && w + (int)gridDim.x < num_work)
+          named_bar_arrive(TURN_BAR + (c ^ 1), 256);  // the next item's turn
+        wgmma_wait<0>();
         fence_regs(acc[0]);
         fence_regs(acc[1]);
+        if (t == 0) mbar_arrive(&empty_bar[prev_s]);
+        if constexpr (FOLD) {
+          if (fold) {
 #pragma unroll
-        for (int k = 0; k < BLOCK_K / 16; ++k) {
-          const uint64_t db = B_MN ? make_smem_desc_sw128(sb + k * 2048, BLOCK_K * 128, 1024)
-                                   : make_smem_desc_sw128(sb + k * 32, 16, 1024);
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const uint32_t sah = sa + h * (64 * 128);
-            const uint64_t da = A_MN ? make_smem_desc_sw128(sah + k * 2048, BLOCK_K * 128, 1024)
-                                     : make_smem_desc_sw128(sah + k * 32, 16, 1024);
-            WgmmaSS<BLOCK_N>::template mma<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc[h], da, db, (i > 0 || k > 0) ? 1 : 0);
+            for (int e = 0; e < BLOCK_N / 2; ++e) {
+              sum[0][e] = __fadd_rn(sum[0][e], __fmul_rn(acc[0][e], p.alpha));
+              sum[1][e] = __fadd_rn(sum[1][e], __fmul_rn(acc[1][e], p.alpha));
+            }
           }
         }
-        wgmma_commit();
-        fence_regs(acc[0]);
-        fence_regs(acc[1]);
-        wgmma_wait<1>();  // the previous k-block's MMAs have read their stage
-        if (prev_s >= 0 && t == 0) mbar_arrive(&empty_bar[prev_s]);
-        prev_s = s;
       }
-      if (w + (int)gridDim.x < num_work) named_bar_arrive(TURN_BAR + (c ^ 1), 256);  // the next item's turn
-      wgmma_wait<0>();
-      fence_regs(acc[0]);
-      fence_regs(acc[1]);
-      if (t == 0) mbar_arrive(&empty_bar[prev_s]);
+      float alpha = p.alpha;
+      if constexpr (FOLD) {
+        if (fold) {
+#pragma unroll
+          for (int e = 0; e < BLOCK_N / 2; ++e) {
+            acc[0][e] = sum[0][e];
+            acc[1][e] = sum[1][e];
+          }
+          alpha = 1.f;  // the sums carry it
+        }
+      }
       const bool inside = tile_inside(p, wi, BLOCK_N);
-      const int split = wi.kb_begin / kb_per;
       const int row = wi.m0 + warp * 16 + (lane >> 2);
       const int col0 = wi.n0 + 2 * (lane & 3);
-      epilogue_block<BLOCK_N>(p, inside, split, wi.n0, row, col0, acc[0]);
-      epilogue_block<BLOCK_N>(p, inside, split, wi.n0, row + 64, col0, acc[1]);
+      finish_block<BLOCK_N>(p, wi, n_tiles, kb_per, inside, alpha, 0, row, col0, acc[0]);
+      finish_block<BLOCK_N>(p, wi, n_tiles, kb_per, inside, alpha, 1, row + 64, col0, acc[1]);
     }
   }
 }
@@ -749,13 +872,13 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
     const int col0 = wi.n0 + 2 * (lane & 3);
     if constexpr (EPI == FP8_EPI_BIAS_BF16) {
       if (tile_inside(p, wi, FP8_BLOCK_N)) {
-        if (p.vec8) epi_tile<EPI_BIAS_BF16, true, false, FP8_BLOCK_N, true>(p, 0, row, col0, acc);
-        else epi_tile<EPI_BIAS_BF16, true, false, FP8_BLOCK_N>(p, 0, row, col0, acc);
+        if (p.vec8) epi_tile<EPI_BIAS_BF16, true, FP8_BLOCK_N, true>(p, p.alpha, row, col0, acc);
+        else epi_tile<EPI_BIAS_BF16, true, FP8_BLOCK_N>(p, p.alpha, row, col0, acc);
       } else {
 #pragma unroll
         for (int j = 0; j < FP8_BLOCK_N / 8; ++j) {
-          epi_pair(p, 0, row, col0 + j * 8, acc[4 * j], acc[4 * j + 1]);
-          epi_pair(p, 0, row + 8, col0 + j * 8, acc[4 * j + 2], acc[4 * j + 3]);
+          epi_pair(p, p.alpha, row, col0 + j * 8, acc[4 * j], acc[4 * j + 1]);
+          epi_pair(p, p.alpha, row + 8, col0 + j * 8, acc[4 * j + 2], acc[4 * j + 3]);
         }
       }
     } else {
@@ -813,7 +936,7 @@ using namespace univl;
 
 namespace {
 struct GemmPlan {
-  int bn, splits, kb_per;
+  int bn, splits, kb_per, kb_seg;
 };
 // tile width and split-K factor for a problem — a pure function of the arguments, shared by the launcher and by
 // univl_gemm_plan
@@ -855,9 +978,21 @@ int plan_gemm(int M, int N, int Kc, int epilogue, int block_n, int split_k, Gemm
     }
     if (splits > total_kb) splits = total_kb;
   }
-  const int kb_per = (total_kb + splits - 1) / splits;
+  int kb_per = (total_kb + splits - 1) / splits;
   splits = (total_kb + kb_per - 1) / kb_per;  // no empty split
-  plan->bn = bn; plan->splits = splits; plan->kb_per = kb_per;
+  int kb_seg = kb_per;
+  // Below SPLIT_MIN_K the automatic split plan cuts K into 2-6 k-blocks per split, and its scratch partials cost
+  // more than the SMs the splits fill.  Such a weight gradient runs unsplit on the 64-wide ping-pong tile instead,
+  // summing the same k-segments in registers in the same order (GemmParams::kb_seg), so it computes the bits of the
+  // split plan.  On an H100 SXM every 1536- and 1024-row weight gradient of the FT-Align step ran unsplit at 64 wide
+  // in about half the time of its split plan (768 x 768 x 1536: 0.014 against 0.027 ms; 3072 x 768 x 1536: 0.026
+  // against 0.052).
+  if (epilogue == EPI_ATOMIC_F32 && block_n == 0 && split_k == 0 && Kc < SPLIT_MIN_K && splits > 1) {
+    bn = 64;
+    splits = 1;
+    kb_per = total_kb;
+  }
+  plan->bn = bn; plan->splits = splits; plan->kb_per = kb_per; plan->kb_seg = kb_seg;
   return UNIVL_OK;
 }
 }  // namespace
@@ -923,16 +1058,29 @@ extern "C" int univl_gemm_bf16(const void* A, long long lda, int a_mn_major, con
   bool vec8 = !out_f32 && ((uintptr_t)out % 16) == 0 && (ldo % 8) == 0;
   if (aux_out != nullptr) vec8 = vec8 && ((uintptr_t)aux_out % 16) == 0 && (ld_aux_out % 8) == 0;
   p.vec8 = vec8 ? 1 : 0;
-  p.part = nullptr;
-  if (plan.splits > 1)
-    if ((rc = scratch_alloc((void**)&p.part, (size_t)plan.splits * M * N * sizeof(float), stream))) return rc;
+  p.slots = nullptr;
+  p.arrived = nullptr;
+  p.splits = plan.splits;
+  p.kb_seg = plan.kb_seg;
+  if (plan.splits > 1) {  // the split-K fix-up's slots and arrival counters, one stream-ordered block
+    const long long tiles = (long long)((M + BLOCK_M - 1) / BLOCK_M) * ((N + bn - 1) / bn);
+    const size_t slot_bytes = (size_t)tiles * plan.splits * BLOCK_M * bn * sizeof(float);
+    const size_t counter_bytes = (size_t)tiles * 8 * sizeof(unsigned);
+    if ((rc = scratch_alloc((void**)&p.slots, slot_bytes + counter_bytes, stream))) return rc;
+    p.arrived = reinterpret_cast<unsigned*>(p.slots + slot_bytes / sizeof(float));
+    const cudaError_t e = cudaMemsetAsync(p.arrived, 0, counter_bytes, stream);
+    if (e != cudaSuccess) {
+      cudaFreeAsync(p.slots, stream);
+      return set_error(UNIVL_ERR_CUDA, "gemm split-K counters: %s", cudaGetErrorString(e));
+    }
+  }
 
   const bool amn = a_mn_major != 0, bmn = b_mn_major != 0;
   if (bn == 256) rc = dispatch_major<256, 4>(amn, bmn, ta, tb, p, plan.splits, stream);
   else if (bn == 128) rc = dispatch_major<128, 6>(amn, bmn, ta, tb, p, plan.splits, stream);
   else rc = dispatch_major<64, 8>(amn, bmn, ta, tb, p, plan.splits, stream);
-  if (rc != UNIVL_OK || p.part == nullptr) return rc;
-  return partials_reduce(p.part, plan.splits, M, N, reinterpret_cast<float*>(out), ldo, stream);
+  if (p.slots != nullptr) cudaFreeAsync(p.slots, stream);
+  return rc;
 }
 
 // FP8 GEMM (see gemm_fp8_kernel).  epilogue 0: out bf16 [M, ldo] = acc + bias; 1: out e4m3 [M, ldo] with out_scale
@@ -975,7 +1123,10 @@ extern "C" int univl_gemm_fp8(const void* A, long long lda, const float* a_scale
   p.aux_out = nullptr; p.ld_aux_out = 0;
   p.vec2 = (((uintptr_t)out % 4) == 0 && (ldo % 2) == 0) ? 1 : 0;
   p.vec8 = (((uintptr_t)out % 16) == 0 && (ldo % 8) == 0) ? 1 : 0;
-  p.part = nullptr;
+  p.slots = nullptr;
+  p.arrived = nullptr;
+  p.splits = 1;
+  p.kb_seg = p.k_blocks_per_split;
   Fp8Params f;
   f.a_scale = a_scale;
   f.b_scale = b_scale;
