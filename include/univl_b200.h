@@ -225,6 +225,26 @@ int univl_softmax_xent_bwd(const float* logits, long long ld, const long long* l
                            const float* lse, const float* sum_count, const float* gscale, void* dlogits,
                            long long ld_d, int T, int V, int target_mode, long long ignore_index, int groups,
                            void* stream);
+/* The same CrossEntropyLoss(ignore_index = -1) for target_mode 0 over the tied vocabulary projection, with the logits
+ * never written to memory (module_bert.py:327-330 + modeling.py:253, :275):
+ *   logit[r, c] = x[r, :] . W[c, :] + bias[c]   (x bf16 [T, Kc], W bf16 [V, Kc], both K-major; bias fp32 [V], nullable)
+ * computed by the wgmma GEMM's mainloop with EPI_BIAS_F32's bits.
+ * univl_vocab_xent_fwd: loss, lse [T] (0 for unscored rows) and sum_count [2 G] as univl_softmax_xent_fwd defines them;
+ *   the per-group sums are taken in a fixed order (no floating-point atomics), so the result is deterministic.
+ *   workspace: device memory of at least univl_vocab_xent_workspace(T, V) bytes, 16-byte aligned, used within the call
+ *   on `stream` only (so one buffer per stream; safe under CUDA-graph capture).  Labels must be -1 or in [0, V); any
+ *   other label makes the loss NaN.
+ * univl_vocab_xent_bwd: recomputes the logits and writes dlogits bf16 [T, ld_d] = univl_softmax_xent_bwd's result from
+ *   them: (exp(logit - lse) - onehot) (gscale / G) / count[group] for scored rows, 0 for unscored rows and columns
+ *   [V, ld_d); V <= ld_d <= V rounded up to 128, ld_d even.  The dgrad, wgrad and bias gradient then read dlogits.
+ * univl_vocab_xent_workspace: bytes (>= 0) of that workspace, or negative on error. */
+int univl_vocab_xent_workspace(int T, int V);
+int univl_vocab_xent_fwd(const void* x, long long ldx, const void* w, long long ldw, const float* bias,
+                         const long long* labels, float* lse, float* sum_count, float* loss, void* workspace,
+                         long long workspace_bytes, int T, int V, int Kc, int groups, void* stream);
+int univl_vocab_xent_bwd(const void* x, long long ldx, const void* w, long long ldw, const float* bias,
+                         const long long* labels, const float* lse, const float* sum_count, const float* gscale,
+                         void* dlogits, long long ld_d, int T, int V, int Kc, int groups, void* stream);
 /* cross pooler tanh + similarity_dense (module_cross.py:281-287; modeling.py:371): out[r] = tanh(u[r,:]).w + b */
 int univl_pooler_sim_fwd(const void* u, const float* w, const float* b, float* out, int N, int H, void* stream);
 int univl_pooler_sim_bwd(const void* u, const float* w, const float* dout, void* du, float* dw, float* db, int N,

@@ -930,6 +930,302 @@ static int launch_gemm_fp8(const CUtensorMap& ta, const CUtensorMap& tb, const G
   return UNIVL_OK;
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// Vocabulary cross-entropy without logits in HBM (the MLM and caption heads):
+//   logit[r, c] = sum_k x(r,k) W(c,k) + bias[c],  loss = mean over groups of the mean over scored rows of
+//   logsumexp(logit[r, :V]) - logit[r, labels[r]]
+// The mainloop is the bf16 kernel's cooperative one on 128 x 128 tiles (both operands K-major), so every logit has the
+// bits EPI_BIAS_F32 gives it: the same k16 wgmma chain and the same fp32 bias add.  A work item is one 128-row tile x
+// a chunk of VX_CHUNK consecutive 128-column tiles; the CTA walks the chunk's tiles in column order.
+//   forward  (BWD = false): each thread keeps, per row of its fragment, a running max m and sum s of exp(logit - m)
+//            over the columns it holds, updated tile by tile; at the end of the item the four lanes of a quad fold
+//            their (m, s) with two xor shuffles (symmetric, so every lane gets the same bits) and lane 0 writes the
+//            row's (m, s, label logit) for the chunk.  vocab_xent_rows_kernel folds the chunks in chunk order.
+//   backward (BWD = true):  dl[r, c] = (exp(logit - lse[r]) - [c == label]) * g(r) as bf16, the arithmetic of
+//            xent_bwd_kernel; columns [V, ld_d) and rows with label -1 get 0.
+// The chunking is a pure function of (T, V) (vx_plan), never of the SMs in use, so the bits do not depend on the
+// grid, reserved SMs or which CTA runs an item.
+constexpr int VX_BLOCK_N = 128;
+constexpr int VX_STAGES = 6;
+
+struct VocabXentParams {
+  int T, V, Kc;
+  int m_tiles, n_tiles, chunks, chunk_tiles;
+  const float* bias;        // nullable
+  const long long* labels;  // [T], -1 = not scored
+  float4* part;             // forward: [T, chunks] (m, s, label logit, 0)
+  // backward
+  const float* lse;
+  const float* count;   // [groups]
+  const float* gscale;  // nullable: 1
+  int rows_per_group, groups;
+  bf16* dl;
+  long long ld_d;
+};
+
+template <bool BWD>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+vocab_xent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                  const VocabXentParams p, const int num_work) {
+  using L = GemmSmem<VX_BLOCK_N, VX_STAGES>;
+  pdl_trigger();
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFFSET);
+  uint64_t* empty_bar = full_bar + VX_STAGES;
+  const int wg = threadIdx.x >> 7;
+  const int total_kb = (p.Kc + BLOCK_K - 1) / BLOCK_K;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmap_a);
+    tma_prefetch_desc(&tmap_b);
+    for (int s = 0; s < VX_STAGES; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 2);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  pdl_wait();
+
+  // work item w: chunk w / m_tiles, m-tile w % m_tiles — the CTAs in flight share a few chunks of W through L2
+  if (wg == 0) {
+    regs_dealloc<40>();
+    if (threadIdx.x != 0) return;
+    uint32_t it = 0;
+    for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
+      const int chunk = w / p.m_tiles;
+      const int m0 = (w - chunk * p.m_tiles) * BLOCK_M;
+      const int nt1 = min(p.n_tiles, (chunk + 1) * p.chunk_tiles);
+      for (int nt = chunk * p.chunk_tiles; nt < nt1; ++nt) {
+        for (int kb = 0; kb < total_kb; ++kb, ++it) {
+          const int s = it % VX_STAGES;
+          mbar_wait(&empty_bar[s], ((it / VX_STAGES) & 1) ^ 1);
+          uint8_t* sa = smem + s * L::STAGE_BYTES;
+          mbar_arrive_expect_tx(&full_bar[s], L::STAGE_BYTES);
+          tma_load_2d(sa, &tmap_a, &full_bar[s], kb * BLOCK_K, m0);
+          tma_load_2d(sa + L::A_BYTES, &tmap_b, &full_bar[s], kb * BLOCK_K, nt * VX_BLOCK_N);
+        }
+      }
+    }
+    return;
+  }
+  regs_alloc<232>();
+  const int c = wg - 1;  // rows [64 c, 64 c + 64) of every tile
+  const int t = threadIdx.x & 127;
+  const int warp = t >> 5, lane = t & 31, q = lane & 3;
+  uint32_t it = 0;
+  for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
+    const int chunk = w / p.m_tiles;
+    const int row = (w - chunk * p.m_tiles) * BLOCK_M + c * 64 + warp * 16 + (lane >> 2);  // and row + 8
+    long long lab[2];
+    float m[2], s[2], xt[2], lse[2], g[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = row + 8 * h;
+      lab[h] = r < p.T ? __ldg(p.labels + r) : -1;
+      m[h] = -INFINITY;
+      s[h] = 0.f;
+      xt[h] = 0.f;
+      if constexpr (BWD) {
+        lse[h] = 0.f;
+        g[h] = 0.f;
+        if (lab[h] != -1) {
+          lse[h] = __ldg(p.lse + r);
+          // (gscale / G) / count: xent_bwd_kernel's scale, in its order
+          g[h] = ((p.gscale ? __ldg(p.gscale) : 1.f) / (float)p.groups) / __ldg(p.count + r / p.rows_per_group);
+        }
+      }
+    }
+    const int nt1 = min(p.n_tiles, (chunk + 1) * p.chunk_tiles);
+    for (int nt = chunk * p.chunk_tiles; nt < nt1; ++nt) {
+      float acc[VX_BLOCK_N / 2];
+#pragma unroll
+      for (int e = 0; e < VX_BLOCK_N / 2; ++e) acc[e] = 0.f;
+      int prev_s = -1;
+      for (int i = 0; i < total_kb; ++i, ++it) {
+        const int st = it % VX_STAGES;
+        mbar_wait(&full_bar[st], (it / VX_STAGES) & 1);
+        const uint32_t sa = smem_u32(smem + st * L::STAGE_BYTES) + c * (64 * 128);
+        const uint32_t sb = smem_u32(smem + st * L::STAGE_BYTES) + L::A_BYTES;
+        wgmma_fence();
+        fence_regs(acc);
+#pragma unroll
+        for (int k = 0; k < BLOCK_K / 16; ++k)
+          WgmmaSS<VX_BLOCK_N>::template mma<0, 0>(acc, make_smem_desc_sw128(sa + k * 32, 16, 1024),
+                                                  make_smem_desc_sw128(sb + k * 32, 16, 1024),
+                                                  (i > 0 || k > 0) ? 1 : 0);
+        wgmma_commit();
+        fence_regs(acc);
+        wgmma_wait<1>();  // the previous k-block's MMAs have read their stage
+        if (prev_s >= 0 && t == 0) mbar_arrive(&empty_bar[prev_s]);
+        prev_s = st;
+      }
+      wgmma_wait<0>();
+      fence_regs(acc);
+      if (t == 0) mbar_arrive(&empty_bar[prev_s]);
+
+      const int col0 = nt * VX_BLOCK_N + 2 * q;
+      // the logits of this thread's columns (bias added as EPI_BIAS_F32 adds it); columns >= V are never read
+#pragma unroll
+      for (int j = 0; j < VX_BLOCK_N / 8; ++j) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int col = col0 + 8 * j + e;
+          const float b = (p.bias != nullptr && col < p.V) ? __ldg(p.bias + col) : 0.f;
+          acc[4 * j + e] = __fadd_rn(acc[4 * j + e], b);
+          acc[4 * j + 2 + e] = __fadd_rn(acc[4 * j + 2 + e], b);
+        }
+      }
+      if constexpr (!BWD) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float tm = -INFINITY;
+#pragma unroll
+          for (int j = 0; j < VX_BLOCK_N / 8; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e)
+              if (col0 + 8 * j + e < p.V) tm = fmaxf(tm, acc[4 * j + 2 * h + e]);
+          if (tm > m[h]) {  // a new running max: rescale the sum (exp(-inf) = 0 on the first tile)
+            s[h] = s[h] * __expf(m[h] - tm);
+            m[h] = tm;
+          }
+#pragma unroll
+          for (int j = 0; j < VX_BLOCK_N / 8; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int col = col0 + 8 * j + e;
+              const float v = acc[4 * j + 2 * h + e];
+              if (col < p.V) s[h] += __expf(v - m[h]);
+              if (col == lab[h]) xt[h] = v;
+            }
+        }
+      } else {
+        const int ncol = min(p.ld_d - (long long)nt * VX_BLOCK_N, (long long)VX_BLOCK_N);  // this tile's columns
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = row + 8 * h;
+          if (r >= p.T) continue;
+          bf16* drow = p.dl + (long long)r * p.ld_d + col0;
+          const bool scored = lab[h] != -1;
+#pragma unroll
+          for (int j = 0; j < VX_BLOCK_N / 8; ++j) {
+            if (8 * j + 2 * q >= ncol) break;  // ld_d is even, so the pair is whole
+            float d[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int col = col0 + 8 * j + e;
+              d[e] = 0.f;
+              if (scored && col < p.V)
+                d[e] = (__expf(acc[4 * j + 2 * h + e] - lse[h]) - (col == lab[h] ? 1.f : 0.f)) * g[h];
+            }
+            *reinterpret_cast<uint32_t*>(drow + 8 * j) = pack_bf16x2(d[0], d[1]);
+          }
+        }
+      }
+    }
+    if constexpr (!BWD) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int o = 1; o <= 2; o <<= 1) {
+          const float mo = __shfl_xor_sync(0xffffffffu, m[h], o);
+          const float so = __shfl_xor_sync(0xffffffffu, s[h], o);
+          const float xo = __shfl_xor_sync(0xffffffffu, xt[h], o);
+          const float mx = fmaxf(m[h], mo);
+          const float a = m[h] == -INFINITY ? 0.f : s[h] * __expf(m[h] - mx);
+          const float b = mo == -INFINITY ? 0.f : so * __expf(mo - mx);
+          m[h] = mx;
+          s[h] = a + b;    // commutative: both lanes of the pair get the same bits
+          xt[h] += xo;     // one lane of the quad holds the label column, the others add 0
+        }
+        const int r = row + 8 * h;
+        if (q == 0 && r < p.T) p.part[(long long)r * p.chunks + chunk] = make_float4(m[h], s[h], xt[h], 0.f);
+      }
+    }
+  }
+}
+
+// Row r (one thread each): fold its chunk records in chunk order into lse[r] = m + log(s) and nll[r] = lse[r] - the
+// label logit, taken from the label's chunk.  Rows with label -1 get lse 0, as xent_fwd_kernel gives them.
+__global__ void __launch_bounds__(256)
+vocab_xent_rows_kernel(const float4* __restrict__ part, const long long* __restrict__ labels, int T, int V, int chunks,
+                       int chunk_cols, float* __restrict__ lse_out, float* __restrict__ nll) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= T) return;
+  const long long lab = labels[r];
+  if (lab == -1) {
+    lse_out[r] = 0.f;
+    return;
+  }
+  const float4* pr = part + (long long)r * chunks;
+  float4 f = pr[0];
+  float m = f.x, s = f.y;
+  for (int k = 1; k < chunks; ++k) {
+    f = pr[k];
+    const float mx = fmaxf(m, f.x);
+    s = s * __expf(m - mx) + f.y * __expf(f.x - mx);
+    m = mx;
+  }
+  const float lse = m + __logf(s);
+  lse_out[r] = lse;
+  // a label outside [0, V) scores NaN instead of reading past the row
+  nll[r] = (lab >= 0 && lab < V) ? lse - pr[lab / chunk_cols].z : __int_as_float(0x7fc00000);
+}
+
+// Per group (one CTA each): the sum of its scored rows' nll and their count, in a fixed order (no float atomics).
+constexpr int VX_GROUP_THREADS = 512;
+__global__ void __launch_bounds__(VX_GROUP_THREADS)
+vocab_xent_group_kernel(const float* __restrict__ nll, const long long* __restrict__ labels, int rows_per_group,
+                        float* __restrict__ sum_count, int groups) {
+  __shared__ float red[2][VX_GROUP_THREADS];
+  const int grp = blockIdx.x;
+  float sum = 0.f, cnt = 0.f;
+  for (int i = threadIdx.x; i < rows_per_group; i += VX_GROUP_THREADS) {
+    const long long r = (long long)grp * rows_per_group + i;
+    if (labels[r] == -1) continue;
+    sum += nll[r];
+    cnt += 1.f;
+  }
+  red[0][threadIdx.x] = sum;
+  red[1][threadIdx.x] = cnt;
+  __syncthreads();
+  for (int o = VX_GROUP_THREADS / 2; o > 0; o >>= 1) {
+    if (threadIdx.x < o) {
+      red[0][threadIdx.x] += red[0][threadIdx.x + o];
+      red[1][threadIdx.x] += red[1][threadIdx.x + o];
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    sum_count[grp] = red[0][0];
+    sum_count[groups + grp] = red[1][0];
+  }
+}
+
+// finalize_mean_kernel's arithmetic: mean over groups of sum / count, 0 / 0 = NaN for a group without a scored row
+__global__ void vocab_xent_mean_kernel(const float* __restrict__ sum_count, int groups, float* __restrict__ out) {
+  float acc = sum_count[0] / sum_count[groups];
+  for (int g = 1; g < groups; ++g) acc += sum_count[g] / sum_count[groups + g];
+  *out = groups > 1 ? acc / (float)groups : acc;
+}
+
+template <bool BWD>
+static int launch_vocab_xent(const CUtensorMap& ta, const CUtensorMap& tb, const VocabXentParams& p,
+                             cudaStream_t stream) {
+  using L = GemmSmem<VX_BLOCK_N, VX_STAGES>;
+  auto kern = vocab_xent_kernel<BWD>;
+  const char* name = BWD ? "univl_vocab_xent_bwd" : "univl_vocab_xent_fwd";
+  const long long work = (long long)p.m_tiles * p.chunks;
+  if (work > 0x7fffffffLL) return set_error(UNIVL_ERR_ARG, "%s: too many tiles", name);
+  const int sms = usable_sms();
+  const int grid = (int)(work < sms ? work : sms);
+  const cudaError_t e =
+      launch_kernel(kern, dim3(grid), dim3(GEMM_THREADS), (size_t)L::DYN_BYTES, stream, ta, tb, p, (int)work);
+  if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "%s launch: %s", name, cudaGetErrorString(e));
+  return UNIVL_OK;
+}
+
 }  // namespace univl
 
 using namespace univl;
@@ -1138,4 +1434,137 @@ extern "C" int univl_gemm_fp8(const void* A, long long lda, const float* a_scale
                  : launch_gemm_fp8<FP8_EPI_BIAS_BF16, false>(ta, tb, p, f, stream);
   return pairs ? launch_gemm_fp8<FP8_EPI_GELU_E4M3, true>(ta, tb, p, f, stream)
                : launch_gemm_fp8<FP8_EPI_GELU_E4M3, false>(ta, tb, p, f, stream);
+}
+
+namespace {
+// Chunking of the vocabulary cross-entropy: chunks of whole 128-column tiles (at least VX_MIN_CHUNK_TILES of them, so
+// that the per-chunk records stay small), no empty chunk, and among those the fewest chunks that give the shortest
+// schedule on an H100 SXM's 132 SMs, counted as (rounds of work items) x (tiles per item): 4 chunks of 60 tiles at
+// T = 4096 (one round of 128 items), 30 of 8 at T = 17280 (31 rounds).  A pure function of (T, V), never of the SMs in use: the
+// chunk order is the lse's summation order.
+constexpr int VX_MIN_CHUNK_TILES = 8;
+struct VxPlan {
+  int m_tiles, n_tiles, chunks, chunk_tiles;
+};
+VxPlan vx_plan(int T, int V) {
+  VxPlan pl;
+  pl.m_tiles = (T + BLOCK_M - 1) / BLOCK_M;
+  pl.n_tiles = (V + VX_BLOCK_N - 1) / VX_BLOCK_N;
+  long long best = -1;
+  for (int c = 1; c <= pl.n_tiles; ++c) {
+    const int ct = (pl.n_tiles + c - 1) / c;
+    if (ct < VX_MIN_CHUNK_TILES && c > 1) break;
+    if (c > 1 && ct == (pl.n_tiles + c - 2) / (c - 1)) continue;  // same tiles per chunk as c - 1 chunks
+    const int chunks = (pl.n_tiles + ct - 1) / ct;
+    const long long rounds = ((long long)pl.m_tiles * chunks + PLAN_SMS - 1) / PLAN_SMS;
+    if (best < 0 || rounds * ct < best) {
+      best = rounds * ct;
+      pl.chunks = chunks;
+      pl.chunk_tiles = ct;
+    }
+  }
+  return pl;
+}
+
+int vx_check(const char* name, const void* x, long long ldx, const void* w, long long ldw, const long long* labels,
+             int T, int V, int Kc, int groups) {
+  UNIVL_CHECK_ARG(T > 0 && V > 0 && Kc > 0, "%s: empty problem T=%d V=%d K=%d", name, T, V, Kc);
+  UNIVL_CHECK_ARG(x && w && labels, "%s: null x, W or labels", name);
+  UNIVL_CHECK_ARG(ldx >= Kc && ldw >= Kc && (ldx % 8) == 0 && (ldw % 8) == 0,
+                  "%s: ldx/ldw must be >= K and multiples of 8 (got %lld, %lld, K=%d)", name, ldx, ldw, Kc);
+  UNIVL_CHECK_ARG(((uintptr_t)x & 15) == 0 && ((uintptr_t)w & 15) == 0, "%s: x and W must be 16-byte aligned", name);
+  UNIVL_CHECK_ARG(groups > 0 && T % groups == 0, "%s: %d groups must divide T=%d", name, groups, T);
+  return UNIVL_OK;
+}
+
+// Sets the kernel's shared-memory attribute first: a runtime call, which also makes the device's primary context
+// current on this thread before the driver encodes the tensor maps (autograd runs backward on a thread of its own,
+// where this may be the first call of the process into CUDA).
+template <bool BWD>
+int vx_params(const void* x, long long ldx, const void* w, long long ldw, int T, int V, int Kc, CUtensorMap* ta,
+              CUtensorMap* tb, VocabXentParams* p) {
+  const cudaError_t e = cudaFuncSetAttribute(vocab_xent_kernel<BWD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             GemmSmem<VX_BLOCK_N, VX_STAGES>::DYN_BYTES);
+  if (e != cudaSuccess)
+    return set_error(UNIVL_ERR_CUDA, "%s smem attribute: %s", BWD ? "univl_vocab_xent_bwd" : "univl_vocab_xent_fwd",
+                     cudaGetErrorString(e));
+  const VxPlan pl = vx_plan(T, V);
+  int rc;
+  if ((rc = make_tmap(ta, x, T, Kc, ldx, BLOCK_M))) return rc;
+  if ((rc = make_tmap(tb, w, V, Kc, ldw, VX_BLOCK_N))) return rc;
+  *p = VocabXentParams{};
+  p->T = T; p->V = V; p->Kc = Kc;
+  p->m_tiles = pl.m_tiles; p->n_tiles = pl.n_tiles; p->chunks = pl.chunks; p->chunk_tiles = pl.chunk_tiles;
+  return UNIVL_OK;
+}
+
+
+// workspace of univl_vocab_xent_fwd: one 16-byte record per row and vocabulary chunk, then one float per row (the row's
+// loss term), padded to 16 bytes
+long long vx_workspace_bytes(int T, int V) {
+  return (long long)T * vx_plan(T, V).chunks * (long long)sizeof(float4) + ((long long)T * 4 + 15) / 16 * 16;
+}
+}  // namespace
+
+// bytes of workspace univl_vocab_xent_fwd needs for T rows over a V-word vocabulary; negative = error
+extern "C" int univl_vocab_xent_workspace(int T, int V) {
+  UNIVL_CHECK_ARG(T > 0 && V > 0, "univl_vocab_xent_workspace: empty problem T=%d V=%d", T, V);
+  const long long bytes = vx_workspace_bytes(T, V);
+  UNIVL_CHECK_ARG(bytes <= 0x7fffffffLL, "univl_vocab_xent_workspace: T=%d V=%d needs over 2 GiB", T, V);
+  return (int)bytes;
+}
+
+extern "C" int univl_vocab_xent_fwd(const void* x, long long ldx, const void* w, long long ldw, const float* bias,
+                                    const long long* labels, float* lse, float* sum_count, float* loss,
+                                    void* workspace, long long workspace_bytes, int T, int V, int Kc, int groups,
+                                    void* stream_) {
+  const char* name = "univl_vocab_xent_fwd";
+  if (int rc = vx_check(name, x, ldx, w, ldw, labels, T, V, Kc, groups)) return rc;
+  UNIVL_CHECK_ARG(lse && sum_count && loss && workspace, "%s: null lse, sum_count, loss or workspace", name);
+  UNIVL_CHECK_ARG(((uintptr_t)workspace & 15) == 0, "%s: the workspace must be 16-byte aligned", name);
+  const long long need = vx_workspace_bytes(T, V);
+  UNIVL_CHECK_ARG(workspace_bytes >= need, "%s: workspace of %lld bytes, needs %lld (univl_vocab_xent_workspace)",
+                  name, workspace_bytes, need);
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  CUtensorMap ta, tb;
+  VocabXentParams p;
+  if (int rc = vx_params<false>(x, ldx, w, ldw, T, V, Kc, &ta, &tb, &p)) return rc;
+  p.bias = bias;
+  p.labels = labels;
+  p.part = reinterpret_cast<float4*>(workspace);
+  if (int rc = launch_vocab_xent<false>(ta, tb, p, stream)) return rc;
+  float* nll = reinterpret_cast<float*>(p.part + (long long)T * p.chunks);
+  vocab_xent_rows_kernel<<<(T + 255) / 256, 256, 0, stream>>>(p.part, labels, T, V, p.chunks,
+                                                               p.chunk_tiles * VX_BLOCK_N, lse, nll);
+  vocab_xent_group_kernel<<<groups, VX_GROUP_THREADS, 0, stream>>>(nll, labels, T / groups, sum_count, groups);
+  vocab_xent_mean_kernel<<<1, 1, 0, stream>>>(sum_count, groups, loss);
+  UNIVL_CHECK_LAUNCH(name);
+  return UNIVL_OK;
+}
+
+extern "C" int univl_vocab_xent_bwd(const void* x, long long ldx, const void* w, long long ldw, const float* bias,
+                                    const long long* labels, const float* lse, const float* sum_count,
+                                    const float* gscale, void* dlogits, long long ld_d, int T, int V, int Kc,
+                                    int groups, void* stream_) {
+  const char* name = "univl_vocab_xent_bwd";
+  if (int rc = vx_check(name, x, ldx, w, ldw, labels, T, V, Kc, groups)) return rc;
+  UNIVL_CHECK_ARG(lse && sum_count && dlogits, "%s: null lse, sum_count or dlogits", name);
+  const long long cols = (long long)vx_plan(T, V).n_tiles * VX_BLOCK_N;
+  UNIVL_CHECK_ARG(ld_d >= V && ld_d <= cols && (ld_d % 2) == 0 && ((uintptr_t)dlogits & 3) == 0,
+                  "%s: ld_d=%lld must be even, >= V=%d and <= V rounded up to 128, with dlogits 4-byte aligned", name,
+                  ld_d, V);
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  CUtensorMap ta, tb;
+  VocabXentParams p;
+  if (int rc = vx_params<true>(x, ldx, w, ldw, T, V, Kc, &ta, &tb, &p)) return rc;
+  p.bias = bias;
+  p.labels = labels;
+  p.lse = lse;
+  p.count = sum_count + groups;
+  p.gscale = gscale;
+  p.rows_per_group = T / groups;
+  p.groups = groups;
+  p.dl = reinterpret_cast<bf16*>(dlogits);
+  p.ld_d = ld_d;
+  return launch_vocab_xent<true>(ta, tb, p, stream);
 }

@@ -10,6 +10,7 @@ import os
 
 import torch
 
+from . import lib
 from . import runtime as rt
 from .runtime import call, ptr
 
@@ -855,6 +856,49 @@ def _ld_pad(n):
     return (n + LD_VOCAB_ALIGN - 1) // LD_VOCAB_ALIGN * LD_VOCAB_ALIGN
 
 
+VOCAB_LOSS_MODES = ("logits", "fused")
+
+
+def vocab_loss_mode():
+    """UNIVL_VOCAB_LOSS, read on every ProjXentFn call: "logits" (default) writes the fp32 logits and keeps them for
+    backward; "fused" computes the vocabulary cross-entropy (target_mode 0, no pair mask, no logits returned) with
+    univl_vocab_xent_fwd / _bwd, which never write logits, so nothing of size T x V lives from forward to backward.
+    An environment variable, so that training drivers pick it up unchanged."""
+    value = os.environ.get("UNIVL_VOCAB_LOSS", "logits")
+    if value not in VOCAB_LOSS_MODES:
+        raise ValueError("UNIVL_VOCAB_LOSS must be one of %s, got %r" % ("/".join(VOCAB_LOSS_MODES), value))
+    return value
+
+
+def vocab_xent_fwd(x, w16, bias, labels, groups):
+    """-> (loss, lse [T], sum_count [2 G]) of CrossEntropy(x w16^T + bias, labels, ignore_index=-1), mean over `groups`
+    consecutive row groups, without writing the logits"""
+    _check2d(x, "vocab_xent x"); _check2d(w16, "vocab_xent W")
+    T, K = x.shape
+    V = w16.shape[0]
+    nbytes = lib.load().univl_vocab_xent_workspace(T, V)
+    if nbytes < 0:
+        raise RuntimeError("univl_vocab_xent_workspace failed: %s" % lib.load().univl_last_error_string().decode())
+    ws = _empty((nbytes,), torch.uint8, x)
+    lse = _empty((T,), F32, x)
+    sc = _empty((2 * groups,), F32, x)
+    loss = _empty((), F32, x)
+    call("univl_vocab_xent_fwd", x.data_ptr(), x.stride(0), w16.data_ptr(), w16.stride(0), ptr(bias),
+         labels.data_ptr(), lse.data_ptr(), sc.data_ptr(), loss.data_ptr(), ws.data_ptr(), ws.numel(), T, V, K, groups)
+    return loss, lse, sc
+
+
+def vocab_xent_bwd(x, w16, bias, labels, lse, sc, g, groups):
+    """-> dl bf16 [T, _ld_pad(V)]: the logits gradient univl_softmax_xent_bwd gives, from recomputed logits"""
+    T, K = x.shape
+    V = w16.shape[0]
+    ld = _ld_pad(V)
+    dl = _empty((T, ld), BF16, x)
+    call("univl_vocab_xent_bwd", x.data_ptr(), x.stride(0), w16.data_ptr(), w16.stride(0), ptr(bias),
+         labels.data_ptr(), lse.data_ptr(), sc.data_ptr(), ptr(g), dl.data_ptr(), ld, T, V, K, groups)
+    return dl
+
+
 class ProjXentFn(torch.autograd.Function):
     """loss = CrossEntropy(x W^T + bias, labels) without ever exposing logits to autograd: tied vocab projection
     (reference modules/module_bert.py:327-330) + CrossEntropyLoss(ignore_index=-1) (modeling.py:253, :275), or the MFM
@@ -862,13 +906,24 @@ class ProjXentFn(torch.autograd.Function):
     w_is_param: W is an fp32 parameter [V, K] (bf16 copy from the arena); else W is a bf16 activation [V, K].
     groups: the T rows are `groups` consecutive micro-batches; the loss is the mean over groups of each group's mean.
     Grouped NCE (target_mode 1) scores each group's rows against that group's own T / groups frames only: one
-    [T/G x T/G x K] logit GEMM per group, never the T x T matrix."""
+    [T/G x T/G x K] logit GEMM per group, never the T x T matrix.
+    UNIVL_VOCAB_LOSS=fused (vocab_loss_mode) computes the vocabulary cross-entropy (target_mode 0 without pair_mask or
+    return_logits) without logits: forward saves x, W, labels, lse and sum_count only, and backward recomputes the
+    logits tile by tile to form their gradient."""
 
     @staticmethod
     def forward(ctx, x, W, bias, labels, pair_mask, target_mode, w_is_param, return_logits, groups):
         arena = rt.current()
         w16 = arena.bf16(W) if w_is_param else W
         T, K = x.shape
+        fused = vocab_loss_mode() == "fused" and target_mode == 0 and pair_mask is None and not return_logits
+        if fused:
+            labels = labels.contiguous()
+            loss, lse, sc = vocab_xent_fwd(x, w16, bias, labels, groups)
+            ctx.save_for_backward(x, w16, None, labels, None, lse, sc, W if w_is_param else None, bias)
+            ctx.cfg = (target_mode, w_is_param, bias is not None, groups, False)
+            ctx.sink = GradSink()
+            return loss
         windowed = target_mode == 1 and groups > 1
         if windowed and (w_is_param or w16.shape[0] != T or T % groups):
             raise ValueError("grouped NCE needs one frame row per scored row and T divisible by the %d groups" % groups)
@@ -899,12 +954,16 @@ class ProjXentFn(torch.autograd.Function):
         x, w16, logits, labels, pair_mask, lse, sc, W, bias = ctx.saved_tensors
         target_mode, w_is_param, has_bias, groups, windowed = ctx.cfg
         T, K = x.shape
-        V = logits.shape[1]
-        ld = _ld_pad(V)
         g = g.contiguous().to(F32)
-        dl = _empty((T, ld), BF16, x)
-        call("univl_softmax_xent_bwd", logits.data_ptr(), logits.stride(0), labels.data_ptr(), ptr(pair_mask),
-             lse.data_ptr(), sc.data_ptr(), g.data_ptr(), dl.data_ptr(), ld, T, V, target_mode, -1, groups)
+        if logits is None:  # UNIVL_VOCAB_LOSS=fused
+            V = w16.shape[0]
+            dl = vocab_xent_bwd(x, w16, bias, labels, lse, sc, g, groups)
+        else:
+            V = logits.shape[1]
+            ld = _ld_pad(V)
+            dl = _empty((T, ld), BF16, x)
+            call("univl_softmax_xent_bwd", logits.data_ptr(), logits.stride(0), labels.data_ptr(), ptr(pair_mask),
+                 lse.data_ptr(), sc.data_ptr(), g.data_ptr(), dl.data_ptr(), ld, T, V, target_mode, -1, groups)
         dlv = dl[:, :V]
         dx = _empty((T, K), BF16, x)
         if windowed:
