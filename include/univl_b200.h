@@ -27,6 +27,11 @@ int univl_abi_version(void);
  * (default).  Process-wide; read at enqueue time (captured graphs keep their grids).
  * No reference counterpart: DDP's overlapped bucket all-reduce (main_task_retrieval.py:197) leaves this to cuBLAS. */
 int univl_set_reserved_sms(int n);
+/* dst[r * ld + c] += sum over k of part[k][r][c] (fp32, part [nparts][rows][cols] contiguous, left unchanged): the
+ * ordered reduction every deterministic cross-block sum of the library ends in.  Each element's rows are added in
+ * ascending k (t = 0; t += part[k]), then t is added into dst, so the bits depend only on the inputs. */
+int univl_partials_reduce(const float* part, int nparts, long long rows, long long cols, float* dst, long long ld,
+                          void* stream);
 
 /* ---- GEMM (wgmma / TMA) ---------------------------------------------------------------------------------
  * D[M,N] = epilogue(sum_k A(m,k) B(n,k)), bf16 operands, fp32 accumulation.

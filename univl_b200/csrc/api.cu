@@ -65,28 +65,71 @@ int scratch_alloc(void** p, size_t bytes, cudaStream_t st) {
   return UNIVL_OK;
 }
 
-__global__ void __launch_bounds__(256)
-partials_reduce_kernel(const float* __restrict__ part, int nparts, long long rows, long long cols, float* __restrict__ dst,
+// Every element's partial rows are added in row order, t = 0; t += row 0; t += row 1; ..., then dst += t: the same
+// arithmetic, and so the same bits, as one thread walking the rows, on every launch and with any grid.  What is
+// parallel is the reading.  A CTA owns 32 consecutive elements (a warp reads 128 contiguous bytes of a row); its 8
+// warps load the rows in stages of 256 (32 loads in flight per lane) into a double-buffered shared-memory tile, and
+// warp 0 adds each staged tile in row order while the next stage's loads are in flight.  The loads, not the serial
+// adds, bound the time, and they no longer wait on each other.
+constexpr int PR_WARPS = 8;
+constexpr int PR_STAGE = 256;                      // rows per stage, PR_STAGE / PR_WARPS per lane
+constexpr int PR_SMEM = 2 * PR_STAGE * 32 * 4;     // two staged tiles [PR_STAGE][32] fp32: 64 KB
+
+__global__ void __launch_bounds__(PR_WARPS * 32)
+partials_reduce_kernel(const float* __restrict__ part, int nparts, long long n, long long cols, float* __restrict__ dst,
                        long long ld) {
-  const long long n = rows * cols;
-  for (long long i = blockIdx.x * 256LL + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
-    float t = 0.f;
-    for (int k = 0; k < nparts; ++k) t += part[(long long)k * n + i];
-    const long long r = i / cols, c = i - r * cols;
+  extern __shared__ float pr_tile[];  // [2][PR_STAGE][32]
+  constexpr int PER = PR_STAGE / PR_WARPS;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long long e = blockIdx.x * 32LL + lane;
+  const bool ok = e < n;
+  const int stages = (nparts + PR_STAGE - 1) / PR_STAGE;
+  float v[PER];
+  // stage s, row s * PR_STAGE + i * PR_WARPS + warp -> v[i]; rows past nparts are never added
+  auto load = [&](int s) {
+#pragma unroll
+    for (int i = 0; i < PER; ++i) {
+      const int k = s * PR_STAGE + i * PR_WARPS + warp;
+      v[i] = ok && k < nparts ? __ldcs(part + (long long)k * n + e) : 0.f;
+    }
+  };
+  if (stages > 0) load(0);
+  float t = 0.f;
+  for (int s = 0; s < stages; ++s) {
+    // tile s & 1 was last read by warp 0 at stage s - 2, before it reached the barrier of stage s - 1
+    float* tile = pr_tile + (s & 1) * PR_STAGE * 32;
+#pragma unroll
+    for (int i = 0; i < PER; ++i) tile[(i * PR_WARPS + warp) * 32 + lane] = v[i];
+    __syncthreads();
+    if (s + 1 < stages) load(s + 1);
+    if (warp == 0) {
+      const int kn = nparts - s * PR_STAGE < PR_STAGE ? nparts - s * PR_STAGE : PR_STAGE;
+      for (int k = 0; k < kn; ++k) t += tile[k * 32 + lane];
+    }
+  }
+  if (warp == 0 && ok) {
+    const long long r = e / cols, c = e - r * cols;
     dst[r * ld + c] += t;
   }
 }
 
-int partials_reduce(float* part, int nparts, long long rows, long long cols, float* dst, long long ld, cudaStream_t st) {
+static int partials_reduce_launch(const float* part, int nparts, long long rows, long long cols, float* dst, long long ld,
+                                  cudaStream_t st) {
   const long long n = rows * cols;
-  long long blocks = (n + 255) / 256;
-  if (blocks > device_sms() * 8LL) blocks = device_sms() * 8LL;
-  if (blocks < 1) blocks = 1;
-  partials_reduce_kernel<<<(int)blocks, 256, 0, st>>>(part, nparts, rows, cols, dst, ld);
-  const cudaError_t e = cudaGetLastError();
-  cudaFreeAsync(part, st);
+  const long long blocks = n > 0 ? (n + 31) / 32 : 1;
+  if (blocks > 0x7fffffffLL) return set_error(UNIVL_ERR_UNSUPPORTED, "partials_reduce: %lld elements", n);
+  cudaError_t e = cudaFuncSetAttribute(partials_reduce_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PR_SMEM);
+  if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "partials_reduce smem attribute: %s", cudaGetErrorString(e));
+  partials_reduce_kernel<<<(unsigned)blocks, PR_WARPS * 32, PR_SMEM, st>>>(part, nparts, n, cols, dst, ld);
+  e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "partials_reduce launch: %s", cudaGetErrorString(e));
   return UNIVL_OK;
+}
+
+int partials_reduce(float* part, int nparts, long long rows, long long cols, float* dst, long long ld, cudaStream_t st) {
+  const int rc = partials_reduce_launch(part, nparts, rows, cols, dst, ld, st);
+  cudaFreeAsync(part, st);
+  return rc;
 }
 
 }  // namespace univl
@@ -95,6 +138,12 @@ extern "C" int univl_set_reserved_sms(int n) {
   if (n < 0) return univl::set_error(UNIVL_ERR_ARG, "univl_set_reserved_sms: n = %d", n);
   univl::g_reserved_sms = n;
   return UNIVL_OK;
+}
+extern "C" int univl_partials_reduce(const float* part, int nparts, long long rows, long long cols, float* dst,
+                                     long long ld, void* stream) {
+  UNIVL_CHECK_ARG(part && dst && nparts >= 0 && rows >= 0 && cols > 0 && ld >= cols,
+                  "partials_reduce: bad arguments nparts=%d rows=%lld cols=%lld ld=%lld", nparts, rows, cols, ld);
+  return univl::partials_reduce_launch(part, nparts, rows, cols, dst, ld, (cudaStream_t)stream);
 }
 extern "C" const char* univl_last_error_string() { return univl::g_err; }
 extern "C" int univl_abi_version() { return 1; }
