@@ -10,10 +10,10 @@
 // Work item = (row block, head).  A row block is G = floor(128 / S) whole sequences = RB = G*S <= 128 consecutive
 // token rows (S = 48 -> 96 rows, S = 96 -> 96, S = 128 -> 128); a CTA walks a contiguous range of items, heads
 // fastest, so its x rows stay in L2 for the 12 heads.  RB is a template parameter (80, 96, 112 or 128), so every
-// product below has its exact width.  Warp roles (384 threads): warpgroup 0 is the TMA producer, warpgroups 1 and 2
-// each own 64 query rows of the block.  Per item:
+// product below has its exact width.  Warp roles: those of pipeline.cuh, the consumer warpgroups each owning 64 query
+// rows of the block.  Per item:
 //   1. projection   acc[64, 192] = x[64 rows, 768] . Wqkv_h[192, 768]^T   12 k-blocks x 4 wgmma m64n192k16 per
-//                   warpgroup; x and the three 64-row weight slices arrive by TMA into a 4-stage mbarrier ring
+//                   warpgroup; x and the three 64-row weight slices arrive by TMA into a 4-stage ring
 //   2. drain        registers (+bias) -> bf16 -> Q, K, V shared-memory tiles in the 128B-swizzled operand layout (one
 //                   physical layout serves Q as K-major A, K as K-major B, V as MN-major B)
 //   3. S = Q K^T    4 wgmma (m64, N = RB, k16) into registers
@@ -23,12 +23,11 @@
 #include <stdlib.h>
 
 #include "common.cuh"
+#include "pipeline.cuh"
 #include "tmap.cuh"
-#include "wgmma.cuh"
 
 namespace univl {
 
-constexpr int FA_THREADS = 384;                 // TMA producer warpgroup + two consumer warpgroups
 constexpr int FA_STAGES = 4;
 constexpr int FA_KB = 12;                       // 768 / 64 k-blocks
 constexpr int FA_X_BYTES = 128 * 64 * 2;        // 16 KB: x rows of one k-block
@@ -116,53 +115,32 @@ __device__ __forceinline__ void fa_keep_bits(uint64_t seed, uint64_t stream, uin
 }
 
 template <int NK>
-__global__ void __launch_bounds__(FA_THREADS, 1)
+__global__ void __launch_bounds__(PIPELINE_THREADS, 1)
 fused_qkv_attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
                                const __grid_constant__ CUtensorMap tmap_qkv, const FusedAttnParams p) {
-  pdl_trigger();
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + FA_OFF_BAR);
-  uint64_t* empty_bar = full_bar + FA_STAGES;
+  Ring<FA_STAGES> ring;
+  uint8_t* smem = kernel_prologue(ring, FA_OFF_BAR, 2, &tmap_x, &tmap_w, p.store_qkv ? &tmap_qkv : nullptr);
   float* madd = reinterpret_cast<float*>(smem + FA_OFF_MADD);
 
   const int wg = threadIdx.x >> 7;
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmap_x);
-    tma_prefetch_desc(&tmap_w);
-    if (p.store_qkv) tma_prefetch_desc(&tmap_qkv);
-    for (int s = 0; s < FA_STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 2);  // one arrival per consumer warpgroup
-    }
-    fence_mbar_init();
-  }
-  __syncthreads();
-  pdl_wait();
-
   int item_begin, item_end;
   fa_item_range(p.n_blocks * p.heads, item_begin, item_end);
 
   if (wg == 0) {
-    // ------------------------------------------ TMA producer ------------------------------------------
-    regs_dealloc<40>();
-    if (threadIdx.x == 0) {
+    if (producer_regs()) {
       uint32_t it = 0;
       for (int w = item_begin; w < item_end; ++w) {
         const int rb = w / p.heads, h = w - rb * p.heads;
         const int r0 = rb * p.RB;
         for (int kb = 0; kb < FA_KB; ++kb, ++it) {
-          const int s = it % FA_STAGES;
-          const uint32_t ph = (it / FA_STAGES) & 1;
-          mbar_wait(&empty_bar[s], ph ^ 1);
+          // the x box holds only the RB rows that carry queries / keys (tile rows RB..127 feed only rows nobody reads)
+          const int s = ring.acquire(it, (uint32_t)(p.x_box_rows * 128 + FA_W_BYTES));
           uint8_t* sx = smem + s * FA_STAGE_BYTES;
           uint8_t* sw = sx + FA_X_BYTES;
-          // the x box holds only the RB rows that carry queries / keys (tile rows RB..127 feed only rows nobody reads)
-          mbar_arrive_expect_tx(&full_bar[s], (uint32_t)(p.x_box_rows * 128 + FA_W_BYTES));
-          tma_load_2d(sx, &tmap_x, &full_bar[s], kb * 64, r0);  // rows >= T arrive as zeros
+          tma_load_2d(sx, &tmap_x, &ring.full[s], kb * 64, r0);  // rows >= T arrive as zeros
 #pragma unroll
           for (int m = 0; m < 3; ++m)  // q / k / v weight rows of head h: rows m*H + h*64 of Wqkv[3H, 768]
-            tma_load_2d(sw + m * 8192, &tmap_w, &full_bar[s], kb * 64, m * p.heads * 64 + h * 64);
+            tma_load_2d(sw + m * 8192, &tmap_w, &ring.full[s], kb * 64, m * p.heads * 64 + h * 64);
         }
       }
     }
@@ -170,7 +148,7 @@ fused_qkv_attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_x, const
   }
 
   // ------------------------------------------ consumer warpgroups ------------------------------------------
-  regs_alloc<232>();
+  consumer_regs();
   const int c = wg - 1;
   const int t = threadIdx.x & 127;
   const int warp = t >> 5, lane = t & 31, quad = lane & 3;
@@ -189,28 +167,9 @@ fused_qkv_attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_x, const
     float acc[96];
 #pragma unroll
     for (int e = 0; e < 96; ++e) acc[e] = 0.f;
-    int prev_s = -1;
-    for (int kb = 0; kb < FA_KB; ++kb, ++it) {
-      const int s = it % FA_STAGES;
-      const uint32_t ph = (it / FA_STAGES) & 1;
-      mbar_wait(&full_bar[s], ph);
-      const uint32_t sx = smem_u32(smem + s * FA_STAGE_BYTES) + c * (64 * 128);
-      const uint32_t sw = smem_u32(smem + s * FA_STAGE_BYTES) + FA_X_BYTES;
-      wgmma_fence();
-      fence_regs(acc);
-#pragma unroll
-      for (int k = 0; k < 4; ++k)
-        WgmmaSS<192>::mma<0, 0>(acc, make_smem_desc_sw128(sx + 32 * k, 16, 1024),
-                                make_smem_desc_sw128(sw + 32 * k, 16, 1024), (kb > 0 || k > 0) ? 1 : 0);
-      wgmma_commit();
-      fence_regs(acc);
-      wgmma_wait<1>();
-      if (prev_s >= 0 && t == 0) mbar_arrive(&empty_bar[prev_s]);
-      prev_s = s;
-    }
-    wgmma_wait<0>();
-    fence_regs(acc);
-    if (t == 0) mbar_arrive(&empty_bar[prev_s]);
+    const int last = mma_kblocks<192, false, false, FA_STAGE_BYTES, FA_X_BYTES>(ring, smem, c * (64 * 128), acc, 0,
+                                                                                FA_KB, it, t == 0);
+    mma_drain(ring, last, acc, t == 0);
 
     // ---- 2. Q / K / V tiles (and the key mask when the row block changes) ----
     if (p.store_qkv && t == 0) bulk_wait_read<0>();  // the previous item's q/k/v stores have read the tiles
@@ -427,16 +386,11 @@ extern "C" int univl_fused_qkv_attention_fwd(const void* x, long long ldx, const
   } else {
     tq = tx;
   }
-  const int sms = usable_sms();
   const long long items = (long long)p.n_blocks * heads;
-  const int grid = (int)(items < sms ? items : sms);
   return fa_dispatch<FaFwdKernel>(p.RB, [&](auto kern) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, FA_SMEM_BYTES);
-    if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "fused_attention smem attribute: %s", cudaGetErrorString(e));
-    e = launch_kernel(kern, dim3(grid), dim3(FA_THREADS), (size_t)FA_SMEM_BYTES, (cudaStream_t)stream, tx, tw, tq, p);
-    if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "fused_attention launch: %s", cudaGetErrorString(e));
-    UNIVL_CHECK_LAUNCH("fused_qkv_attention_fwd");
-    return UNIVL_OK;
+    const char* name = "univl_fused_qkv_attention_fwd";
+    if (int prc = persistent_prepare(kern, FA_SMEM_BYTES, name)) return prc;
+    return persistent_launch(kern, name, items, FA_SMEM_BYTES, (cudaStream_t)stream, tx, tw, tq, p);
   });
 }
 
@@ -459,7 +413,7 @@ constexpr int FB_IN_BYTES = 5 * FA_TILE_BYTES;              // Q, K, V, dO, O ti
 constexpr int FB_OFF_P = 2 * FB_IN_BYTES;                   // P~ tile (two 64-key atoms)
 constexpr int FB_OFF_DS = FB_OFF_P + 2 * FA_TILE_BYTES;     // dS tile
 constexpr int FB_OFF_MADD = FB_OFF_DS + 2 * FA_TILE_BYTES;
-constexpr int FB_OFF_BAR = FB_OFF_MADD + 512;               // in_full[2] in_empty[2]
+constexpr int FB_OFF_BAR = FB_OFF_MADD + 512;               // full[2] empty[2] of the item buffers' ring
 constexpr int FB_SMEM_BYTES = FB_OFF_BAR + 4 * 8 + 1024;
 static_assert(FB_SMEM_BYTES <= 227 * 1024, "shared memory per block");
 
@@ -512,58 +466,38 @@ __device__ __forceinline__ void fb_drain(const FusedAttnBwdParams& p, const floa
 }
 
 template <int NK>
-__global__ void __launch_bounds__(FA_THREADS, 1)
+__global__ void __launch_bounds__(PIPELINE_THREADS, 1)
 fused_attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_constant__ CUtensorMap tmap_do,
                            const __grid_constant__ CUtensorMap tmap_o, const FusedAttnBwdParams p) {
-  pdl_trigger();
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* in_full = reinterpret_cast<uint64_t*>(smem + FB_OFF_BAR);   // [2] TMA -> consumers
-  uint64_t* in_empty = in_full + 2;                                      // [2] consumers -> TMA
+  Ring<2> ring;  // the two item buffers
+  uint8_t* smem = kernel_prologue(ring, FB_OFF_BAR, 2, &tmap_qkv, &tmap_do, &tmap_o);
   float* madd = reinterpret_cast<float*>(smem + FB_OFF_MADD);
 
   const int wg = threadIdx.x >> 7;
   const int H = p.heads * 64;
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmap_qkv);
-    tma_prefetch_desc(&tmap_do);
-    tma_prefetch_desc(&tmap_o);
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&in_full[b], 1);
-      mbar_init(&in_empty[b], 2);
-    }
-    fence_mbar_init();
-  }
-  __syncthreads();
-  pdl_wait();
-
   int item_begin, item_end;
   fa_item_range(p.n_blocks * p.heads, item_begin, item_end);
   const int n_items = item_end - item_begin;
 
   if (wg == 0) {
-    // ------------------------------------------ TMA producer ------------------------------------------
-    regs_dealloc<40>();
-    if (threadIdx.x == 0) {
+    if (producer_regs()) {
       for (int j = 0; j < n_items; ++j) {
-        const int b = j & 1;
         const int w = item_begin + j;
         const int rb = w / p.heads, h = w - rb * p.heads;
         const int r0 = rb * p.RB;
-        mbar_wait(&in_empty[b], (((uint32_t)j >> 1) & 1) ^ 1);
+        const int b = ring.acquire(j, FB_IN_BYTES);
         uint8_t* dst = smem + b * FB_IN_BYTES;
-        mbar_arrive_expect_tx(&in_full[b], FB_IN_BYTES);
 #pragma unroll
-        for (int m = 0; m < 3; ++m) tma_load_2d(dst + m * FA_TILE_BYTES, &tmap_qkv, &in_full[b], m * H + h * 64, r0);
-        tma_load_2d(dst + 3 * FA_TILE_BYTES, &tmap_do, &in_full[b], h * 64, r0);
-        tma_load_2d(dst + 4 * FA_TILE_BYTES, &tmap_o, &in_full[b], h * 64, r0);
+        for (int m = 0; m < 3; ++m) tma_load_2d(dst + m * FA_TILE_BYTES, &tmap_qkv, &ring.full[b], m * H + h * 64, r0);
+        tma_load_2d(dst + 3 * FA_TILE_BYTES, &tmap_do, &ring.full[b], h * 64, r0);
+        tma_load_2d(dst + 4 * FA_TILE_BYTES, &tmap_o, &ring.full[b], h * 64, r0);
       }
     }
     return;
   }
 
   // ------------------------------------------ consumer warpgroups ------------------------------------------
-  regs_alloc<232>();
+  consumer_regs();
   const int c = wg - 1;
   const int t = threadIdx.x & 127;
   const int warp = t >> 5, lane = t & 31, quad = lane & 3;
@@ -578,7 +512,7 @@ fused_attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const _
   for (int j = 0; j < n_items; ++j) {
     const int w = item_begin + j;
     const int rb = w / p.heads, h = w - rb * p.heads;
-    const int b = j & 1;
+    const int b = ring.stage(j);
     uint8_t* in = smem + b * FB_IN_BYTES;
     const uint32_t sQ = smem_u32(in), sK = sQ + FA_TILE_BYTES, sV = sQ + 2 * FA_TILE_BYTES,
                    sdO = sQ + 3 * FA_TILE_BYTES;
@@ -590,7 +524,7 @@ fused_attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const _
       named_bar(2, 256);
       cur_rb = rb;
     }
-    mbar_wait(&in_full[b], ((uint32_t)j >> 1) & 1);
+    ring.wait(j);
 
     // ---- S = Q K^T, dP = dO V^T for this warpgroup's 64 query rows ----
     float sa[NK / 2], dpa[NK / 2];
@@ -710,7 +644,7 @@ fused_attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const _
     fence_regs(dqa);
     fence_regs(dva);
     fence_regs(dka);
-    if (t == 0) mbar_arrive(&in_empty[b]);  // this warpgroup no longer reads the item's input tiles
+    if (t == 0) ring.release(b);  // this warpgroup no longer reads the item's input tiles
 
     const int part_row = rb * 8 + c * 4 + warp;
     fb_drain(p, dqa, rb, r_lo, quad, lane, h * 64, part_row);
@@ -768,20 +702,14 @@ extern "C" int univl_fused_attention_bwd(const void* qkv, long long ld_qkv, cons
   if ((rc = make_tmap(&tq, qkv, p.T, 3 * H, ld_qkv, 128))) return rc;   // box {64 cols, 128 rows}
   if ((rc = make_tmap(&td, d_o, p.T, H, lddo, 128))) return rc;
   if ((rc = make_tmap(&to, o, p.T, H, ldo, 128))) return rc;
-  const int sms = usable_sms();
   const long long items = (long long)p.n_blocks * heads;
-  const int grid = (int)(items < sms ? items : sms);
   const int n_parts = p.n_blocks * 8;
   if (dbias != nullptr)
     if ((rc = scratch_alloc((void**)&p.dbias, (size_t)n_parts * 3 * H * sizeof(float), (cudaStream_t)stream))) return rc;
   rc = fa_dispatch<FaBwdKernel>(p.RB, [&](auto kern) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, FB_SMEM_BYTES);
-    if (e != cudaSuccess)
-      return set_error(UNIVL_ERR_CUDA, "fused_attention_bwd smem attribute: %s", cudaGetErrorString(e));
-    e = launch_kernel(kern, dim3(grid), dim3(FA_THREADS), (size_t)FB_SMEM_BYTES, (cudaStream_t)stream, tq, td, to, p);
-    if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "fused_attention_bwd launch: %s", cudaGetErrorString(e));
-    UNIVL_CHECK_LAUNCH("fused_attention_bwd");
-    return UNIVL_OK;
+    const char* name = "univl_fused_attention_bwd";
+    if (int prc = persistent_prepare(kern, FB_SMEM_BYTES, name)) return prc;
+    return persistent_launch(kern, name, items, FB_SMEM_BYTES, (cudaStream_t)stream, tq, td, to, p);
   });
   if (rc != UNIVL_OK || dbias == nullptr) return rc;
   return partials_reduce(p.dbias, n_parts, 1, 3 * H, dbias, 3 * H, (cudaStream_t)stream);

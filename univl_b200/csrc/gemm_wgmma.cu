@@ -10,10 +10,9 @@
 // so neither weights nor activations are ever transposed in HBM: the operand "major" is the transpose bit of the wgmma
 // instruction and a different TMA box shape.
 //
-// Structure (per CTA, 384 threads, 128 x BLOCK_N output tiles, optional split-K):
-//   warpgroup 0      TMA producer : one thread streams 2D boxes (128B swizzle) into a STAGES-deep mbarrier ring
-//   warpgroups 1, 2  consumers    : issue wgmma on the stage and run the fused epilogue straight from their
-//                                   accumulator registers, in one of two schedules chosen by the tile width:
+// Structure: the producer / consumer ring of pipeline.cuh on 128 x BLOCK_N output tiles, optional split-K.  The
+// consumer warpgroups issue wgmma on each stage and run the fused epilogue straight from their accumulator registers,
+// in one of two schedules chosen by the tile width:
 //     BLOCK_N = 256       cooperative: both warpgroups work on every tile, each on 64 of its 128 rows
 //                         (m64 x 256 x k16 per k16 step); the tensor cores idle while the two run the epilogue.
 //     BLOCK_N = 64 / 128  ping-pong: each warpgroup owns whole tiles, the two alternating the CTA's tiles, and issues
@@ -34,8 +33,8 @@
 // same bits.
 #include "common.cuh"
 #include "fp8.cuh"
+#include "pipeline.cuh"
 #include "tmap.cuh"
-#include "wgmma.cuh"
 
 #include <stdio.h>
 #include <type_traits>
@@ -78,7 +77,6 @@ struct GemmParams {
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;  // 64 bf16 = 128 bytes = one swizzle row
-constexpr int GEMM_THREADS = 384;
 constexpr int PLAN_SMS = 132;  // H100 SXM: the tile-width / split-K plan is a pure function of the problem
 // below it, an automatic split-K plan runs unsplit with in-register k-segment sums (see plan_gemm)
 constexpr int SPLIT_MIN_K = 4096;
@@ -488,51 +486,46 @@ constexpr int TURN_BAR = 1;
 // of a block differs.
 template <int BLOCK_N, int STAGES, bool A_MN, bool B_MN, int ELEM = 2>
 __device__ __forceinline__ void produce_ring(const CUtensorMap* tmap_a, const CUtensorMap* tmap_b, uint8_t* smem,
-                                             uint64_t* full_bar, uint64_t* empty_bar, int num_work, int m_tiles,
-                                             int n_tiles, int total_kb, int kb_per) {
+                                             const Ring<STAGES>& ring, int num_work, int m_tiles, int n_tiles,
+                                             int total_kb, int kb_per) {
   using L = GemmSmem<BLOCK_N, STAGES>;
   uint32_t it = 0;
   for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
     const WorkItem wi = decode_work(w, m_tiles, n_tiles, total_kb, kb_per, BLOCK_N);
     for (int i = 0; i < wi.num_kb; ++i, ++it) {
-      const int s = it % STAGES;
-      const uint32_t ph = (it / STAGES) & 1;
-      mbar_wait(&empty_bar[s], ph ^ 1);
+      const int s = ring.acquire(it, L::STAGE_BYTES);
+      uint64_t* bar = &ring.full[s];
       uint8_t* sa = smem + s * L::STAGE_BYTES;
       uint8_t* sb = sa + L::A_BYTES;
-      mbar_arrive_expect_tx(&full_bar[s], L::STAGE_BYTES);
       const int k_elem = (wi.kb_begin + i) * (128 / ELEM);
       if (!A_MN) {
-        tma_load_2d(sa, tmap_a, &full_bar[s], k_elem, wi.m0);  // box {128 B of k, 128 rows}
+        tma_load_2d(sa, tmap_a, bar, k_elem, wi.m0);  // box {128 B of k, 128 rows}
       } else {
 #pragma unroll
         for (int c = 0; c < BLOCK_M / 64; ++c)  // box {64 m, 64 k-rows}
-          tma_load_2d(sa + c * (BLOCK_K * 128), tmap_a, &full_bar[s], wi.m0 + c * 64, k_elem);
+          tma_load_2d(sa + c * (BLOCK_K * 128), tmap_a, bar, wi.m0 + c * 64, k_elem);
       }
       if (!B_MN) {
-        tma_load_2d(sb, tmap_b, &full_bar[s], k_elem, wi.n0);  // box {128 B of k, BLOCK_N rows}
+        tma_load_2d(sb, tmap_b, bar, k_elem, wi.n0);  // box {128 B of k, BLOCK_N rows}
       } else {
 #pragma unroll
         for (int c = 0; c < BLOCK_N / 64; ++c)
-          tma_load_2d(sb + c * (BLOCK_K * 128), tmap_b, &full_bar[s], wi.n0 + c * 64, k_elem);
+          tma_load_2d(sb + c * (BLOCK_K * 128), tmap_b, bar, wi.n0 + c * 64, k_elem);
       }
     }
   }
 }
 
 template <int BLOCK_N, int STAGES, bool A_MN, bool B_MN>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
+__global__ void __launch_bounds__(PIPELINE_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                   const GemmParams p, const int num_work) {
   using L = GemmSmem<BLOCK_N, STAGES>;
   constexpr bool PING = BLOCK_N <= 128;  // ping-pong schedule (else cooperative), see the top of this file
   // in-register k-segment sums (p.kb_seg): the 64-wide tile has the registers for a second accumulator set
   constexpr bool FOLD = BLOCK_N == 64;
-  pdl_trigger();
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFFSET);
-  uint64_t* empty_bar = full_bar + STAGES;
+  Ring<STAGES> ring;
+  uint8_t* smem = kernel_prologue(ring, L::BAR_OFFSET, PING ? 1 : 2, &tmap_a, &tmap_b);  // consumers per stage
 
   const int wg = threadIdx.x >> 7;
   const int m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M;
@@ -540,27 +533,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   const int total_kb = (p.Kc + BLOCK_K - 1) / BLOCK_K;
   const int kb_per = p.k_blocks_per_split;
 
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmap_a);
-    tma_prefetch_desc(&tmap_b);
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], PING ? 1 : 2);  // one arrival per consumer warpgroup that reads the stage
-    }
-    fence_mbar_init();
-  }
-  __syncthreads();
-  pdl_wait();  // everything above overlapped the previous kernel's tail; global memory is touched only from here on
-
   if (wg == 0) {
-    // ------------------------------ TMA producer ------------------------------
-    regs_dealloc<40>();
-    if (threadIdx.x == 0)
-      produce_ring<BLOCK_N, STAGES, A_MN, B_MN>(&tmap_a, &tmap_b, smem, full_bar, empty_bar, num_work, m_tiles, n_tiles,
-                                                total_kb, kb_per);
+    if (producer_regs())
+      produce_ring<BLOCK_N, STAGES, A_MN, B_MN>(&tmap_a, &tmap_b, smem, ring, num_work, m_tiles, n_tiles, total_kb,
+                                                kb_per);
   } else if constexpr (!PING) {
     // ------------------------------ cooperative consumers ------------------------------
-    regs_alloc<232>();
+    consumer_regs();
     const int c = wg - 1;  // rows [64 c, 64 c + 64) of every tile
     const int t = threadIdx.x & 127;
     const int warp = t >> 5, lane = t & 31;
@@ -570,34 +549,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       float acc[BLOCK_N / 2];
 #pragma unroll
       for (int e = 0; e < BLOCK_N / 2; ++e) acc[e] = 0.f;
-      int prev_s = -1;
-      for (int i = 0; i < wi.num_kb; ++i, ++it) {
-        const int s = it % STAGES;
-        const uint32_t ph = (it / STAGES) & 1;
-        mbar_wait(&full_bar[s], ph);
-        // this warpgroup's 64 rows of A start 8 KB into the stage in both layouts (64 rows x 128 B K-major, or the
-        // second 64-wide MN block); a k16 step is +32 B K-major, +16 rows of 128 B MN-major
-        const uint32_t sa = smem_u32(smem + s * L::STAGE_BYTES) + c * (64 * 128);
-        const uint32_t sb = smem_u32(smem + s * L::STAGE_BYTES) + L::A_BYTES;
-        wgmma_fence();
-        fence_regs(acc);
-#pragma unroll
-        for (int k = 0; k < BLOCK_K / 16; ++k) {
-          const uint64_t da = A_MN ? make_smem_desc_sw128(sa + k * 2048, BLOCK_K * 128, 1024)
-                                   : make_smem_desc_sw128(sa + k * 32, 16, 1024);
-          const uint64_t db = B_MN ? make_smem_desc_sw128(sb + k * 2048, BLOCK_K * 128, 1024)
-                                   : make_smem_desc_sw128(sb + k * 32, 16, 1024);
-          WgmmaSS<BLOCK_N>::template mma<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, (i > 0 || k > 0) ? 1 : 0);
-        }
-        wgmma_commit();
-        fence_regs(acc);
-        wgmma_wait<1>();  // the previous k-block's MMAs have read their stage
-        if (prev_s >= 0 && t == 0) mbar_arrive(&empty_bar[prev_s]);
-        prev_s = s;
-      }
-      wgmma_wait<0>();
-      fence_regs(acc);
-      if (t == 0) mbar_arrive(&empty_bar[prev_s]);
+      const int last = mma_kblocks<BLOCK_N, A_MN, B_MN, L::STAGE_BYTES, L::A_BYTES>(ring, smem, c * (64 * 128), acc,
+                                                                                     0, wi.num_kb, it, t == 0);
+      mma_drain(ring, last, acc, t == 0);
       const int row = wi.m0 + c * 64 + warp * 16 + (lane >> 2);
       const int col0 = wi.n0 + 2 * (lane & 3);
       finish_block<BLOCK_N>(p, wi, n_tiles, kb_per, tile_inside(p, wi, BLOCK_N), p.alpha, c, row, col0, acc);
@@ -607,10 +561,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     // Warpgroup c owns the CTA's items j = c, c + 2, c + 4, ...: all 128 rows of each.  Its mainloop of item j starts
     // only once the other warpgroup has issued its last MMA of item j - 1 (TURN_BAR + c), and it hands over the same
     // way when it has issued its own, so the two mainloops take turns in item order and each warpgroup's epilogue runs
-    // under the other's MMAs.  The hand-off is also what makes the ring safe: every k-block before item j has passed
-    // its full_bar wait when item j starts, so no full_bar wait runs more than one phase ahead of the barrier, where
-    // its parity would match a phase that has already completed and it would read a stage before its load lands.
-    regs_alloc<232>();
+    // under the other's MMAs.  The hand-off is also what keeps the two warpgroups' ring waits in order (Ring::wait):
+    // every k-block before item j has passed its wait when item j starts.
+    consumer_regs();
     const int c = wg - 1;
     const int t = threadIdx.x & 127;
     const int warp = t >> 5, lane = t & 31;
@@ -637,43 +590,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       if (j > 0) named_bar(TURN_BAR + c, 256);
       for (int i0 = 0; i0 < wi.num_kb; i0 += seg) {
         const int i1 = min(wi.num_kb, i0 + seg);
-        int prev_s = -1;
-        for (int i = i0; i < i1; ++i, ++it) {
-          const int s = it % STAGES;
-          const uint32_t ph = (it / STAGES) & 1;
-          mbar_wait(&full_bar[s], ph);
-          // rows 64-127 of A start 8 KB into the stage in both layouts, as in the cooperative schedule
-          const uint32_t sa = smem_u32(smem + s * L::STAGE_BYTES);
-          const uint32_t sb = sa + L::A_BYTES;
-          wgmma_fence();
-          fence_regs(acc[0]);
-          fence_regs(acc[1]);
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / 16; ++k) {
-            const uint64_t db = B_MN ? make_smem_desc_sw128(sb + k * 2048, BLOCK_K * 128, 1024)
-                                     : make_smem_desc_sw128(sb + k * 32, 16, 1024);
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const uint32_t sah = sa + h * (64 * 128);
-              const uint64_t da = A_MN ? make_smem_desc_sw128(sah + k * 2048, BLOCK_K * 128, 1024)
-                                       : make_smem_desc_sw128(sah + k * 32, 16, 1024);
-              WgmmaSS<BLOCK_N>::template mma<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc[h], da, db,
-                                                                          (i > i0 || k > 0) ? 1 : 0);
-            }
-          }
-          wgmma_commit();
-          fence_regs(acc[0]);
-          fence_regs(acc[1]);
-          wgmma_wait<1>();  // the previous k-block's MMAs have read their stage
-          if (prev_s >= 0 && t == 0) mbar_arrive(&empty_bar[prev_s]);
-          prev_s = s;
-        }
+        const int last =
+            mma_kblocks<BLOCK_N, 2, A_MN, B_MN, L::STAGE_BYTES, L::A_BYTES>(ring, smem, 0, acc, i0, i1, it, t == 0);
         if (i1 == wi.num_kb && w + (int)gridDim.x < num_work)
           named_bar_arrive(TURN_BAR + (c ^ 1), 256);  // the next item's turn
-        wgmma_wait<0>();
-        fence_regs(acc[0]);
-        fence_regs(acc[1]);
-        if (t == 0) mbar_arrive(&empty_bar[prev_s]);
+        mma_drain(ring, last, acc, t == 0);
         if constexpr (FOLD) {
           if (fold) {
 #pragma unroll
@@ -709,18 +630,11 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmP
                        cudaStream_t stream) {
   using L = GemmSmem<BLOCK_N, STAGES>;
   auto kern = gemm_wgmma_kernel<BLOCK_N, STAGES, A_MN, B_MN>;
-  // per launch: the attribute is per device and callers may drive several devices from one process
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::DYN_BYTES);
-  if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "gemm smem attribute: %s", cudaGetErrorString(e));
-  const int sms = usable_sms();
+  const char* name = "univl_gemm_bf16";
+  if (int rc = persistent_prepare(kern, L::DYN_BYTES, name)) return rc;
   const long long work =
       (long long)((p.M + BLOCK_M - 1) / BLOCK_M) * ((p.N + BLOCK_N - 1) / BLOCK_N) * (long long)splits;
-  if (work > 0x7fffffffLL) return set_error(UNIVL_ERR_ARG, "gemm: too many tiles");
-  const int grid = (int)(work < sms ? work : sms);
-  e = launch_kernel(kern, dim3(grid), dim3(GEMM_THREADS), (size_t)L::DYN_BYTES, stream, ta, tb, p, (int)work);
-  if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "gemm launch: %s", cudaGetErrorString(e));
-  UNIVL_CHECK_LAUNCH("gemm_wgmma");
-  return UNIVL_OK;
+  return persistent_launch(kern, name, work, L::DYN_BYTES, stream, ta, tb, p, (int)work);
 }
 
 template <int BLOCK_N, int STAGES>
@@ -760,41 +674,25 @@ constexpr int FP8_BLOCK_N = 128;
 constexpr int FP8_STAGES = 6;
 
 template <int EPI, bool PAIRS>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
+__global__ void __launch_bounds__(PIPELINE_THREADS, 1)
 gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                 const GemmParams p, const Fp8Params f, const int num_work) {
   using L = GemmSmem<FP8_BLOCK_N, FP8_STAGES>;
-  pdl_trigger();
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFFSET);
-  uint64_t* empty_bar = full_bar + FP8_STAGES;
+  Ring<FP8_STAGES> ring;
+  uint8_t* smem = kernel_prologue(ring, L::BAR_OFFSET, 2, &tmap_a, &tmap_b);
 
   const int wg = threadIdx.x >> 7;
   const int m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M;
   const int n_tiles = p.N / FP8_BLOCK_N;
   const int total_kb = p.Kc / 128;
 
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmap_a);
-    tma_prefetch_desc(&tmap_b);
-    for (int s = 0; s < FP8_STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 2);
-    }
-    fence_mbar_init();
-  }
-  __syncthreads();
-  pdl_wait();
-
   if (wg == 0) {
-    regs_dealloc<40>();
-    if (threadIdx.x == 0)
-      produce_ring<FP8_BLOCK_N, FP8_STAGES, false, false, 1>(&tmap_a, &tmap_b, smem, full_bar, empty_bar, num_work,
-                                                              m_tiles, n_tiles, total_kb, total_kb);
+    if (producer_regs())
+      produce_ring<FP8_BLOCK_N, FP8_STAGES, false, false, 1>(&tmap_a, &tmap_b, smem, ring, num_work, m_tiles, n_tiles,
+                                                              total_kb, total_kb);
     return;
   }
-  regs_alloc<232>();
+  consumer_regs();
   const int c = wg - 1;  // rows [64 c, 64 c + 64) of every tile
   const int t = threadIdx.x & 127;
   const int warp = t >> 5, lane = t & 31;
@@ -815,9 +713,7 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
     // wgmmas and waits sit in straight-line code and a loop, never under a data-dependent branch, which would make
     // ptxas serialize them.  An odd number of blocks takes one temporary and waits for each block's MMAs.
     auto issue = [&](float (&tmp)[FP8_BLOCK_N / 2], int kb) {
-      const uint32_t r = it + kb;
-      const int s = r % FP8_STAGES;
-      mbar_wait(&full_bar[s], (r / FP8_STAGES) & 1);
+      const int s = ring.wait(it + kb);
       const uint32_t a_s = smem_u32(smem + s * L::STAGE_BYTES) + c * (64 * 128);
       const uint32_t b_s = smem_u32(smem + s * L::STAGE_BYTES) + L::A_BYTES;
       wgmma_fence();
@@ -836,7 +732,7 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
       const float s1 = in1 ? __ldg(sa + (long long)kb * M + 8) : 0.f;
       wgmma_wait<decltype(newer)::value>();
       fence_regs(tmp);
-      if (t == 0) mbar_arrive(&empty_bar[(it + kb) % FP8_STAGES]);
+      if (t == 0) ring.release(ring.stage(it + kb));
       const float f0 = s0 * bs, f1 = s1 * bs;
 #pragma unroll
       for (int j = 0; j < FP8_BLOCK_N / 8; ++j) {
@@ -918,16 +814,10 @@ static int launch_gemm_fp8(const CUtensorMap& ta, const CUtensorMap& tb, const G
                            cudaStream_t stream) {
   using L = GemmSmem<FP8_BLOCK_N, FP8_STAGES>;
   auto kern = gemm_fp8_kernel<EPI, PAIRS>;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::DYN_BYTES);
-  if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "univl_gemm_fp8 smem attribute: %s", cudaGetErrorString(e));
+  const char* name = "univl_gemm_fp8";
+  if (int rc = persistent_prepare(kern, L::DYN_BYTES, name)) return rc;
   const long long work = (long long)((p.M + BLOCK_M - 1) / BLOCK_M) * (p.N / FP8_BLOCK_N);
-  if (work > 0x7fffffffLL) return set_error(UNIVL_ERR_ARG, "univl_gemm_fp8: too many tiles");
-  const int sms = usable_sms();
-  const int grid = (int)(work < sms ? work : sms);
-  e = launch_kernel(kern, dim3(grid), dim3(GEMM_THREADS), (size_t)L::DYN_BYTES, stream, ta, tb, p, f, (int)work);
-  if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "univl_gemm_fp8 launch: %s", cudaGetErrorString(e));
-  UNIVL_CHECK_LAUNCH("gemm_fp8");
-  return UNIVL_OK;
+  return persistent_launch(kern, name, work, L::DYN_BYTES, stream, ta, tb, p, f, (int)work);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -964,34 +854,18 @@ struct VocabXentParams {
 };
 
 template <bool BWD>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
+__global__ void __launch_bounds__(PIPELINE_THREADS, 1)
 vocab_xent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                   const VocabXentParams p, const int num_work) {
   using L = GemmSmem<VX_BLOCK_N, VX_STAGES>;
-  pdl_trigger();
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFFSET);
-  uint64_t* empty_bar = full_bar + VX_STAGES;
+  Ring<VX_STAGES> ring;
+  uint8_t* smem = kernel_prologue(ring, L::BAR_OFFSET, 2, &tmap_a, &tmap_b);
   const int wg = threadIdx.x >> 7;
   const int total_kb = (p.Kc + BLOCK_K - 1) / BLOCK_K;
 
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmap_a);
-    tma_prefetch_desc(&tmap_b);
-    for (int s = 0; s < VX_STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 2);
-    }
-    fence_mbar_init();
-  }
-  __syncthreads();
-  pdl_wait();
-
   // work item w: chunk w / m_tiles, m-tile w % m_tiles — the CTAs in flight share a few chunks of W through L2
   if (wg == 0) {
-    regs_dealloc<40>();
-    if (threadIdx.x != 0) return;
+    if (!producer_regs()) return;
     uint32_t it = 0;
     for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
       const int chunk = w / p.m_tiles;
@@ -999,18 +873,16 @@ vocab_xent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       const int nt1 = min(p.n_tiles, (chunk + 1) * p.chunk_tiles);
       for (int nt = chunk * p.chunk_tiles; nt < nt1; ++nt) {
         for (int kb = 0; kb < total_kb; ++kb, ++it) {
-          const int s = it % VX_STAGES;
-          mbar_wait(&empty_bar[s], ((it / VX_STAGES) & 1) ^ 1);
+          const int s = ring.acquire(it, L::STAGE_BYTES);
           uint8_t* sa = smem + s * L::STAGE_BYTES;
-          mbar_arrive_expect_tx(&full_bar[s], L::STAGE_BYTES);
-          tma_load_2d(sa, &tmap_a, &full_bar[s], kb * BLOCK_K, m0);
-          tma_load_2d(sa + L::A_BYTES, &tmap_b, &full_bar[s], kb * BLOCK_K, nt * VX_BLOCK_N);
+          tma_load_2d(sa, &tmap_a, &ring.full[s], kb * BLOCK_K, m0);
+          tma_load_2d(sa + L::A_BYTES, &tmap_b, &ring.full[s], kb * BLOCK_K, nt * VX_BLOCK_N);
         }
       }
     }
     return;
   }
-  regs_alloc<232>();
+  consumer_regs();
   const int c = wg - 1;  // rows [64 c, 64 c + 64) of every tile
   const int t = threadIdx.x & 127;
   const int warp = t >> 5, lane = t & 31, q = lane & 3;
@@ -1042,28 +914,9 @@ vocab_xent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       float acc[VX_BLOCK_N / 2];
 #pragma unroll
       for (int e = 0; e < VX_BLOCK_N / 2; ++e) acc[e] = 0.f;
-      int prev_s = -1;
-      for (int i = 0; i < total_kb; ++i, ++it) {
-        const int st = it % VX_STAGES;
-        mbar_wait(&full_bar[st], (it / VX_STAGES) & 1);
-        const uint32_t sa = smem_u32(smem + st * L::STAGE_BYTES) + c * (64 * 128);
-        const uint32_t sb = smem_u32(smem + st * L::STAGE_BYTES) + L::A_BYTES;
-        wgmma_fence();
-        fence_regs(acc);
-#pragma unroll
-        for (int k = 0; k < BLOCK_K / 16; ++k)
-          WgmmaSS<VX_BLOCK_N>::template mma<0, 0>(acc, make_smem_desc_sw128(sa + k * 32, 16, 1024),
-                                                  make_smem_desc_sw128(sb + k * 32, 16, 1024),
-                                                  (i > 0 || k > 0) ? 1 : 0);
-        wgmma_commit();
-        fence_regs(acc);
-        wgmma_wait<1>();  // the previous k-block's MMAs have read their stage
-        if (prev_s >= 0 && t == 0) mbar_arrive(&empty_bar[prev_s]);
-        prev_s = st;
-      }
-      wgmma_wait<0>();
-      fence_regs(acc);
-      if (t == 0) mbar_arrive(&empty_bar[prev_s]);
+      const int last = mma_kblocks<VX_BLOCK_N, false, false, L::STAGE_BYTES, L::A_BYTES>(ring, smem, c * (64 * 128),
+                                                                                          acc, 0, total_kb, it, t == 0);
+      mma_drain(ring, last, acc, t == 0);
 
       const int col0 = nt * VX_BLOCK_N + 2 * q;
       // the logits of this thread's columns (bias added as EPI_BIAS_F32 adds it); columns >= V are never read
@@ -1210,20 +1063,13 @@ __global__ void vocab_xent_mean_kernel(const float* __restrict__ sum_count, int 
   *out = groups > 1 ? acc / (float)groups : acc;
 }
 
+// after vx_params, which runs persistent_prepare
 template <bool BWD>
 static int launch_vocab_xent(const CUtensorMap& ta, const CUtensorMap& tb, const VocabXentParams& p,
                              cudaStream_t stream) {
-  using L = GemmSmem<VX_BLOCK_N, VX_STAGES>;
-  auto kern = vocab_xent_kernel<BWD>;
-  const char* name = BWD ? "univl_vocab_xent_bwd" : "univl_vocab_xent_fwd";
   const long long work = (long long)p.m_tiles * p.chunks;
-  if (work > 0x7fffffffLL) return set_error(UNIVL_ERR_ARG, "%s: too many tiles", name);
-  const int sms = usable_sms();
-  const int grid = (int)(work < sms ? work : sms);
-  const cudaError_t e =
-      launch_kernel(kern, dim3(grid), dim3(GEMM_THREADS), (size_t)L::DYN_BYTES, stream, ta, tb, p, (int)work);
-  if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "%s launch: %s", name, cudaGetErrorString(e));
-  return UNIVL_OK;
+  return persistent_launch(vocab_xent_kernel<BWD>, BWD ? "univl_vocab_xent_bwd" : "univl_vocab_xent_fwd", work,
+                           GemmSmem<VX_BLOCK_N, VX_STAGES>::DYN_BYTES, stream, ta, tb, p, (int)work);
 }
 
 }  // namespace univl
@@ -1291,6 +1137,37 @@ int plan_gemm(int M, int N, int Kc, int epilogue, int block_n, int split_k, Gemm
   plan->bn = bn; plan->splits = splits; plan->kb_per = kb_per; plan->kb_seg = kb_seg;
   return UNIVL_OK;
 }
+
+// the parameters of an unsplit launch (no split-K slots, kb_seg = kb_per), with the epilogue's vector widths read off
+// its operands' alignment
+GemmParams gemm_params(int M, int N, int Kc, int kb_per, int epilogue, float alpha, void* out, long long ldo,
+                       const float* bias, const void* aux_in, long long ld_aux_in, void* aux_out,
+                       long long ld_aux_out) {
+  GemmParams p;
+  p.M = M; p.N = N; p.Kc = Kc;
+  p.k_blocks_per_split = kb_per;
+  p.epilogue = epilogue;
+  p.alpha = alpha;
+  p.out = out; p.ldo = ldo;
+  p.bias = bias;
+  p.aux_in = reinterpret_cast<const bf16*>(aux_in); p.ld_aux_in = ld_aux_in;
+  p.aux_out = reinterpret_cast<bf16*>(aux_out); p.ld_aux_out = ld_aux_out;
+  // 2-element vector accesses need every epilogue operand's pairs (even columns) aligned to the pair size
+  const bool out_f32 = epilogue == EPI_BIAS_F32 || epilogue == EPI_ATOMIC_F32;
+  bool vec2 = ((uintptr_t)out % (out_f32 ? 8 : 4)) == 0 && (ldo % 2) == 0;
+  if (aux_in != nullptr) vec2 = vec2 && ((uintptr_t)aux_in % 4) == 0 && (ld_aux_in % 2) == 0;
+  if (aux_out != nullptr) vec2 = vec2 && ((uintptr_t)aux_out % 4) == 0 && (ld_aux_out % 2) == 0;
+  p.vec2 = vec2 ? 1 : 0;
+  // 16-byte stores of the bf16 outputs: 8-column groups start at multiples of 8 columns from a 16-byte aligned base
+  bool vec8 = !out_f32 && ((uintptr_t)out % 16) == 0 && (ldo % 8) == 0;
+  if (aux_out != nullptr) vec8 = vec8 && ((uintptr_t)aux_out % 16) == 0 && (ld_aux_out % 8) == 0;
+  p.vec8 = vec8 ? 1 : 0;
+  p.slots = nullptr;
+  p.arrived = nullptr;
+  p.splits = 1;
+  p.kb_seg = kb_per;
+  return p;
+}
 }  // namespace
 
 // Which kernel univl_gemm_bf16 launches for this problem: 1 = the persistent wgmma kernel (the only one); negative =
@@ -1335,27 +1212,8 @@ extern "C" int univl_gemm_bf16(const void* A, long long lda, int a_mn_major, con
   else             rc = make_tmap(&tb, B, Kc, N, ldb, BLOCK_K);
   if (rc) return rc;
 
-  GemmParams p;
-  p.M = M; p.N = N; p.Kc = Kc;
-  p.k_blocks_per_split = plan.kb_per;
-  p.epilogue = epilogue;
-  p.alpha = alpha;
-  p.out = out; p.ldo = ldo;
-  p.bias = bias;
-  p.aux_in = reinterpret_cast<const bf16*>(aux_in); p.ld_aux_in = ld_aux_in;
-  p.aux_out = reinterpret_cast<bf16*>(aux_out); p.ld_aux_out = ld_aux_out;
-  // 2-element vector accesses need every epilogue operand's pairs (even columns) aligned to the pair size
-  const bool out_f32 = epilogue == EPI_BIAS_F32 || epilogue == EPI_ATOMIC_F32;
-  bool vec2 = ((uintptr_t)out % (out_f32 ? 8 : 4)) == 0 && (ldo % 2) == 0;
-  if (aux_in != nullptr) vec2 = vec2 && ((uintptr_t)aux_in % 4) == 0 && (ld_aux_in % 2) == 0;
-  if (aux_out != nullptr) vec2 = vec2 && ((uintptr_t)aux_out % 4) == 0 && (ld_aux_out % 2) == 0;
-  p.vec2 = vec2 ? 1 : 0;
-  // 16-byte stores of the bf16 outputs: 8-column groups start at multiples of 8 columns from a 16-byte aligned base
-  bool vec8 = !out_f32 && ((uintptr_t)out % 16) == 0 && (ldo % 8) == 0;
-  if (aux_out != nullptr) vec8 = vec8 && ((uintptr_t)aux_out % 16) == 0 && (ld_aux_out % 8) == 0;
-  p.vec8 = vec8 ? 1 : 0;
-  p.slots = nullptr;
-  p.arrived = nullptr;
+  GemmParams p = gemm_params(M, N, Kc, plan.kb_per, epilogue, alpha, out, ldo, bias, aux_in, ld_aux_in, aux_out,
+                             ld_aux_out);
   p.splits = plan.splits;
   p.kb_seg = plan.kb_seg;
   if (plan.splits > 1) {  // the split-K fix-up's slots and arrival counters, one stream-ordered block
@@ -1408,21 +1266,7 @@ extern "C" int univl_gemm_fp8(const void* A, long long lda, const float* a_scale
   if ((rc = make_tmap(&ta, A, M, Kc, lda, BLOCK_M, true))) return rc;
   if ((rc = make_tmap(&tb, B, N, Kc, ldb, FP8_BLOCK_N, true))) return rc;
 
-  GemmParams p;
-  p.M = M; p.N = N; p.Kc = Kc;
-  p.k_blocks_per_split = Kc / 128;
-  p.epilogue = EPI_BIAS_BF16;
-  p.alpha = 1.f;
-  p.out = out; p.ldo = ldo;
-  p.bias = bias;
-  p.aux_in = nullptr; p.ld_aux_in = 0;
-  p.aux_out = nullptr; p.ld_aux_out = 0;
-  p.vec2 = (((uintptr_t)out % 4) == 0 && (ldo % 2) == 0) ? 1 : 0;
-  p.vec8 = (((uintptr_t)out % 16) == 0 && (ldo % 8) == 0) ? 1 : 0;
-  p.slots = nullptr;
-  p.arrived = nullptr;
-  p.splits = 1;
-  p.kb_seg = p.k_blocks_per_split;
+  const GemmParams p = gemm_params(M, N, Kc, Kc / 128, EPI_BIAS_BF16, 1.f, out, ldo, bias, nullptr, 0, nullptr, 0);
   Fp8Params f;
   f.a_scale = a_scale;
   f.b_scale = b_scale;
@@ -1477,17 +1321,15 @@ int vx_check(const char* name, const void* x, long long ldx, const void* w, long
   return UNIVL_OK;
 }
 
-// Sets the kernel's shared-memory attribute first: a runtime call, which also makes the device's primary context
-// current on this thread before the driver encodes the tensor maps (autograd runs backward on a thread of its own,
-// where this may be the first call of the process into CUDA).
+// Runs persistent_prepare first: a runtime call, which also makes the device's primary context current on this thread
+// before the driver encodes the tensor maps (autograd runs backward on a thread of its own, where this may be the
+// first call of the process into CUDA).
 template <bool BWD>
 int vx_params(const void* x, long long ldx, const void* w, long long ldw, int T, int V, int Kc, CUtensorMap* ta,
               CUtensorMap* tb, VocabXentParams* p) {
-  const cudaError_t e = cudaFuncSetAttribute(vocab_xent_kernel<BWD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             GemmSmem<VX_BLOCK_N, VX_STAGES>::DYN_BYTES);
-  if (e != cudaSuccess)
-    return set_error(UNIVL_ERR_CUDA, "%s smem attribute: %s", BWD ? "univl_vocab_xent_bwd" : "univl_vocab_xent_fwd",
-                     cudaGetErrorString(e));
+  if (int rc = persistent_prepare(vocab_xent_kernel<BWD>, GemmSmem<VX_BLOCK_N, VX_STAGES>::DYN_BYTES,
+                                  BWD ? "univl_vocab_xent_bwd" : "univl_vocab_xent_fwd"))
+    return rc;
   const VxPlan pl = vx_plan(T, V);
   int rc;
   if ((rc = make_tmap(ta, x, T, Kc, ldx, BLOCK_M))) return rc;
