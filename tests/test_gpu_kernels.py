@@ -8,6 +8,7 @@ import torch
 
 pytestmark = pytest.mark.gpu
 
+from tests import attn_check as ac  # noqa: E402
 from tests import gemm_check as gc  # noqa: E402
 from univl_b200 import ops  # noqa: E402
 from univl_b200 import runtime as rt  # noqa: E402
@@ -156,17 +157,12 @@ def test_dropout_statistics_and_backward_mask_consistency():
 
 
 # ---------------------------------------------------------------------------------------------------------
-def _attn_ref(q, k, v, add_mask):
-    s = torch.matmul(q, k.transpose(-1, -2)) / 8.0 + add_mask
-    return torch.matmul(torch.softmax(s, -1), v)
-
-
 @pytest.mark.parametrize("n_seq,Sq,Sk,causal", [(3, 48, 48, False), (2, 96, 96, False), (2, 20, 52, False),
                                                  (2, 128, 128, True), (1, 224, 224, False), (2, 33, 33, True),
                                                  (3, 1, 96, False),   # Sq = 1: first-token-only last cross layer
                                                  (1024, 96, 96, False), (1024, 1, 96, False)])  # all-pairs cross encoder
 def test_attention_fwd_bwd(n_seq, Sq, Sk, causal):
-    H, h = 768, 12
+    H = 768
     g = torch.Generator(device=DEV).manual_seed(Sq + Sk)
     q = _bf(torch.randn(n_seq * Sq, H, device=DEV, generator=g))
     kv = _bf(torch.randn(n_seq * Sk, 2 * H, device=DEV, generator=g))
@@ -177,31 +173,19 @@ def test_attention_fwd_bwd(n_seq, Sq, Sk, causal):
         mask[0] = 0  # a fully masked sequence: softmax of the raw scores, NOT NaN / uniform (SURVEY.md §4)
     spec = ops.MaskSpec(mask, causal=causal)
     o, lse = ops.attention_fwd(q, k, v, n_seq, Sq, Sk, spec)
-
-    def heads(t, S):
-        return t.float().view(n_seq, S, h, 64).permute(0, 2, 1, 3)
-    qf, kf, vf = heads(q, Sq).requires_grad_(), heads(k, Sk).requires_grad_(), heads(v, Sk).requires_grad_()
-    add = (1.0 - mask.float()).view(n_seq, 1, 1, Sk) * -10000.0
-    if causal:
-        fut = torch.triu(torch.ones(Sq, Sk, device=DEV), diagonal=1).view(1, 1, Sq, Sk)
-        add = ((1.0 - mask.float()).view(n_seq, 1, 1, Sk) + fut).gt(0).float() * -10000.0
-    ref = _attn_ref(qf, kf, vf, add)
-    ref2d = ref.permute(0, 2, 1, 3).reshape(n_seq * Sq, H)
-    assert torch.isfinite(o.float()).all()
-    assert (o.float() - ref2d).abs().max() <= 3e-2
     d_o = _bf(torch.randn(n_seq * Sq, H, device=DEV, generator=g))
-    ref2d.backward(d_o.float())
     dq = torch.empty_like(q)
     dkv = torch.empty_like(kv)
     dbias = torch.ones(3, H, device=DEV)  # accumulated into: starts at 1
     ops.attention_bwd(q, k, v, o, lse, d_o, dq, dkv[:, :H], dkv[:, H:], n_seq, Sq, Sk, spec,
                       dbias=(dbias[0], dbias[1], dbias[2]))
-
-    def unheads(t, S):
-        return t.permute(0, 2, 1, 3).reshape(n_seq * S, H)
-    for n, (got, want, S) in enumerate(((dq, qf.grad, Sq), (dkv[:, :H], kf.grad, Sk), (dkv[:, H:], vf.grad, Sk))):
-        want = unheads(want, S)
-        assert (got.float() - want).abs().max() <= 4e-2 * max(1.0, float(want.abs().max()))
+    torch.cuda.synchronize()
+    # every output element against fp64 (tests/attn_check.py)
+    what = "attention n%d Sq%d Sk%d causal%d" % (n_seq, Sq, Sk, causal)
+    ref = ac.reference(q, k, v, n_seq, Sq, Sk, mask, causal, d_o=d_o, o_kernel=o)
+    ac.check_fwd(o, lse, ref, what)
+    ac.check_bwd(dq, dkv[:, :H], dkv[:, H:], ref, what)
+    for n, got in enumerate((dq, dkv[:, :H], dkv[:, H:])):
         # fused projection-bias gradient = column sums of the same gradient (fp32 accumulators, before the bf16
         # rounding of the stored tile): equal to the column sums of what was stored up to that rounding, 2^-9 per
         # element.  (The sums themselves may cancel to ~0 — dK columns do, exactly, in exact arithmetic — so the bound
@@ -285,34 +269,26 @@ def _fused_inputs(n_seq, S, seed):
                                             (9, 16, True), (4, 32, False), (3, 64, False), (2, 80, False), (1, 112, False),
                                             (40, 96, False), (301, 48, False)])
 def test_fused_qkv_attention_fwd_matches_unfused_and_fp32(n_seq, S, causal):
-    """ONE wgmma kernel (projection + softmax(QK^T)V) against (a) fp32 PyTorch on the same bf16 inputs and (b) the
-    QKV-GEMM + attention-core pair; packed sequences (S = 16 ... 64), partial last row block, several items per CTA."""
-    H, h = 768, 12
+    """ONE wgmma kernel (projection + softmax(QK^T)V) and the QKV-GEMM + attention-core pair on its q/k/v, both per
+    element against fp64 (tests/attn_check.py); packed sequences (S = 16 ... 64), partial last row block, several items
+    per CTA."""
+    H = 768
     assert ops.fused_attention_supported(n_seq, S, H)
     x, w, b, mask = _fused_inputs(n_seq, S, S + n_seq)
     spec = ops.MaskSpec(mask, causal=causal)
     o, lse, qkv = ops.fused_qkv_attention_fwd(x, w, b, n_seq, S, spec)
     torch.cuda.synchronize()
-    assert torch.isfinite(o.float()).all() and torch.isfinite(lse).all()
-    qkv_ref = _bf(x.float() @ w.float().t() + b)                      # the kernel rounds q/k/v to bf16 operand tiles
-    assert (qkv.float() - qkv_ref.float()).abs().max() <= 2.0 ** -7 * max(1.0, float(qkv_ref.float().abs().max()))
-
-    def heads(t):
-        return t.float().view(n_seq, S, h, 64).permute(0, 2, 1, 3)
-    qf, kf, vf = heads(qkv_ref[:, :H]), heads(qkv_ref[:, H:2 * H]), heads(qkv_ref[:, 2 * H:])
-    add = (1.0 - mask.float()).view(n_seq, 1, 1, S) * -10000.0
-    if causal:
-        fut = torch.triu(torch.ones(S, S, device=DEV), diagonal=1).view(1, 1, S, S)
-        add = ((1.0 - mask.float()).view(n_seq, 1, 1, S) + fut).gt(0).float() * -10000.0
-    sc = torch.matmul(qf, kf.transpose(-1, -2)) / 8.0 + add
-    ref = torch.matmul(torch.softmax(sc, -1), vf).permute(0, 2, 1, 3).reshape(n_seq * S, H)
-    assert (o.float() - ref).abs().max() <= 3e-2
-    lse_ref = torch.logsumexp(sc, -1).reshape(-1)
-    assert (lse - lse_ref).abs().max() <= 2e-2 + 2e-3 * float(lse_ref.abs().max())
+    what = "fused n%d S%d causal%d" % (n_seq, S, causal)
+    # the saved q/k/v per element (tests/gemm_check.py), then the attention on them against fp64 (tests/attn_check.py)
+    acc, mag = gc.mm64(x, w)
+    qkv_ref = acc + b.double()
+    gc.within(qkv, qkv_ref, gc.elem_bound(mag, H, b.double().abs(), qkv_ref), what + " qkv")
+    q, k, v = qkv[:, :H], qkv[:, H:2 * H], qkv[:, 2 * H:]
+    ref = ac.reference(q, k, v, n_seq, S, S, mask, causal, kind="fused")
+    ac.check_fwd(o, lse, ref, what)
     # the unfused pair on the kernel's own q/k/v
-    o2, lse2 = ops.attention_fwd(qkv[:, :H], qkv[:, H:2 * H], qkv[:, 2 * H:], n_seq, S, S, spec)
-    assert (o.float() - o2.float()).abs().max() <= 2e-2
-    assert (lse - lse2).abs().max() <= 2e-3 * max(1.0, float(lse2.abs().max()))
+    o2, lse2 = ops.attention_fwd(q, k, v, n_seq, S, S, spec)
+    ac.check_fwd(o2, lse2, ref, what + " unfused")
     # no q/k/v copy requested: same context
     o3, _, none = ops.fused_qkv_attention_fwd(x, w, b, n_seq, S, spec, save_qkv=False)
     assert none is None and torch.equal(o3, o)
@@ -323,9 +299,9 @@ def test_fused_qkv_attention_fwd_matches_unfused_and_fp32(n_seq, S, causal):
                                               (40, 96, False, 0.0), (3, 48, False, 0.25), (2, 128, False, 0.25),
                                               (301, 48, False, 0.1), (1024, 96, False, 0.0), (1024, 96, False, 0.1)])
 def test_fused_attention_bwd_matches_fp32_and_unfused_backward(n_seq, S, causal, p):
-    """wgmma attention backward: (p = 0) against fp32 autograd of the same op, and (any p) against the mma.sync
-    backward kernel regenerating the same row-major dropout mask; bias-gradient column sums included."""
-    H, h = 768, 12
+    """wgmma attention backward and the mma.sync backward regenerating the same row-major dropout mask, both against
+    fp64 under that mask (tests/attn_check.py); bias-gradient column sums included."""
+    H = 768
     x, w, b, mask = _fused_inputs(n_seq, S, 100 + S + n_seq)
     spec = ops.MaskSpec(mask, causal=causal)
     o, lse, qkv = ops.fused_qkv_attention_fwd(x, w, b, n_seq, S, spec, p=p, seed=RNG.data_ptr(), stream=7)
@@ -342,10 +318,15 @@ def test_fused_attention_bwd_matches_fp32_and_unfused_backward(n_seq, S, causal,
     ops.attention_bwd(qkv[:, :H], qkv[:, H:2 * H], qkv[:, 2 * H:], o, lse, d_o, dq2[:, :H], dq2[:, H:2 * H],
                       dq2[:, 2 * H:], n_seq, S, S, spec, p=p, seed=RNG.data_ptr(), stream=7,
                       dbias=(db2[0], db2[1], db2[2]), rng_layout=1)
-    scale = max(1.0, float(dq2.float().abs().max()))
-    assert (dqkv.float() - dq2.float()).abs().max() <= 3e-2 * scale
-    rel = float((dqkv.float() - dq2.float()).norm() / dq2.float().norm())
-    assert rel <= 1e-2, rel
+    torch.cuda.synchronize()
+    what = "fused bwd n%d S%d causal%d p%g" % (n_seq, S, causal, p)
+    rng = [int(t) for t in RNG.cpu()]
+    keep = ac.keep_rowmajor(rng[0], ac.kernel_stream(7, rng[1]), p, n_seq * 12, S) if p > 0 else None
+    ref = ac.reference(qkv[:, :H], qkv[:, H:2 * H], qkv[:, 2 * H:], n_seq, S, S, mask, causal, keep, p, d_o=d_o,
+                       o_kernel=o, kind="fused")
+    ac.check_fwd(o, lse, ref, what)
+    ac.check_bwd(dqkv[:, :H], dqkv[:, H:2 * H], dqkv[:, 2 * H:], ref, what)
+    ac.check_bwd(dq2[:, :H], dq2[:, H:2 * H], dq2[:, 2 * H:], ref, what + " mma.sync")
     tol = dqkv.float().abs().sum(0) * 2.0 ** -7 + 2e-3
     assert bool(((dbias - 1.0 - dqkv.float().sum(0)).abs() <= tol).all())
 
@@ -355,23 +336,6 @@ def test_fused_attention_bwd_matches_fp32_and_unfused_backward(n_seq, S, causal,
         return [dq_, db_]
     for a, b in zip((dqkv, dbias), _same_bits(again, launches=2)):
         assert torch.equal(a, b)
-    if p == 0.0:
-        # (b) fp32 autograd
-        def heads(t):
-            return t.float().view(n_seq, S, h, 64).permute(0, 2, 1, 3)
-        qf = heads(qkv[:, :H]).requires_grad_()
-        kf = heads(qkv[:, H:2 * H]).requires_grad_()
-        vf = heads(qkv[:, 2 * H:]).requires_grad_()
-        add = (1.0 - mask.float()).view(n_seq, 1, 1, S) * -10000.0
-        if causal:
-            fut = torch.triu(torch.ones(S, S, device=DEV), diagonal=1).view(1, 1, S, S)
-            add = ((1.0 - mask.float()).view(n_seq, 1, 1, S) + fut).gt(0).float() * -10000.0
-        ref = _attn_ref(qf, kf, vf, add).permute(0, 2, 1, 3).reshape(n_seq * S, H)
-        ref.backward(d_o.float())
-        for n, gr in enumerate((qf.grad, kf.grad, vf.grad)):
-            want = gr.permute(0, 2, 1, 3).reshape(n_seq * S, H)
-            got = dqkv[:, n * H:(n + 1) * H].float()
-            assert (got - want).abs().max() <= 4e-2 * max(1.0, float(want.abs().max())), n
 
 
 def _all_pairs_fused_case(Na, Nb, W, F):
