@@ -161,6 +161,31 @@ int univl_attention_pair_fwd(const void* qa, long long ldqa, const void* ka, lon
                              const void* vb, long long ldvb, void* o, long long ldo, float* lse,
                              const long long* mask_a, const long long* mask_b, int Na, int Wa, int Nb, int Fb,
                              int heads, int Sq, float scale, void* stream);
+/* Forward only, no dropout, no mask: the attention core of n_seq variable-length sequences in one launch.  Sequence p
+ * has Sk_p = cu_seqlens[p + 1] - cu_seqlens[p] keys (int32 [n_seq + 1], ascending), all of them real.  Two row
+ * addressings of q/k/v:
+ *   - pair (idx_a non-null): row r < len_a[p] of sequence p is row idx_a[start_a[p] + r] of (qa, ka, va), row
+ *     r >= len_a[p] is row idx_b[start_b[p] + r - len_a[p]] of (qb, kb, vb) — univl_attention_pair_fwd's two sources
+ *     with per-row index lists (int32) in place of i * Wa + r / j * Fb + r - Wa;
+ *   - packed (idx_a, idx_b, start_a, start_b, len_a all null): row r of sequence p is row cu_seqlens[p] + r of
+ *     (qa, ka, va); qb / kb / vb are ignored.
+ * q_first = 0: every row queries and the context row of (p, r) is o[cu_seqlens[p] + r]; q_first = 1: one query per
+ * sequence, its row 0 (under packed addressing: row p of qa instead), context in o[p].  lse (nullable) is fp32
+ * [context rows, heads].  max_sk >= every Sk_p, 0 < max_sk <= 1024, sizes the launch: univl_attention_fwd's kernel up to
+ * 256 keys, univl_attention_long_fwd's above; a sequence computes exactly what those kernels compute for it alone.  A
+ * sequence without keys writes nothing.  12 heads; row strides multiples of 8 and 16-byte aligned q/k/v. */
+int univl_attention_varlen_fwd(const void* qa, long long ldqa, const void* ka, long long ldka, const void* va,
+                               long long ldva, const void* qb, long long ldqb, const void* kb, long long ldkb,
+                               const void* vb, long long ldvb, const int* idx_a, const int* idx_b, const int* start_a,
+                               const int* start_b, const int* len_a, const int* cu_seqlens, int n_seq, int max_sk,
+                               int heads, int q_first, void* o, long long ldo, float* lse, float scale, void* stream);
+/* The rows of univl_attention_varlen_fwd's sequences gathered into packed order: with the same addressing (pair: a, b
+ * and the index lists; packed: a alone), row r of sequence p is copied to out[cu_seqlens[p] + r], or with q_first = 1
+ * only row 0, to out[p].  bf16 [*, cols], cols a multiple of 8, 16-byte aligned rows (16-byte vectors). */
+int univl_gather_rows_varlen(const void* a, long long lda, const void* b, long long ldb, const int* idx_a,
+                             const int* idx_b, const int* start_a, const int* start_b, const int* len_a,
+                             const int* cu_seqlens, int n_seq, int q_first, int cols, void* out, long long ldo,
+                             void* stream);
 /* ---- fused QKV projection + self-attention, forward (wgmma / TMA; module_bert.py:171-197 as ONE kernel) --------------
  * ctx[T,H] = merge_heads(dropout(softmax((x Wq^T + bq)(x Wk^T + bk)^T * scale + mask)) (x Wv^T + bv)), T = n_seq * S,
  * H = heads * 64 = 768.  wqkv: bf16 [3H, H] (query | key | value rows), bias fp32 [3H].  The [T,3H] projections and the

@@ -18,11 +18,20 @@ one call per size and precision under torch.profiler, in runs of their own, spli
 (gemm_wgmma_kernel, gemm_fp8_kernel) and all other work.  The card's name, power limit and SM clock are read in the
 same call.  Prints one JSON line per row, then a table.
 
+--layout padded,packed alternates the tiled path's layouts (UNIVL_EVAL_LAYOUT) within every run as well, the pairs
+computed at W + F tokens or on their valid tokens alone, and --valid picks the valid-length distributions, each run
+in turn: "uniform" (default; text and clip lengths uniform in [L/4, L]) and "short" (text 8-20 tokens, clips 12-30
+frames).  Rows then also give the packed-token fraction (valid pair tokens / padded pair tokens), the max |logit
+difference| of packed against padded at the same precision, and a second rate, tflop_per_s_packed: the FLOPs of the
+packed tokens actually computed (same formula, S the pair's valid tokens) per second.  tflop_per_s stays the
+algorithmic count over padded tokens for every layout.
+
 FLOPs (multiply-add = 2) per pair at S = W + F, H = 768, I = 3072, L cross layers, the last one token-0 only:
   (L-1) S (8H^2 + 4HI + 4SH)  +  S 4H^2 (last layer K/V)  +  2H^2 + 4SH + 2H^2 + 4HI (last layer, token 0)  +  2H^2
   (pooler); (b) does S 6H^2 less per pair (first layer Q/K/V) and (Nt W + Nv F) 6H^2 once per call.
 
 usage: python scripts/bench_retrieval_eval.py [--old 128] [--sizes 1024,3500] [--runs 3] [--precision bf16,fp8]
+                                             [--layout padded,packed] [--valid uniform,short]
 """
 import argparse
 import json
@@ -57,6 +66,20 @@ def flops(Nt, Nv, tiled):
     return Nt * Nv * (per_pair - S * 6 * H * H) + (Nt * W + Nv * F) * 6 * H * H
 
 
+def flops_packed(am, vm):
+    """flops(tiled=True) with every pair at its valid length S_ij = len_t(i) + len_v(j): sums of S and S^2 over pairs"""
+    lt, lv = am.sum(1).double().cpu(), vm.sum(1).double().cpu()
+    Nt, Nv = lt.numel(), lv.numel()
+    T = float(Nv * lt.sum() + Nt * lv.sum())                                         # sum of S
+    Q = float(Nv * (lt * lt).sum() + 2 * lt.sum() * lv.sum() + Nt * (lv * lv).sum())  # sum of S^2
+    return ((LAYERS - 1) * (T * (8 * H * H + 4 * H * I) + 4 * Q * H) + T * 4 * H * H
+            + Nt * Nv * (6 * H * H + 4 * H * I) + 4 * T * H - T * 6 * H * H + (Nt * W + Nv * F) * 6 * H * H)
+
+
+# valid-length range per role (text rows, video rows), inclusive; None: uniform in [L/4, L] for a row of L tokens
+VALID = {"uniform": None, "short": {"text": (8, 20), "video": (12, 30)}}
+
+
 def build():
     from oracle import synth
     from tests.model_util import build_model
@@ -65,17 +88,21 @@ def build():
     return build_model(cfg, seed=0).eval()
 
 
-def inputs(N, seed):
+def inputs(N, seed, valid="uniform"):
+    """N random rows of encoder output and their mask: text rows (W tokens) for an even seed, video rows (F) for odd"""
     g = torch.Generator().manual_seed(seed)
-    x = torch.randn(N, W if seed % 2 == 0 else F, H, generator=g).to(torch.bfloat16).cuda()
-    L = x.shape[1]
-    lens = torch.randint(L // 4, L + 1, (N,), generator=g)
+    role = "text" if seed % 2 == 0 else "video"
+    L = W if role == "text" else F
+    x = torch.randn(N, L, H, generator=g).to(torch.bfloat16).cuda()
+    lo, hi = VALID[valid][role] if VALID[valid] else (L // 4, L)
+    lens = torch.randint(lo, hi + 1, (N,), generator=g)
     return x, (torch.arange(L).view(1, L) < lens.view(N, 1)).long().cuda()
 
 
-def run(model, N, tiled, seq, vis, am, vm, precision="bf16"):
+def run(model, N, tiled, seq, vis, am, vm, precision="bf16", layout="padded"):
     from univl_b200 import runtime as rt
     os.environ["UNIVL_EVAL_PRECISION"] = precision
+    os.environ["UNIVL_EVAL_LAYOUT"] = layout
     s2, v2 = seq.reshape(-1, H), vis.reshape(-1, H)
     with torch.no_grad(), rt.use_model(model, seq.device):
         torch.cuda.synchronize()
@@ -92,32 +119,43 @@ def run(model, N, tiled, seq, vis, am, vm, precision="bf16"):
     return out, ms, peak
 
 
-def profile(model, N, seq, vis, am, vm, precision):
-    """GPU time of one tiled call, split into GEMM kernels and everything else"""
+def profile(model, N, seq, vis, am, vm, precision, layout="padded", valid="uniform"):
+    """GPU time of one tiled call, split into GEMM kernels, attention kernels and everything else"""
     from torch.autograd import DeviceType
     from torch.profiler import ProfilerActivity
     with torch.profiler.profile(activities=[ProfilerActivity.CUDA]) as prof:
-        run(model, N, True, seq, vis, am, vm, precision)
-    gemm = other = 0.0
+        run(model, N, True, seq, vis, am, vm, precision, layout)
+    gemm = attn = other = 0.0
     for e in prof.key_averages():
         if e.device_type != DeviceType.CUDA:
             continue
         if "gemm" in e.key:
             gemm += e.self_device_time_total
+        elif "attention" in e.key:
+            attn += e.self_device_time_total
         else:
             other += e.self_device_time_total
-    r = dict(profile="tiled", precision=precision, Nt=N, Nv=N, gemm_ms=round(gemm / 1e3, 1),
-             other_ms=round(other / 1e3, 1), gemm_share=round(gemm / max(gemm + other, 1e-9), 3))
+    r = dict(profile="tiled", precision=precision, layout=layout, valid=valid, Nt=N, Nv=N,
+             gemm_ms=round(gemm / 1e3, 1), attention_ms=round(attn / 1e3, 1), other_ms=round(other / 1e3, 1),
+             gemm_share=round(gemm / max(gemm + attn + other, 1e-9), 3))
     print(json.dumps(r), flush=True)
     return r
 
 
-def row(name, N, tiled, ms, peak, precision="bf16", dlogit=None):
+def row(name, N, tiled, ms, peak, precision="bf16", dlogit=None, layout="padded", valid="uniform", masks=None,
+        dpacked=None):
     from univl_b200.modules import modeling
     f = flops(N, N, tiled)
-    r = dict(path=name, precision=precision, Nt=N, Nv=N, W=W, F=F, cross_layers=LAYERS, ms=round(ms, 2),
-             pairs_per_s=round(N * N / ms * 1e3), tflop=round(f / 1e12, 2), tflop_per_s=round(f / ms / 1e9, 1),
-             peak_gib=round(peak / 2 ** 30, 3))
+    r = dict(path=name, precision=precision, layout=layout, valid=valid, Nt=N, Nv=N, W=W, F=F, cross_layers=LAYERS,
+             ms=round(ms, 2), pairs_per_s=round(N * N / ms * 1e3), tflop=round(f / 1e12, 2),
+             tflop_per_s=round(f / ms / 1e9, 1), peak_gib=round(peak / 2 ** 30, 3))
+    if masks is not None:
+        am, vm = masks
+        r["packed_fraction"] = round(float(N * (am.sum() + vm.sum())) / (N * N * (W + F)), 4)
+        if layout == "packed":
+            r["tflop_per_s_packed"] = round(flops_packed(am, vm) / ms / 1e9, 1)
+    if dpacked is not None:
+        r["max_abs_dlogit_vs_padded"] = dpacked
     if tiled:
         per_source = 2 * N * W * (H + 3 * H) * 2   # source embedding rows and their Q/K/V projections
         r["tile_peak_gib"] = round((peak - per_source - N * N * 4) / 2 ** 30, 3)
@@ -135,8 +173,14 @@ def main():
     ap.add_argument("--sizes", default="1024,3500")
     ap.add_argument("--runs", type=int, default=3)
     ap.add_argument("--precision", default="bf16", help="comma-separated eval precisions of the tiled path: bf16,fp8")
+    ap.add_argument("--layout", default="padded", help="comma-separated eval layouts of the tiled path: padded,packed")
+    ap.add_argument("--valid", default="uniform", help="comma-separated valid-length distributions: uniform,short")
     a = ap.parse_args()
     precisions = [p for p in a.precision.split(",") if p]
+    layouts = [x for x in a.layout.split(",") if x]
+    if "padded" not in layouts:
+        layouts.insert(0, "padded")  # the reference result of the packed logit differences
+    valids = [x for x in a.valid.split(",") if x]
     if "bf16" not in precisions:
         precisions.insert(0, "bf16")  # the reference result of the logit differences
     if not torch.cuda.is_available():
@@ -160,41 +204,55 @@ def main():
     print(json.dumps({"max_abs_logit_diff_tiled_vs_all_pairs": diff, "N": N}), flush=True)
     del seq, vis, am, vm, outs
     profiles = []
-    for N in [int(s) for s in a.sizes.split(",") if s]:
-        seq, am = inputs(N, 2)
-        vis, vm = inputs(N, 3)
-        n = min(N, 512)  # warm-up of every precision at every size: loads each kernel before the timed calls
-        for p in precisions:
-            run(model, n, True, seq[:n], vis[:n], am[:n], vm[:n], p)
-        runs = 1 if N > 2048 and len(precisions) == 1 else a.runs
-        for _ in range(runs):
-            ref = None
-            for p in precisions:
-                out, ms, peak = run(model, N, True, seq, vis, am, vm, p)
-                d = None
-                if p == "bf16":
-                    ref = out
-                elif ref is not None:
-                    d = float((out - ref).abs().max())
-                rows.append(row("tiled", N, True, ms, peak, p, d))
-                del out
-            del ref
-        if len(precisions) > 1:
-            for p in precisions:
-                profiles.append(profile(model, N, seq, vis, am, vm, p))
-        del seq, vis, am, vm
+    for valid in valids:
+        for N in [int(s) for s in a.sizes.split(",") if s]:
+            seq, am = inputs(N, 2, valid)
+            vis, vm = inputs(N, 3, valid)
+            n = min(N, 512)  # warm-up of every variant at every size: loads each kernel before the timed calls
+            for lay in layouts:
+                for p in precisions:
+                    run(model, n, True, seq[:n], vis[:n], am[:n], vm[:n], p, lay)
+            runs = 1 if N > 2048 and len(precisions) * len(layouts) == 1 else a.runs
+            for _ in range(runs):
+                ref = None
+                padded = {}
+                for lay in layouts:
+                    for p in precisions:
+                        out, ms, peak = run(model, N, True, seq, vis, am, vm, p, lay)
+                        d = dp = None
+                        if lay == "padded":
+                            padded[p] = out
+                        elif p in padded:
+                            dp = float((out - padded[p]).abs().max())
+                        if p == "bf16" and lay == "padded":
+                            ref = out
+                        elif p != "bf16" and ref is not None:
+                            d = float((out - ref).abs().max())
+                        rows.append(row("tiled", N, True, ms, peak, p, d, lay, valid, (am, vm), dp))
+                        del out
+                del ref, padded
+            if len(precisions) * len(layouts) > 1:
+                for lay in layouts:
+                    for p in precisions:
+                        profiles.append(profile(model, N, seq, vis, am, vm, p, lay, valid))
+            del seq, vis, am, vm
     os.environ.pop("UNIVL_EVAL_PRECISION", None)
-    print("\n| path | precision | pairs | ms | pairs/s | TFLOP | TFLOP/s | peak GiB |")
-    print("|---|---|---|---|---|---|---|---|")
+    os.environ.pop("UNIVL_EVAL_LAYOUT", None)
+    print("\n| path | layout | valid | precision | pairs | ms | pairs/s | packed frac | TFLOP | TFLOP/s (padded) "
+          "| TFLOP/s (packed) | max dlogit vs padded | peak GiB |")
+    print("|---|---|---|---|---|---|---|---|---|---|---|---|---|")
     for r in rows:
-        print("| %s | %s | %d x %d | %.1f | %.3g | %.2f | %.1f | %.2f |" % (
-            r["path"], r["precision"], r["Nt"], r["Nv"], r["ms"], r["pairs_per_s"], r["tflop"], r["tflop_per_s"],
-            r["peak_gib"]))
+        print("| %s | %s | %s | %s | %d x %d | %.1f | %.3g | %s | %.2f | %.1f | %s | %s | %.2f |" % (
+            r["path"], r["layout"], r["valid"], r["precision"], r["Nt"], r["Nv"], r["ms"], r["pairs_per_s"],
+            r.get("packed_fraction", "-"), r["tflop"], r["tflop_per_s"], r.get("tflop_per_s_packed", "-"),
+            r.get("max_abs_dlogit_vs_padded", "-"), r["peak_gib"]))
     if profiles:
-        print("\n| precision | pairs | GEMM ms | other ms | GEMM share |\n|---|---|---|---|---|")
+        print("\n| layout | valid | precision | pairs | GEMM ms | attention ms | other ms | GEMM share |\n"
+              "|---|---|---|---|---|---|---|---|")
         for r in profiles:
-            print("| %s | %d x %d | %.1f | %.1f | %.2f |" % (r["precision"], r["Nt"], r["Nv"], r["gemm_ms"],
-                                                            r["other_ms"], r["gemm_share"]))
+            print("| %s | %s | %s | %d x %d | %.1f | %.1f | %.1f | %.2f |" % (
+                r["layout"], r["valid"], r["precision"], r["Nt"], r["Nv"], r["gemm_ms"], r["attention_ms"],
+                r["other_ms"], r["gemm_share"]))
 
 
 if __name__ == "__main__":

@@ -51,16 +51,22 @@ __device__ __forceinline__ void tile_rng_rowmajor(const AttnParams& p, long long
 // ------------------------------------------------------------------------------------------------------------
 // NKB > 0: the whole score row (<= NKB 16-key blocks) stays in registers — one QK^T pass, exact softmax, 2 * NKB
 // independent accumulator chains for the tensor pipe.  NKB == 0: 16-key chunks with a stats pre-pass (any Sk <= 256).
-// PAIR: the Q/K/V rows come from two sources (load_pair_tile; univl_attention_pair_fwd).
-template <int NKB, bool PAIR>
+// ADDR: the row addressing of Q/K/V (attention_common.cuh Addr).  Under the varlen addressings each CTA takes its own
+// sequence's Sq / Sk (the launch is sized for the longest) and writes output / lse at VarlenSrc's rows.
+template <int NKB, int ADDR>
 __global__ void __launch_bounds__(ATT_FWD_WARPS * 32)  // (capping S=96 at 112 registers for 3 CTAs/SM measured 6% slower)
-attention_fwd_kernel(const AttnParams p_in, const PairSrc pb) {
+attention_fwd_kernel(const AttnParams p_in, const PairSrc pb, const VarlenSrc vl) {
   pdl_trigger();
   pdl_wait();
   AttnParams p = p_in;
   if (p.drop_on && p.rng != nullptr) {
     p.seed = p.rng[0];
     p.stream += p.rng[1] << 20;
+  }
+  constexpr bool VARLEN = ADDR == ADDR_VARLEN_PAIR || ADDR == ADDR_VARLEN_PACKED;
+  if constexpr (VARLEN) {
+    varlen_shape(p, vl, blockIdx.x / p.heads);
+    if (p.Sk <= 0) return;
   }
   extern __shared__ __align__(16) uint8_t smem_att[];
   const int Sq16 = (p.Sq + 15) & ~15, Sk16 = (p.Sk + 15) & ~15;
@@ -74,7 +80,11 @@ attention_fwd_kernel(const AttnParams p_in, const PairSrc pb) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
 
-  if constexpr (PAIR) {
+  if constexpr (VARLEN) {
+    load_varlen_q(sQ, p.q, p.ldq, pb.q, pb.ldq, vl, seq, h, 0, p.Sq, Sq16);
+    load_varlen_tile(sK, p.k, p.ldk, pb.k, pb.ldk, vl, seq, h, 0, p.Sk, Sk16);
+    load_varlen_tile(sV, p.v, p.ldv, pb.v, pb.ldv, vl, seq, h, 0, p.Sk, Sk16);
+  } else if constexpr (ADDR == ADDR_PAIR) {
     load_pair_tile(sQ, p.q, p.ldq, pb.q, pb.ldq, p, seq, h, 0, p.Sq, Sq16);
     load_pair_tile(sK, p.k, p.ldk, pb.k, pb.ldk, p, seq, h, 0, p.Sk, Sk16);
     load_pair_tile(sV, p.v, p.ldv, pb.v, pb.ldv, p, seq, h, 0, p.Sk, Sk16);
@@ -170,16 +180,18 @@ attention_fwd_kernel(const AttnParams p_in, const PairSrc pb) {
           pa[3] = pack_bf16x2(s[kb][1][2], s[kb][1][3]);
           mma_p_z(pa, sV, kb * 16, lane, o);
         }
-      bf16* orow0 = p.o + ((long long)seq * p.Sq + i0) * p.ldo + h * HD;
-      bf16* orow1 = p.o + ((long long)seq * p.Sq + i1) * p.ldo + h * HD;
+      // output row of query 0; lse [n_seq, heads, Sq], or [rows, heads] under the varlen addressings
+      const long long ob = VARLEN ? varlen_out_row(vl, seq) : (long long)seq * p.Sq;
+      bf16* orow0 = p.o + (ob + i0) * p.ldo + h * HD;
+      bf16* orow1 = p.o + (ob + i1) * p.ldo + h * HD;
 #pragma unroll
       for (int nb = 0; nb < 8; ++nb) {
         if (i0 < p.Sq) *reinterpret_cast<uint32_t*>(orow0 + nb * 8 + 2 * t) = pack_bf16x2(o[nb][0], o[nb][1]);
         if (i1 < p.Sq) *reinterpret_cast<uint32_t*>(orow1 + nb * 8 + 2 * t) = pack_bf16x2(o[nb][2], o[nb][3]);
       }
       if (t == 0 && p.lse != nullptr) {
-        if (i0 < p.Sq) p.lse[bh * p.Sq + i0] = mx0 + __logf(sum0);
-        if (i1 < p.Sq) p.lse[bh * p.Sq + i1] = mx1 + __logf(sum1);
+        if (i0 < p.Sq) p.lse[VARLEN ? (ob + i0) * p.heads + h : bh * p.Sq + i0] = mx0 + __logf(sum0);
+        if (i1 < p.Sq) p.lse[VARLEN ? (ob + i1) * p.heads + h : bh * p.Sq + i1] = mx1 + __logf(sum1);
       }
       continue;
     }
@@ -269,16 +281,17 @@ attention_fwd_kernel(const AttnParams p_in, const PairSrc pb) {
       mma_p_z(pa, sV, j0, lane, o);
     }
     // store context rows (heads merged: column h*64 + d) and the row log-sum-exp
-    bf16* orow0 = p.o + ((long long)seq * p.Sq + i0) * p.ldo + h * HD;
-    bf16* orow1 = p.o + ((long long)seq * p.Sq + i1) * p.ldo + h * HD;
+    const long long ob = VARLEN ? varlen_out_row(vl, seq) : (long long)seq * p.Sq;
+    bf16* orow0 = p.o + (ob + i0) * p.ldo + h * HD;
+    bf16* orow1 = p.o + (ob + i1) * p.ldo + h * HD;
 #pragma unroll
     for (int nb = 0; nb < 8; ++nb) {
       if (i0 < p.Sq) *reinterpret_cast<uint32_t*>(orow0 + nb * 8 + 2 * t) = pack_bf16x2(o[nb][0], o[nb][1]);
       if (i1 < p.Sq) *reinterpret_cast<uint32_t*>(orow1 + nb * 8 + 2 * t) = pack_bf16x2(o[nb][2], o[nb][3]);
     }
     if (t == 0 && p.lse != nullptr) {
-      if (i0 < p.Sq) p.lse[bh * p.Sq + i0] = m0 + __logf(l0);
-      if (i1 < p.Sq) p.lse[bh * p.Sq + i1] = m1 + __logf(l1);
+      if (i0 < p.Sq) p.lse[VARLEN ? (ob + i0) * p.heads + h : bh * p.Sq + i0] = m0 + __logf(l0);
+      if (i1 < p.Sq) p.lse[VARLEN ? (ob + i1) * p.heads + h : bh * p.Sq + i1] = m1 + __logf(l1);
     }
   }
 }
@@ -602,19 +615,21 @@ attention_bwd_kernel(const AttnParams p_in) {
   }
 }
 
-int attention_fwd_launch(const AttnParams& p, bool pair, const PairSrc& pb, cudaStream_t stream) {
+template <int ADDR>
+static void (*fwd_kernel_for(int nkb))(const AttnParams, const PairSrc, const VarlenSrc) {
+  return nkb <= 3 ? attention_fwd_kernel<3, ADDR>
+         : nkb <= 6 ? attention_fwd_kernel<6, ADDR>
+         : nkb <= 8 ? attention_fwd_kernel<8, ADDR> : attention_fwd_kernel<0, ADDR>;
+}
+
+int attention_fwd_launch(const AttnParams& p, Addr addr, const PairSrc& pb, const VarlenSrc& vl, cudaStream_t stream) {
   const int Sq16 = (p.Sq + 15) & ~15, Sk16 = (p.Sk + 15) & ~15;
   const size_t smem = (size_t)(Sq16 + 2 * Sk16) * LDS * 2 + (size_t)Sk16 * 4;
   const int nkb = Sk16 / 16;
-  void (*kern)(const AttnParams, const PairSrc);
-  if (pair)
-    kern = nkb <= 3 ? attention_fwd_kernel<3, true>
-           : nkb <= 6 ? attention_fwd_kernel<6, true>
-           : nkb <= 8 ? attention_fwd_kernel<8, true> : attention_fwd_kernel<0, true>;
-  else
-    kern = nkb <= 3 ? attention_fwd_kernel<3, false>
-           : nkb <= 6 ? attention_fwd_kernel<6, false>
-           : nkb <= 8 ? attention_fwd_kernel<8, false> : attention_fwd_kernel<0, false>;
+  void (*kern)(const AttnParams, const PairSrc, const VarlenSrc) =
+      addr == ADDR_PAIR ? fwd_kernel_for<ADDR_PAIR>(nkb)
+      : addr == ADDR_VARLEN_PAIR ? fwd_kernel_for<ADDR_VARLEN_PAIR>(nkb)
+      : addr == ADDR_VARLEN_PACKED ? fwd_kernel_for<ADDR_VARLEN_PACKED>(nkb) : fwd_kernel_for<ADDR_DENSE>(nkb);
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "attention_fwd smem attribute: %s", cudaGetErrorString(e));
   // warps per CTA: one per 16-row task up to 3, else two tasks per warp — smaller CTAs, more of them resident per SM, so
@@ -630,7 +645,7 @@ int attention_fwd_launch(const AttnParams& p, bool pair, const PairSrc& pb, cuda
     }
     if (cap > 0 && fwd_warps > cap) fwd_warps = cap;
   }
-  launch_kernel(kern, dim3(p.n_seq * p.heads), dim3(fwd_warps * 32), smem, stream, p, pb);
+  launch_kernel(kern, dim3(p.n_seq * p.heads), dim3(fwd_warps * 32), smem, stream, p, pb, vl);
   UNIVL_CHECK_LAUNCH("attention_fwd");
   return UNIVL_OK;
 }
@@ -654,7 +669,7 @@ extern "C" int univl_attention_fwd(const void* q, long long ldq, const void* k, 
   UNIVL_CHECK_ARG(o != nullptr && (ldo % 2) == 0, "attention_fwd: bad output");
   if (n_seq == 0) return UNIVL_OK;
   p.o = (bf16*)o; p.ldo = ldo; p.lse = lse;
-  return attention_fwd_launch(p, false, PairSrc{}, (cudaStream_t)stream);
+  return attention_fwd_launch(p, ADDR_DENSE, PairSrc{}, VarlenSrc{}, (cudaStream_t)stream);
 }
 
 extern "C" int univl_attention_bwd(const void* q, long long ldq, const void* k, long long ldk, const void* v,

@@ -44,6 +44,24 @@ struct PairSrc {
   long long ldq, ldk, ldv;
 };
 
+// Row addressing of the forward kernels' Q/K/V tiles, a compile-time variant:
+//   ADDR_DENSE          sequence s is rows [s * S, (s + 1) * S) of q/k/v (univl_attention_fwd)
+//   ADDR_PAIR           all-pairs concat(a_i, b_j) of two sources (load_pair_tile, univl_attention_pair_fwd)
+//   ADDR_VARLEN_PAIR    varlen sequences whose rows are picked from two sources by index lists (VarlenSrc)
+//   ADDR_VARLEN_PACKED  varlen sequences stored back to back (VarlenSrc)
+enum Addr : int { ADDR_DENSE = 0, ADDR_PAIR = 1, ADDR_VARLEN_PAIR = 2, ADDR_VARLEN_PACKED = 3 };
+
+// The varlen forward's sequences (univl_attention_varlen_fwd, univl_gather_rows_varlen).  Sequence p has
+// Sk_p = cu[p + 1] - cu[p] rows, every one of them a real key (no mask).  Pair addressing (idx_a != null): row r < len_a[p]
+// is row idx_a[start_a[p] + r] of source a, row r >= len_a[p] is row idx_b[start_b[p] + r - len_a[p]] of source b.
+// Packed addressing: row r is row cu[p] + r of source a.  q_first: one query per sequence, its row 0 (under packed
+// addressing the query rows are instead row p of q), and output row p; otherwise all Sk_p rows query, output at cu[p].
+struct VarlenSrc {
+  const int* cu;  // [n_seq + 1]
+  const int *idx_a, *idx_b, *start_a, *start_b, *len_a;
+  int q_first;
+};
+
 __device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
                : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
@@ -88,6 +106,44 @@ __device__ __forceinline__ void load_pair_tile(bf16* dst, const bf16* a, long lo
     if (r < rows) cp_async16(d, (s < p.Wa ? ra + (long long)s * lda : rb + (long long)(s - p.Wa) * ldb) + c * 8);
     else *reinterpret_cast<uint4*>(d) = make_uint4(0, 0, 0, 0);
   }
+}
+
+// column 0 of row r of varlen sequence p (VarlenSrc); a / b point at column 0 of each source
+__device__ __forceinline__ const bf16* varlen_row(const VarlenSrc& vl, const bf16* a, long long lda, const bf16* b,
+                                                  long long ldb, int p, int r) {
+  if (vl.idx_a == nullptr) return a + (long long)(vl.cu[p] + r) * lda;
+  const int la = vl.len_a[p];
+  return r < la ? a + (long long)vl.idx_a[vl.start_a[p] + r] * lda : b + (long long)vl.idx_b[vl.start_b[p] + r - la] * ldb;
+}
+
+// load_head_tile for the varlen forward: rows [r0, r0 + rows) of varlen sequence `seq`, zero-filling rows >= rows
+__device__ __forceinline__ void load_varlen_tile(bf16* dst, const bf16* a, long long lda, const bf16* b, long long ldb,
+                                                 const VarlenSrc& vl, int seq, int h, int r0, int rows, int rows16) {
+  for (int idx = threadIdx.x; idx < rows16 * 8; idx += blockDim.x) {
+    const int r = idx >> 3, c = idx & 7;
+    bf16* d = dst + r * LDS + c * 8;
+    if (r < rows) cp_async16(d, varlen_row(vl, a, lda, b, ldb, seq, r0 + r) + h * HD + c * 8);
+    else *reinterpret_cast<uint4*>(d) = make_uint4(0, 0, 0, 0);
+  }
+}
+
+// the query rows [r0, r0 + rows) of varlen sequence `seq`: as its keys, except packed token-0 queries (row seq of q)
+__device__ __forceinline__ void load_varlen_q(bf16* dst, const bf16* a, long long lda, const bf16* b, long long ldb,
+                                              const VarlenSrc& vl, int seq, int h, int r0, int rows, int rows16) {
+  if (vl.q_first && vl.idx_a == nullptr) load_head_tile(dst, a + (long long)seq * lda + h * HD, lda, rows, rows16);
+  else load_varlen_tile(dst, a, lda, b, ldb, vl, seq, h, r0, rows, rows16);
+}
+
+// this CTA's varlen sequence `seq` into p's Sk / Sq
+__device__ __forceinline__ void varlen_shape(AttnParams& p, const VarlenSrc& vl, int seq) {
+  p.Sk = vl.cu[seq + 1] - vl.cu[seq];
+  p.Sq = vl.q_first ? 1 : p.Sk;
+}
+
+// output row of query 0 of varlen sequence `seq` (its lse rows: row * heads + h).  Looked up where the output is stored
+// rather than kept live through the kernel.
+__device__ __forceinline__ long long varlen_out_row(const VarlenSrc& vl, int seq) {
+  return vl.q_first ? seq : vl.cu[seq];
 }
 
 // additive key mask for this sequence into smem: 0 / -10000 for real keys, -inf for padding beyond Sk
@@ -203,10 +259,13 @@ static inline int fill_common(AttnParams& p, const void* q, long long ldq, const
   return UNIVL_OK;
 }
 
-// Launch the forward kernels for a filled AttnParams (o, lse and the shape set, n_seq > 0).  pair: read Q/K/V through
-// load_pair_tile from p's q/k/v and pb (univl_attention_pair_fwd); pb is ignored otherwise.
+// Launch the forward kernels for a filled AttnParams (o, lse and the shape set, n_seq > 0).  addr: the row addressing
+// (Addr); pb is the second source of ADDR_PAIR and ADDR_VARLEN_PAIR, vl the sequences of the varlen addressings, each
+// ignored otherwise.  Under the varlen addressings p.Sq / p.Sk are the longest sequence's, which size the launch, and
+// the output / lse rows are VarlenSrc's (lse[row * heads + h]).
 // attention.cu: Sq, Sk <= 256; attention_long.cu: Sq, Sk <= 1024 and 12 heads.
-int attention_fwd_launch(const AttnParams& p, bool pair, const PairSrc& pb, cudaStream_t stream);
-int attention_long_fwd_launch(const AttnParams& p, bool pair, const PairSrc& pb, cudaStream_t stream);
+int attention_fwd_launch(const AttnParams& p, Addr addr, const PairSrc& pb, const VarlenSrc& vl, cudaStream_t stream);
+int attention_long_fwd_launch(const AttnParams& p, Addr addr, const PairSrc& pb, const VarlenSrc& vl,
+                              cudaStream_t stream);
 
 }  // namespace univl

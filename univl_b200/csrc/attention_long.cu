@@ -69,25 +69,31 @@ __device__ __forceinline__ void write_partial_row(const float* slots, int nwarps
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// forward (PAIR: the Q/K/V rows come from two sources through load_pair_tile, univl_attention_pair_fwd; a key tile
-// may straddle the boundary between them)
+// forward (ADDR: the row addressing of Q/K/V, attention_common.cuh Addr; under ADDR_PAIR and ADDR_VARLEN_PAIR a key tile
+// may straddle the boundary between the two sources.  Under the varlen addressings each CTA takes its own sequence's
+// Sq / Sk, the query blocks past its Sq exit at once, and output / lse go to VarlenSrc's rows.)
 // ------------------------------------------------------------------------------------------------------------
-template <bool PAIR>
+template <int ADDR>
 __global__ void __launch_bounds__(LONG_WARPS * 32)
-attention_long_fwd_kernel(const AttnParams p_in, const PairSrc pb) {
+attention_long_fwd_kernel(const AttnParams p_in, const PairSrc pb, const VarlenSrc vl) {
   pdl_trigger();
   pdl_wait();
   AttnParams p = p_in;
   resolve_rng(p);
+  constexpr bool VARLEN = ADDR == ADDR_VARLEN_PAIR || ADDR == ADDR_VARLEN_PACKED;
+  const int seq = blockIdx.x / p.heads, h = blockIdx.x % p.heads;
+  const long long bh = blockIdx.x;
+  const int qbase = blockIdx.y * LB;
+  if constexpr (VARLEN) {
+    varlen_shape(p, vl, seq);
+    if (p.Sk <= 0 || qbase >= p.Sq) return;  // the whole CTA leaves before any barrier
+  }
   extern __shared__ __align__(16) uint8_t smem_att[];
   const int Sq16 = (p.Sq + 15) & ~15, Sk16 = (p.Sk + 15) & ~15;
   bf16* sQ = reinterpret_cast<bf16*>(smem_att);                 // [LB][LDS]
   bf16* sKV = sQ + LB * LDS;                                    // stage s: K at s * 2 * LT rows, V after it
   float* madd = reinterpret_cast<float*>(sKV + 4 * LT * LDS);  // [Sk16]
 
-  const int seq = blockIdx.x / p.heads, h = blockIdx.x % p.heads;
-  const long long bh = blockIdx.x;
-  const int qbase = blockIdx.y * LB;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
   const int qrows = min(LB, p.Sq - qbase), qrows16 = min(LB, Sq16 - qbase);
@@ -96,7 +102,10 @@ attention_long_fwd_kernel(const AttnParams p_in, const PairSrc pb) {
   auto load_kv = [&](int tile, int stage) {
     const int k0 = tile * LT;
     bf16* sK = sKV + stage * 2 * LT * LDS;
-    if constexpr (PAIR) {
+    if constexpr (VARLEN) {
+      load_varlen_tile(sK, p.k, p.ldk, pb.k, pb.ldk, vl, seq, h, k0, min(LT, p.Sk - k0), LT);
+      load_varlen_tile(sK + LT * LDS, p.v, p.ldv, pb.v, pb.ldv, vl, seq, h, k0, min(LT, p.Sk - k0), LT);
+    } else if constexpr (ADDR == ADDR_PAIR) {
       load_pair_tile(sK, p.k, p.ldk, pb.k, pb.ldk, p, seq, h, k0, min(LT, p.Sk - k0), LT);
       load_pair_tile(sK + LT * LDS, p.v, p.ldv, pb.v, pb.ldv, p, seq, h, k0, min(LT, p.Sk - k0), LT);
     } else {
@@ -104,7 +113,8 @@ attention_long_fwd_kernel(const AttnParams p_in, const PairSrc pb) {
       load_head_tile(sK + LT * LDS, p.v + ((long long)seq * p.Sk + k0) * p.ldv + h * HD, p.ldv, min(LT, p.Sk - k0), LT);
     }
   };
-  if constexpr (PAIR) load_pair_tile(sQ, p.q, p.ldq, pb.q, pb.ldq, p, seq, h, qbase, qrows, qrows16);
+  if constexpr (VARLEN) load_varlen_q(sQ, p.q, p.ldq, pb.q, pb.ldq, vl, seq, h, qbase, qrows, qrows16);
+  else if constexpr (ADDR == ADDR_PAIR) load_pair_tile(sQ, p.q, p.ldq, pb.q, pb.ldq, p, seq, h, qbase, qrows, qrows16);
   else load_head_tile(sQ, p.q + ((long long)seq * p.Sq + qbase) * p.ldq + h * HD, p.ldq, qrows, qrows16);
   build_key_mask(madd, p, seq, Sk16);
   load_kv(0, 0);
@@ -216,10 +226,12 @@ attention_long_fwd_kernel(const AttnParams p_in, const PairSrc pb) {
     o[nb][2] *= r1;
     o[nb][3] *= r1;
   }
-  store_rows(p.o + ((long long)seq * p.Sq + qbase) * p.ldo + h * HD, p.ldo, warp * 16, qrows, lane, o);
+  const long long obase = VARLEN ? varlen_out_row(vl, seq) : (long long)seq * p.Sq;  // output row of query 0
+  store_rows(p.o + (obase + qbase) * p.ldo + h * HD, p.ldo, warp * 16, qrows, lane, o);
   if (t == 0 && p.lse != nullptr) {
-    if (i0 < p.Sq) p.lse[bh * p.Sq + i0] = m0 + __logf(l0);
-    if (i1 < p.Sq) p.lse[bh * p.Sq + i1] = m1 + __logf(l1);
+    // lse: [n_seq, heads, Sq], or [rows, heads] under the varlen addressings
+    if (i0 < p.Sq) p.lse[VARLEN ? (obase + i0) * p.heads + h : bh * p.Sq + i0] = m0 + __logf(l0);
+    if (i1 < p.Sq) p.lse[VARLEN ? (obase + i1) * p.heads + h : bh * p.Sq + i1] = m1 + __logf(l1);
   }
 }
 
@@ -511,15 +523,18 @@ attention_long_bwd_dkdv_kernel(const AttnParams p_in, const float* __restrict__ 
   }
 }
 
-int attention_long_fwd_launch(const AttnParams& p, bool pair, const PairSrc& pb, cudaStream_t stream) {
+int attention_long_fwd_launch(const AttnParams& p, Addr addr, const PairSrc& pb, const VarlenSrc& vl,
+                              cudaStream_t stream) {
   const int Sq16 = (p.Sq + 15) & ~15, Sk16 = (p.Sk + 15) & ~15;
   const size_t smem = (size_t)(LB + 4 * LT) * LDS * 2 + (size_t)Sk16 * 4;
-  void (*kern)(const AttnParams, const PairSrc) =
-      pair ? attention_long_fwd_kernel<true> : attention_long_fwd_kernel<false>;
+  void (*kern)(const AttnParams, const PairSrc, const VarlenSrc) =
+      addr == ADDR_PAIR ? attention_long_fwd_kernel<ADDR_PAIR>
+      : addr == ADDR_VARLEN_PAIR ? attention_long_fwd_kernel<ADDR_VARLEN_PAIR>
+      : addr == ADDR_VARLEN_PACKED ? attention_long_fwd_kernel<ADDR_VARLEN_PACKED> : attention_long_fwd_kernel<ADDR_DENSE>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "attention_long_fwd smem attribute: %s", cudaGetErrorString(e));
   const int warps = Sq16 / 16 < LONG_WARPS ? Sq16 / 16 : LONG_WARPS;
-  launch_kernel(kern, dim3(p.n_seq * p.heads, (Sq16 + LB - 1) / LB), dim3(warps * 32), smem, stream, p, pb);
+  launch_kernel(kern, dim3(p.n_seq * p.heads, (Sq16 + LB - 1) / LB), dim3(warps * 32), smem, stream, p, pb, vl);
   UNIVL_CHECK_LAUNCH("attention_long_fwd");
   return UNIVL_OK;
 }
@@ -542,7 +557,7 @@ extern "C" int univl_attention_long_fwd(const void* q, long long ldq, const void
   UNIVL_CHECK_ARG(o != nullptr && (ldo % 2) == 0, "attention_long_fwd: bad output");
   if (n_seq == 0) return UNIVL_OK;
   p.o = (bf16*)o; p.ldo = ldo; p.lse = lse;
-  return attention_long_fwd_launch(p, false, PairSrc{}, (cudaStream_t)stream);
+  return attention_long_fwd_launch(p, ADDR_DENSE, PairSrc{}, VarlenSrc{}, (cudaStream_t)stream);
 }
 
 // As univl_attention_bwd, for 0 < Sq, Sk <= 1024, 12 heads and rng_layout 0 (the forward was univl_attention_long_fwd

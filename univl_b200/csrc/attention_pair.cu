@@ -42,6 +42,6 @@ extern "C" int univl_attention_pair_fwd(const void* qa, long long ldqa, const vo
   if (n_seq == 0) return UNIVL_OK;
   const PairSrc pb{(const bf16*)qb, (const bf16*)kb, (const bf16*)vb, ldqb, ldkb, ldvb};
   p.o = (bf16*)o; p.ldo = ldo; p.lse = lse;
-  if (S <= 256) return attention_fwd_launch(p, true, pb, (cudaStream_t)stream);
-  return attention_long_fwd_launch(p, true, pb, (cudaStream_t)stream);
+  if (S <= 256) return attention_fwd_launch(p, ADDR_PAIR, pb, VarlenSrc{}, (cudaStream_t)stream);
+  return attention_long_fwd_launch(p, ADDR_PAIR, pb, VarlenSrc{}, (cudaStream_t)stream);
 }

@@ -10,6 +10,7 @@ import logging
 import math
 import os
 
+import numpy as np
 import torch
 from torch import nn
 
@@ -39,6 +40,20 @@ def eval_precision():
     value = os.environ.get("UNIVL_EVAL_PRECISION", "bf16")
     if value not in EVAL_PRECISIONS:
         raise ValueError("UNIVL_EVAL_PRECISION must be one of %s, got %r" % ("/".join(EVAL_PRECISIONS), value))
+    return value
+
+
+EVAL_LAYOUTS = ("padded", "packed")
+
+
+def eval_layout():
+    """UNIVL_EVAL_LAYOUT, read on every tiled evaluation call: "padded" (default) computes every pair at W + F tokens;
+    "packed" computes pair (i, j) on text i's and video j's valid tokens alone (CrossModel.
+    encode_pairs_first_token_eval_packed), under either UNIVL_EVAL_PRECISION.  Training, calls with gradients and
+    micro-batched calls never read it."""
+    value = os.environ.get("UNIVL_EVAL_LAYOUT", "padded")
+    if value not in EVAL_LAYOUTS:
+        raise ValueError("UNIVL_EVAL_LAYOUT must be one of %s, got %r" % ("/".join(EVAL_LAYOUTS), value))
     return value
 
 
@@ -124,6 +139,33 @@ def _eval_tile(Nt, Nv, S, budget):
     bv = min(Nv, max(1, math.isqrt(pairs)))
     bt = min(Nt, max(1, pairs // bv))
     return bt, min(Nv, max(1, pairs // bt))
+
+
+def _packed_eval_tiles(len_t, len_v, budget):
+    """Tiles (t0, t1, v0, v1) of the packed eval similarity, each at most `budget` packed pair tokens (at least one
+    pair).  len_t / len_v: valid tokens of every text / video row.  Video blocks have _eval_tile's width at the mean
+    pair length, capped so that one text row against a whole block fits; each block's text rows are then cut greedily,
+    a tile of text rows [t0, t1) costing (v1 - v0) * sum(len_t[t0:t1]) + (t1 - t0) * sum(len_v[v0:v1]) tokens."""
+    lt = np.asarray(len_t, dtype=np.int64)
+    lv = np.asarray(len_v, dtype=np.int64)
+    Nt, Nv = lt.size, lv.size
+    if Nt == 0 or Nv == 0:
+        return []
+    mean = max(1, math.ceil(lt.mean() + lv.mean()))
+    longest = max(1, int(lt.max() + lv.max()))
+    bv = max(1, min(_eval_tile(Nt, Nv, mean, budget)[1], budget // longest))
+    ct = np.concatenate([[0], np.cumsum(lt)])
+    tiles = []
+    for v0 in range(0, Nv, bv):
+        v1 = min(Nv, v0 + bv)
+        cost = (v1 - v0) * ct + int(lv[v0:v1].sum()) * np.arange(Nt + 1)  # tokens of text rows [0, t)
+        t0 = 0
+        while t0 < Nt:
+            t1 = int(np.searchsorted(cost, cost[t0] + budget, side="right")) - 1
+            t1 = min(Nt, max(t0 + 1, t1))
+            tiles.append((t0, t1, v0, v1))
+            t0 = t1
+    return tiles
 
 
 class UniVL(UniVLPreTrainedModel):
@@ -246,11 +288,18 @@ class UniVL(UniVLPreTrainedModel):
         projections of a pair's token depend on its text or video row alone, so they are computed once per source row
         (CrossModel.first_layer_source_qkv) and every tile reads them in place.  Every other stage is row- or
         sequence-local, so a pair's logit does not depend on the tiling.  UNIVL_EVAL_PRECISION=fp8 (eval_precision)
-        runs the cross layers' dense GEMMs over the pair tokens in FP8, with weights quantized once per call."""
+        runs the cross layers' dense GEMMs over the pair tokens in FP8, with weights quantized once per call.
+        UNIVL_EVAL_LAYOUT=packed (eval_layout) scores the pairs on their valid tokens alone
+        (_cross_similarity_eval_packed).  Token 0 is the one the pooler reads, and it must be a real key of every pair:
+        a packed call with any text row whose attention_mask[i, 0] == 0 takes the padded path as a whole."""
         Nt, W = attention_mask.shape
         Nv, F = video_mask.shape
         fp8 = eval_precision() == "fp8" and len(self.cross.encoder.layer) > 1
         qw = self.cross.fp8_eval_weights() if fp8 else None
+        if eval_layout() == "packed":
+            packing = ops.PairPacking(attention_mask, video_mask)
+            if packing.token0_valid:
+                return self._cross_similarity_eval_packed(seq2d, vis2d, packing, qw)
         qkv = self.cross.first_layer_source_qkv(seq2d, vis2d, Nt, W, Nv, F)
         qkv_t, qkv_v = qkv[:Nt * W], qkv[Nt * W:]
         logits = torch.empty((Nt, Nv), dtype=torch.float32, device=seq2d.device)
@@ -268,6 +317,24 @@ class UniVL(UniVLPreTrainedModel):
                 u = self.cross.pooler.pre_activation(first, (t1 - t0) * (v1 - v0), 1)
                 tile = ops.PoolerSimFn.apply(u, self.similarity_dense.weight, self.similarity_dense.bias)
                 logits[t0:t1, v0:v1] = tile.view(t1 - t0, v1 - v0)
+        return logits
+
+    def _cross_similarity_eval_packed(self, seq2d, vis2d, packing, qw):
+        """_cross_similarity_eval on the packed layout: pair (i, j) is computed on text i's and video j's valid tokens
+        alone, each at its original position.  A padded key adds -10000 to its score, so next to a real key its
+        exp(s - max) is exactly 0 in fp32, and every other stage acts on each row alone: a real row's result does not
+        depend on the padded rows, and the logits equal the padded path's up to the order of the fp32 sums inside
+        attention.  Tiles hold at most EVAL_PAIR_TOKENS packed tokens (_packed_eval_tiles); a pair's logit does not
+        depend on the tiling.  packing: the call's ops.PairPacking; qw: fp8_eval_weights() or None (bf16)."""
+        (Nt, W), (Nv, F) = packing.text_shape, packing.video_shape
+        x, qkv = self.cross.first_layer_source_rows(seq2d, vis2d, Nt, W, Nv, F)
+        logits = torch.empty((Nt, Nv), dtype=torch.float32, device=seq2d.device)
+        for t0, t1, v0, v1 in _packed_eval_tiles(packing.len_t, packing.len_v, EVAL_PAIR_TOKENS):
+            seqs = packing.tile(t0, t1, v0, v1)
+            first = self.cross.encode_pairs_first_token_eval_packed(x, qkv, Nt * W, seqs, qw)
+            u = self.cross.pooler.pre_activation(first, seqs.n_seq, 1)
+            tile = ops.PoolerSimFn.apply(u, self.similarity_dense.weight, self.similarity_dense.bias)
+            logits[t0:t1, v0:v1] = tile.view(t1 - t0, v1 - v0)
         return logits
 
     def _mean_pool_similarity(self, seq2d, vis2d, attention_mask, video_mask, groups=1):

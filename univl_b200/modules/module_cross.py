@@ -98,6 +98,11 @@ class CrossModel(PreTrainedModel):
         row -> [Nt*W + Nv*F, 3H], text rows first.  With dropout off, a pair's first-layer input row is the embedding
         LayerNorm of its text or video row alone (position and type rows are the same for every pair), so these are
         the projections every pair sequence would compute for itself."""
+        return self.first_layer_source_rows(text2d, video2d, Nt, W, Nv, F)[1]
+
+    def first_layer_source_rows(self, text2d, video2d, Nt, W, Nv, F):
+        """first_layer_source_qkv and the embedding-LayerNorm rows it projects, the first layer's residual input
+        -> (x [Nt*W + Nv*F, H], qkv [Nt*W + Nv*F, 3H]), text rows first"""
         emb = self.embeddings
         pos, typ = emb.position_embeddings.weight, emb.token_type_embeddings.weight
         gamma, beta = emb.LayerNorm.weight, emb.LayerNorm.bias
@@ -107,7 +112,7 @@ class CrossModel(PreTrainedModel):
         ops.embed_src_rows_eval(video2d, Nv, F, pos[W:], typ[1:], gamma, beta, x[rows_t:])  # video rows: s >= W, type 1
         a = self.encoder.layer[0].attention.self
         wqkv = rt.current().bf16_qkv(a.query.weight, a.key.weight, a.value.weight)
-        return ops.linear_fwd(x, wqkv, rt.packed_bias(a.query.bias, a.key.bias, a.value.bias))
+        return x, ops.linear_fwd(x, wqkv, rt.packed_bias(a.query.bias, a.key.bias, a.value.bias))
 
     def encode_pairs_first_token_eval(self, text2d, video2d, text_mask, video_mask, qkv_t, qkv_v):
         """encode_pairs_first_token over all Nt x Nv pairs in evaluation, with the first layer's Q/K/V projections read
@@ -148,6 +153,19 @@ class CrossModel(PreTrainedModel):
         for i in range(1, len(layers) - 1):
             x = ops.encoder_layer_eval_fp8(x, n_seq, S, mask, _layer_params(layers[i]), qw[i])
         return ops.cls_layer_eval_fp8(x, n_seq, S, mask, _layer_params(layers[-1]), qw[-1])
+
+    def encode_pairs_first_token_eval_packed(self, x, qkv, rows_t, seqs, qw=None):
+        """encode_pairs_first_token_eval (qw None) or _fp8 (qw = fp8_eval_weights()) on the packed layout: every pair
+        of one tile on its valid tokens alone.  x, qkv: first_layer_source_rows of the call, whose first rows_t rows are
+        the text rows; seqs: the tile's ops.VarlenSeqs (PairPacking.tile) -> [seqs.n_seq, H]"""
+        layers = self.encoder.layer
+        h = ops.pair_layer_eval_packed(x[:rows_t], x[rows_t:], qkv[:rows_t], qkv[rows_t:], seqs,
+                                       _layer_params(layers[0]), len(layers) == 1, qw[0] if qw else None)
+        if len(layers) == 1:
+            return h
+        for i in range(1, len(layers) - 1):
+            h = ops.encoder_layer_eval_packed(h, seqs, _layer_params(layers[i]), qw[i] if qw else None)
+        return ops.cls_layer_eval_packed(h, seqs, _layer_params(layers[-1]), qw[-1] if qw else None)
 
     def forward(self, concat_input, concat_type=None, attention_mask=None, output_all_encoded_layers=True):
         """API-parity entry: `concat_type` must be the reference's layout (0s for the text part then 1s)."""

@@ -400,6 +400,192 @@ def cls_layer_eval_fp8(x, n_seq, S, mask, params, qw):
 
 
 # ---------------------------------------------------------------------------------------------------------
+# packed evaluation: the pair sequences on their valid tokens alone (include/univl_b200.h univl_attention_varlen_fwd)
+# ---------------------------------------------------------------------------------------------------------
+I32 = torch.int32
+
+
+def _exclusive_cumsum(n):
+    out = torch.zeros(n.numel() + 1, dtype=torch.int64, device=n.device)
+    torch.cumsum(n, 0, out=out[1:])
+    return out
+
+
+class VarlenSeqs:
+    """Variable-length sequences of univl_attention_varlen_fwd / univl_gather_rows_varlen: cu int32 [n_seq + 1] (sequence
+    p is rows [cu[p], cu[p + 1]) of the packed layout), `total` = cu[-1] and `max_sk` (host ints, max_sk >= every
+    sequence's length); under pair addressing also the int32 index lists idx_a / idx_b and the per-sequence start_a /
+    start_b / len_a (all None: packed addressing)."""
+
+    def __init__(self, cu, total, max_sk, idx_a=None, idx_b=None, start_a=None, start_b=None, len_a=None):
+        self.cu, self.total, self.max_sk = cu, int(total), int(max_sk)
+        self.idx_a, self.idx_b, self.start_a, self.start_b, self.len_a = idx_a, idx_b, start_a, start_b, len_a
+        self.n_seq = cu.numel() - 1
+
+    def packed(self):
+        """the same sequences under packed addressing: their rows stored back to back"""
+        return VarlenSeqs(self.cu, self.total, self.max_sk)
+
+    def index_args(self):
+        return (ptr(self.idx_a), ptr(self.idx_b), ptr(self.start_a), ptr(self.start_b), ptr(self.len_a),
+                self.cu.data_ptr())
+
+
+def _valid_rows(m, n):
+    """int32 indices of the n nonzero entries of the flat bool m, ascending, with no device-to-host sync (unlike
+    nonzero(), which must learn n first): entry k goes to slot cumsum(m)[k] - 1, the others to a spare slot n"""
+    flat = m.reshape(-1)
+    slot = torch.where(flat, torch.cumsum(flat, 0) - 1, n)
+    out = torch.empty(n + 1, dtype=I32, device=m.device)
+    out.scatter_(0, slot, torch.arange(flat.numel(), dtype=I32, device=m.device))
+    return out[:n]
+
+
+class PairPacking:
+    """The packed layout of the (text i, video j) pair sequences of one evaluation call: pair (i, j) is text i's valid
+    tokens then video j's, each at its original row (so its original position), and nothing else.  Built from the int64
+    masks text_mask [Nt, W] and video_mask [Nv, F] with torch ops on their device and one device-to-host copy: the
+    per-row counts (len_t / len_v below), which choose the tiles, and the token-0 flag.
+      token0_valid    every text row's token 0 is valid (the packed layout needs it: the pooler reads token 0)
+      idx_t / idx_v   int32: the valid rows i * W + s of the text source and j * F + s of the video source, ascending
+      start_t / start_v  int32 [Nt] / [Nv]: where row i's (j's) entries begin in idx_t (idx_v)
+      len_t / len_v   host lists of the valid-token counts
+      max_sk          longest pair of the call (max len_t + max len_v).  Every tile passes this one value, so which
+                      attention kernel a pair runs on does not depend on the tiling."""
+
+    def __init__(self, text_mask, video_mask):
+        tm, vm = text_mask != 0, video_mask != 0
+        self.text_shape, self.video_shape = tuple(tm.shape), tuple(vm.shape)
+        nt, nv = tm.sum(1), vm.sum(1)
+        token0 = tm[:, 0].all().view(1) if tm.shape[1] else torch.zeros(1, dtype=torch.bool, device=tm.device)
+        host = torch.cat([nt, nv, token0.long()]).cpu().tolist()  # the one device-to-host copy
+        Nt = tm.shape[0]
+        self.len_t, self.len_v = host[:Nt], host[Nt:-1]
+        self.token0_valid = bool(host[-1])
+        self.idx_t = _valid_rows(tm, sum(self.len_t))
+        self.idx_v = _valid_rows(vm, sum(self.len_v))
+        self.start_t = _exclusive_cumsum(nt)[:-1].to(I32)
+        self.start_v = _exclusive_cumsum(nv)[:-1].to(I32)
+        self.n_t, self.n_v = nt.to(I32), nv.to(I32)
+        self.max_sk = max(self.len_t, default=0) + max(self.len_v, default=0)
+
+    def tokens(self, t0, t1, v0, v1):
+        """packed rows of the tile of text rows [t0, t1) x video rows [v0, v1)"""
+        return (v1 - v0) * sum(self.len_t[t0:t1]) + (t1 - t0) * sum(self.len_v[v0:v1])
+
+    def tile(self, t0, t1, v0, v1):
+        """VarlenSeqs (pair addressing) of the pairs p = (i - t0) * (v1 - v0) + (j - v0) of that tile"""
+        nt, nv = t1 - t0, v1 - v0
+        len_a = self.n_t[t0:t1].repeat_interleave(nv)
+        len_b = self.n_v[v0:v1].repeat(nt)
+        cu = _exclusive_cumsum(len_a.long() + len_b.long()).to(I32)
+        return VarlenSeqs(cu, self.tokens(t0, t1, v0, v1), self.max_sk, self.idx_t, self.idx_v,
+                          self.start_t[t0:t1].repeat_interleave(nv), self.start_v[v0:v1].repeat(nt), len_a)
+
+
+def attention_varlen_fwd(q, k, v, seqs, q_first, qb=None, kb=None, vb=None):
+    """Attention core of the variable-length sequences `seqs` (csrc/attention_varlen.cu), no mask, no dropout.  q/k/v
+    (and qb/kb/vb, the second source under pair addressing): 2-D views whose columns [h*64, h*64+64) hold head h.
+    q_first: token 0 only (under packed addressing q holds one row per sequence) -> ctx [n_seq, H]; else
+    [seqs.total, H] in packed order"""
+    o = _empty((seqs.n_seq if q_first else seqs.total, HEADS * 64), BF16, q)
+    if o.shape[0] == 0:
+        return o
+    b = (qb, kb, vb) if seqs.idx_a is not None else (None, None, None)
+    call("univl_attention_varlen_fwd", q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0), v.data_ptr(),
+         v.stride(0), ptr(b[0]), b[0].stride(0) if b[0] is not None else 0, ptr(b[1]),
+         b[1].stride(0) if b[1] is not None else 0, ptr(b[2]), b[2].stride(0) if b[2] is not None else 0,
+         *seqs.index_args(), seqs.n_seq, seqs.max_sk, HEADS, int(q_first), o.data_ptr(), o.stride(0), None,
+         1.0 / math.sqrt(64.0))
+    return o
+
+
+def gather_rows_varlen(a, b, seqs, q_first):
+    """the rows of `seqs` (a, and b under pair addressing) in packed order -> [seqs.total, cols], or with q_first row 0
+    of every sequence -> [n_seq, cols]"""
+    _check2d(a, "gather_rows_varlen a")
+    out = _empty((seqs.n_seq if q_first else seqs.total, a.shape[1]), BF16, a)
+    if out.shape[0] == 0:
+        return out
+    call("univl_gather_rows_varlen", a.data_ptr(), a.stride(0), ptr(b), b.stride(0) if b is not None else 0,
+         *seqs.index_args(), seqs.n_seq, int(q_first), a.shape[1], out.data_ptr(), out.stride(0))
+    return out
+
+
+def _split_qkv(qkv):
+    H = qkv.shape[1] // 3
+    return qkv[:, :H], qkv[:, H:2 * H], qkv[:, 2 * H:]
+
+
+def _attn_out(ctx, x, params):
+    """LayerNorm(ctx Wo^T + bo + x): the attention block's output in evaluation, bf16 (as pair_layer_eval)"""
+    wa = dict(zip(ATT_KEYS, params[:10]))
+    drop = _Drop(0.0, 0.0, False)
+    ao = linear_fwd(ctx, rt.current().bf16(wa["o"]), wa["bo"])
+    return layernorm_fwd(ao, x, wa["gamma"], wa["beta"], 0.0, 1, drop.seed, drop.stream())[0]
+
+
+def _ffn(y, params):
+    return ffn_block_fwd(y, dict(zip(FFN_KEYS, params[10:16])), _Drop(0.0, 0.0, False))[0]
+
+
+# The packed layer functions below free the attention context (and the Q/K/V rows, and the gathered residual) before
+# the FFN, which keeps a packed tile's peak below a padded tile's of the same token count by more than the per-source
+# embedding rows the packed layout keeps for the whole call.
+def pair_layer_eval_packed(x_a, x_b, qkv_a, qkv_b, seqs, params, first_token, qw=None):
+    """pair_layer_eval on the packed layout: the first cross layer of the tile's pairs `seqs` (pair addressing), its
+    Q/K/V read by index from the per-source projections qkv_a / qkv_b and its residual rows gathered from the
+    per-source embedding rows x_a / x_b.  first_token: token 0 only -> [n_seq, H]; else [seqs.total, H].
+    qw: the FP8 weights "o", "w1", "w2" (pair_layer_eval_fp8), or None for bf16."""
+    xq = gather_rows_varlen(x_a, x_b, seqs, first_token)
+    ctx = attention_varlen_fwd(*_split_qkv(qkv_a), seqs, first_token, *_split_qkv(qkv_b))
+    if qw is not None:
+        return _fp8_layer_tail(ctx, xq, params, qw)
+    y = _attn_out(ctx, xq, params)
+    del ctx, xq
+    return _ffn(y, params)
+
+
+def encoder_layer_eval_packed(x, seqs, params, qw=None):
+    """a middle encoder layer in evaluation on the packed rows x [seqs.total, H]: QKV GEMM, varlen self-attention of
+    every sequence, tail.  qw: the FP8 weights "qkv", "o", "w1", "w2" (encoder_layer_eval_fp8), or None for bf16."""
+    wa = dict(zip(ATT_KEYS, params[:10]))
+    bias = rt.packed_bias(wa["bq"], wa["bk"], wa["bv"])
+    if qw is None:
+        qkv = linear_fwd(x, rt.current().bf16_qkv(wa["q"], wa["k"], wa["v"]), bias)
+    else:
+        qkv = gemm_fp8(*quantize_e4m3_rows(x), *qw["qkv"], bias)
+    ctx = attention_varlen_fwd(*_split_qkv(qkv), seqs.packed(), False)
+    del qkv
+    if qw is not None:
+        return _fp8_layer_tail(ctx, x, params, qw)
+    y = _attn_out(ctx, x, params)
+    del ctx
+    return _ffn(y, params)
+
+
+def cls_layer_eval_packed(x, seqs, params, qw=None):
+    """the last encoder layer in evaluation on the packed rows x [seqs.total, H], token 0 of every sequence only
+    (EncoderLayerClsFn / cls_layer_eval_fp8): K/V GEMM on every packed row (FP8 with qw's "kv"), the Q projection,
+    attention and tail on the n_seq token-0 rows, bf16 -> [n_seq, H]"""
+    arena = rt.current()
+    wa = dict(zip(ATT_KEYS, params[:10]))
+    H = x.shape[1]
+    wqkv = arena.bf16_qkv(wa["q"], wa["k"], wa["v"])
+    bias = rt.packed_bias(wa["bk"], wa["bv"])
+    if qw is None:
+        kv = linear_fwd(x, wqkv[H:], bias)
+    else:
+        kv = gemm_fp8(*quantize_e4m3_rows(x), *qw["kv"], bias)
+    packed = seqs.packed()
+    x0 = gather_rows_varlen(x, None, packed, True)
+    q = linear_fwd(x0, wqkv[:H], wa["bq"])
+    ctx = attention_varlen_fwd(q, kv[:, :H], kv[:, H:], packed, True)
+    del kv
+    return _ffn(_attn_out(ctx, x0, params), params)
+
+
+# ---------------------------------------------------------------------------------------------------------
 # transformer blocks (forward keeps a dict of saved tensors; backward consumes it)
 # ---------------------------------------------------------------------------------------------------------
 class _Drop:
