@@ -186,6 +186,17 @@ int univl_gather_rows_varlen(const void* a, long long lda, const void* b, long l
                              const int* idx_b, const int* start_a, const int* start_b, const int* len_a,
                              const int* cu_seqlens, int n_seq, int q_first, int cols, void* out, long long ldo,
                              void* stream);
+/* Forward only, no mask, no dropout: attention of n_q single-token queries over indexed key rows (one decoder token per
+ * hypothesis, module_decoder.py:225-245 at Sq = 1).  q bf16 [n_q, 768] (ldq), 12 heads of 64.  Keys come from ONE K|V
+ * buffer kv: row x holds k in columns [0, 768) and v in [768, 1536) (ldkv >= 1536).  Query r attends to the n_keys[c]
+ * rows key_rows[c * ld_rows + 0 .. n_keys[c] - 1] of kv, c = list_of_query[r] (list_of_query null: c = r); every
+ * listed row is a real key and no other row is read.  Lists hold 0 to 1024 keys; a query whose list is empty writes
+ * nothing.  Output o bf16 [n_q, 768] (ldo), lse (nullable) fp32 [n_q, 12].  fp32 accumulation; the key splits are
+ * merged in a fixed order (no floating-point atomics) and the launch does not depend on the SM count, so the bits
+ * depend on the inputs alone.  16-byte aligned q / kv with row strides multiples of 8. */
+int univl_attention_decode_fwd(const void* q, long long ldq, const void* kv, long long ldkv, const int* key_rows,
+                               long long ld_rows, const int* n_keys, const int* list_of_query, int n_q, int heads,
+                               void* o, long long ldo, float* lse, float scale, void* stream);
 /* ---- fused QKV projection + self-attention, forward (wgmma / TMA; module_bert.py:171-197 as ONE kernel) --------------
  * ctx[T,H] = merge_heads(dropout(softmax((x Wq^T + bq)(x Wk^T + bk)^T * scale + mask)) (x Wv^T + bv)), T = n_seq * S,
  * H = heads * 64 = 768.  wqkv: bf16 [3H, H] (query | key | value rows), bias fp32 [3H].  The [T,3H] projections and the

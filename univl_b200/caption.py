@@ -19,12 +19,27 @@ tolerance against it).  The beam bookkeeping restates `modules/beam.py` (Beam.ad
 previous beam scores except at the first step, top-k over beam x vocabulary, back-pointers, finished when the top
 hypothesis ends in [SEP]) in batched tensor form.
 """
+import os
+
 import torch
 
 from . import ops
 from . import runtime as rt
 
 BF16 = torch.bfloat16
+I32 = torch.int32
+
+DECODE_CACHE_MODES = ("off", "prefix")
+
+
+def decode_cache_mode():
+    """UNIVL_DECODE_CACHE, read on every `UniVL.decoder_caption` call: "off" (default) computes every call on its full
+    prefix; "prefix" serves the calls through the model's PrefixDecodeCache.  An environment variable, so that the
+    caption driver picks it up unchanged."""
+    value = os.environ.get("UNIVL_DECODE_CACHE", "off")
+    if value not in DECODE_CACHE_MODES:
+        raise ValueError("UNIVL_DECODE_CACHE must be one of %s, got %r" % ("/".join(DECODE_CACHE_MODES), value))
+    return value
 
 
 class CachedCaptionDecoder:
@@ -128,6 +143,289 @@ class CachedCaptionDecoder:
             logits = dec.classifier.cls.logits(x)
         self.t += 1
         return logits
+
+
+# Row fingerprints of PrefixDecodeCache: the bytes of a row as int16 times integer weights in [1, 2^16), summed in fp64.
+# Every partial sum is an integer below 2^53 when a row has fewer than 2^22 int16 words, so the sums are exact in any
+# order: equal rows always get equal fingerprints.  They only pick the candidate parent; equality is then checked bitwise.
+HASH_WEIGHT_BITS = 16
+HASH_MAX_WORDS = 1 << 22
+HASH_CHUNK_ELEMS = 1 << 22          # int16 words converted to fp64 at a time
+PLANES_MIN = 32                     # self-attention cache positions allocated at a fill; doubled as decoding goes on
+
+
+def _int16_rows(t, rows):
+    """the bytes of t [rows, ...] as int16 [rows, n] (1-byte types are widened: the values are what is compared)"""
+    t = t.contiguous().reshape(rows, -1)
+    if t.element_size() == 1:
+        return t.to(torch.int16)
+    return t.view(torch.int16)
+
+
+class _Call:
+    """one decoder_caption call's inputs, flattened: ids int64 [R, t], masks [R, W] / [R, F], and the int16 words of the
+    four encoder inputs (sequence_output, visual_output and both masks) per row"""
+
+    def __init__(self, seq, vis, am, vm, ids, dm, H):
+        self.R, self.t = ids.shape
+        self.W, self.F = am.shape[1], vm.shape[1]
+        self.seq, self.vis, self.am, self.vm, self.ids, self.dm = seq, vis, am, vm, ids, dm
+        self.words = [_int16_rows(x, self.R) for x in (seq, vis, am, vm)]
+        self.sig = (seq.dtype, vis.dtype, am.dtype, vm.dtype, self.W, self.F, H, seq.device)
+
+
+class _State:
+    pass
+
+
+class PrefixDecodeCache:
+    """Incremental evaluation of `UniVL.decoder_caption` for a caller that asks for the logits of a whole prefix once per
+    generated token, as the caption driver's beam search does (main_task_caption.py:434-517).
+
+    A decoder row's K/V and logits are a pure function of its encoder inputs and its prefix tokens, so the cache reuses
+    state only when both are bitwise equal to what it was computed from.  A call of prefix length t continues the
+    previous call (of length t - 1) when every row has a parent: a previous row with the same first t - 1 tokens and
+    bitwise-equal encoder inputs (the lowest such index; equal rows hold equal state).  Beam reordering and the removal
+    of finished instances are then just parent maps.  The continued call decodes one token per row: the row's
+    self-attention reads the K/V of its ancestors through an ancestry table of key rows (one plane of cache rows per
+    position, nothing is copied when beams reorder), its encoder attention reads the valid rows of its own cross-encoder
+    output, computed once at the fill, and the vocabulary projection runs on the new rows only.  Earlier positions'
+    logits come from a per-position history, gathered through the ancestry table.
+
+    Eligible calls: model.eval(), no gradients, every decoder_mask entry nonzero and t within the decoder's position
+    table.  Every other call computes the full path and leaves the cache alone.  An eligible call that does not continue
+    the previous one fills the cache: at t = 1 it decodes position 0 and returns that; at t > 1 it returns the full
+    path's result and refills by decoding the call's t positions.  A call in which any row has no valid encoder key
+    takes the full path, as does a fill of such rows.  The decision costs one device-to-host read per call.  The full
+    path gets decoder_mask as int64 (the caption driver passes uint8 ones, which the default path rejects).
+
+    The state lives on the model (PrefixDecodeCache.of), never in state_dict(), and is released by model.train()."""
+
+    def __init__(self, model):
+        self.model = model
+        self.state = None
+        self._weights = {}
+
+    @staticmethod
+    def of(model):
+        """the cache of this very module: a `parallel_apply` replica carries a copy of the original's __dict__"""
+        c = model.__dict__.get("_univl_decode_cache")
+        if c is None or c.model is not model:
+            c = PrefixDecodeCache(model)
+            model.__dict__["_univl_decode_cache"] = c
+        return c
+
+    @staticmethod
+    def release(model):
+        model.__dict__.pop("_univl_decode_cache", None)
+
+    # ------------------------------------------------------------------------------------------------------
+    def logits(self, sequence_output, visual_output, attention_mask, video_mask, input_caption_ids, decoder_mask,
+               shaped=False):
+        """`UniVL._get_decoder_score`'s logits fp32 [R, t, vocab], incrementally where the call allows it"""
+        model = self.model
+        # the default path takes int64 masks only; the caption driver builds its decoder mask as uint8 ones
+        full_mask = decoder_mask.long() if isinstance(decoder_mask, torch.Tensor) else decoder_mask
+
+        def full():
+            return model._get_decoder_score(sequence_output, visual_output, None, attention_mask, video_mask,
+                                            input_caption_ids, full_mask, shaped=shaped)[0]
+
+        x = self._call(sequence_output, visual_output, attention_mask, video_mask, input_caption_ids, decoder_mask,
+                       shaped)
+        if x is None:
+            return full()
+        st = self.state
+        cont = st is not None and st.sig == x.sig and x.t == st.t + 1 and x.R <= st.R0
+        dev = x.ids.device
+        with torch.no_grad():
+            mask_ok = (x.dm != 0).all()
+            enc_ok = torch.cat([x.am != 0, x.vm != 0], 1).any(1).all()
+            if cont:
+                parent, matched, hashes = self._match(x)
+            else:
+                matched = torch.zeros((), dtype=torch.bool, device=dev)
+            flag = int((mask_ok.long() | (enc_ok.long() << 1) | (matched.long() << 2)).item())  # the one read
+        if not flag & 1:
+            return full()
+        if flag & 4:
+            with torch.no_grad(), rt.use_model(model, dev):
+                st.hash_rows = hashes
+                self._advance(x.ids[:, -1], parent)
+                return self._gather(x.R)
+        self.state = None
+        if not flag & 2:
+            return full()
+        if x.t == 1:
+            with torch.no_grad(), rt.use_model(model, dev):
+                self._fill(x)
+                self._advance(x.ids[:, 0], None)
+                return self._gather(x.R)
+        out = full()
+        with torch.no_grad(), rt.use_model(model, dev):
+            self._fill(x)
+            for p in range(x.t):
+                self._advance(x.ids[:, p], None)
+        return out
+
+    # ------------------------------------------------------------------------------------------------------
+    def _call(self, seq, vis, am, vm, ids, dm, shaped):
+        """_Call of an eligible call's arguments (flattened as _get_decoder_score flattens them), else None"""
+        model = self.model
+        if model.training or torch.is_grad_enabled():
+            return None
+        if not all(isinstance(a, torch.Tensor) for a in (seq, vis, am, vm, ids, dm)):
+            return None
+        if shaped is False:
+            am, vm = am.reshape(-1, am.shape[-1]), vm.reshape(-1, vm.shape[-1])
+            ids, dm = ids.reshape(-1, ids.shape[-1]), dm.reshape(-1, dm.shape[-1])
+        dec = model.decoder
+        H = dec.embeddings.word_embeddings.weight.shape[1]
+        dev = dec.embeddings.word_embeddings.weight.device
+        if ids.dim() != 2 or am.dim() != 2 or vm.dim() != 2 or dm.shape != ids.shape or ids.dtype != torch.int64:
+            return None
+        R, t = ids.shape
+        if R == 0 or t == 0 or t > dec.embeddings.position_embeddings.weight.shape[0]:
+            return None
+        if am.shape[0] != R or vm.shape[0] != R or seq.numel() != R * am.shape[1] * H or \
+                vis.numel() != R * vm.shape[1] * H:
+            return None
+        if any(a.device != dev for a in (seq, vis, am, vm, ids, dm)):
+            return None
+        x = _Call(seq, vis, am, vm, ids.contiguous(), dm, H)
+        if any(w.shape[1] >= HASH_MAX_WORDS for w in x.words):
+            return None
+        return x
+
+    def _weight(self, i, n, device):
+        key = (i, n, device)
+        w = self._weights.get(key)
+        if w is None:
+            g = torch.Generator().manual_seed(0x5EED + i)
+            w = torch.randint(1, 1 << HASH_WEIGHT_BITS, (n, 2), generator=g, dtype=torch.int64).double().to(device)
+            self._weights[key] = w
+        return w
+
+    def _hash(self, words):
+        """fp64 [R, 2 * len(words)] exact fingerprints of int16 rows"""
+        cols = []
+        for i, a in enumerate(words):
+            R, n = a.shape
+            w = self._weight(i, n, a.device)
+            step = max(1, HASH_CHUNK_ELEMS // max(1, n))
+            cols.append(torch.cat([a[r:r + step].double() @ w for r in range(0, R, step)]))
+        return torch.cat(cols, 1)
+
+    def _match(self, x):
+        """-> (parent int64 [R], every row has a parent (device bool), fingerprints of the call's rows)"""
+        st = self.state
+        h = self._hash(x.words)
+        cand = (x.ids[:, None, :-1] == st.tokens[None]).all(2) & (h[:, None] == st.hash_rows[None]).all(2)
+        parent = cand.int().argmax(1)               # the lowest candidate (0 when none: `ok` is then False)
+        ok = cand.any(1)
+        fill_row = st.fill_of.long().index_select(0, parent)
+        for new, kept in zip(x.words, st.words):
+            ok = ok & (new == kept.index_select(0, fill_row)).all(1)
+        return parent, ok.all(), h
+
+    def _fill(self, x):
+        """encoder side of the call's rows: cross encoder once, every decoder layer's encoder K/V once, the valid key
+        lists; an empty self-attention cache"""
+        model = self.model
+        dec = model.decoder
+        H = x.sig[6]
+        arena = rt.current()
+        dev = x.ids.device
+        seq2d = x.seq.to(BF16).reshape(-1, H).contiguous()
+        vis2d = x.vis.to(BF16).reshape(-1, H).contiguous()
+        am, vm = x.am.contiguous(), x.vm.contiguous()
+        enc2d, _, Se = model._cross_pairs(seq2d, vis2d, am, vm, False)
+        st = _State()
+        st.sig, st.R0, st.t = x.sig, x.R, 0
+        st.enc_kv = []
+        for layer in dec.decoder.layer:
+            att = layer.enc_attn.att
+            wqkv = arena.bf16_qkv(att.query.weight, att.key.weight, att.value.weight)
+            st.enc_kv.append(ops.linear_fwd(enc2d, wqkv[H:], rt.packed_bias(att.key.bias, att.value.bias)))
+        del enc2d
+        # key list of row f: its valid encoder rows f * Se + s, ascending (cumsum + scatter, no nonzero())
+        valid = torch.cat([am != 0, vm != 0], 1)
+        slot = torch.where(valid, torch.cumsum(valid, 1) - 1, Se)
+        table = torch.zeros(x.R, Se + 1, dtype=I32, device=dev)
+        table.scatter_(1, slot, torch.arange(x.R * Se, dtype=I32, device=dev).view(x.R, Se))
+        st.enc_rows, st.enc_n = table[:, :Se], valid.sum(1).to(I32)
+        st.words = [w.clone() for w in x.words]
+        st.hash_rows = self._hash(st.words)
+        st.fill_of = torch.arange(x.R, dtype=I32, device=dev)
+        st.anc = torch.empty(x.R, 0, dtype=I32, device=dev)         # key row of every ancestor: p * R0 + its slot
+        st.slots = torch.empty(x.R, 0, dtype=torch.int64, device=dev)  # row of every ancestor in its step's history
+        st.tokens = torch.empty(x.R, 0, dtype=torch.int64, device=dev)
+        st.hist = []
+        cap = min(PLANES_MIN, dec.embeddings.position_embeddings.weight.shape[0])
+        st.planes = [torch.empty(cap, x.R, 2 * H, dtype=BF16, device=dev) for _ in dec.decoder.layer]
+        self.state = st
+
+    def _advance(self, tokens, parent):
+        """decode the token at position st.t of every row; parent int64 [R] (previous row of each row) or None (the
+        rows continue themselves)"""
+        st = self.state
+        dec = self.model.decoder
+        arena = rt.current()
+        H = st.sig[6]
+        R, p, dev = tokens.shape[0], st.t, tokens.device
+        if parent is not None:
+            st.anc, st.slots = st.anc.index_select(0, parent), st.slots.index_select(0, parent)
+            st.fill_of, st.tokens = st.fill_of.index_select(0, parent), st.tokens.index_select(0, parent)
+        here = torch.arange(R, device=dev)
+        st.anc = torch.cat([st.anc, (here + p * st.R0).to(I32)[:, None]], 1)
+        st.slots = torch.cat([st.slots, here[:, None]], 1)
+        st.tokens = torch.cat([st.tokens, tokens[:, None]], 1)
+        cap = st.planes[0].shape[0]
+        if p >= cap:
+            for li, old in enumerate(st.planes):
+                new = torch.empty(min(2 * cap, dec.embeddings.position_embeddings.weight.shape[0]), *old.shape[1:],
+                                  dtype=BF16, device=dev)
+                new[:cap] = old
+                st.planes[li] = new
+        emb = dec.embeddings
+        x = ops.EmbedTextFn.apply(tokens.reshape(R, 1).contiguous(), None, emb.word_embeddings.weight,
+                                  emb.position_embeddings.weight[p:], None, emb.LayerNorm.weight, emb.LayerNorm.bias,
+                                  0.0, False)
+        n_self = torch.full((R,), p + 1, dtype=I32, device=dev)
+        for li, layer in enumerate(dec.decoder.layer):
+            # ---- self-attention of the new token over its ancestors' cache rows ----
+            att, out = layer.slf_attn.att, layer.slf_attn.output
+            wqkv = arena.bf16_qkv(att.query.weight, att.key.weight, att.value.weight)
+            qkv = ops.linear_fwd(x, wqkv, rt.packed_bias(att.query.bias, att.key.bias, att.value.bias))
+            plane = st.planes[li]
+            plane[p, :R] = qkv[:, H:]
+            ctx = ops.attention_decode_fwd(qkv[:, :H], plane.view(-1, 2 * H), st.anc, n_self)
+            ao = ops.linear_fwd(ctx, arena.bf16(out.dense.weight), out.dense.bias)
+            x, _, _ = ops.layernorm_fwd(ao, x, out.LayerNorm.weight, out.LayerNorm.bias)
+            # ---- encoder attention over the valid rows of the row's own cross-encoder output ----
+            att, out = layer.enc_attn.att, layer.enc_attn.output
+            wqkv = arena.bf16_qkv(att.query.weight, att.key.weight, att.value.weight)
+            q = ops.linear_fwd(x, wqkv[:H], att.query.bias)
+            ctx = ops.attention_decode_fwd(q, st.enc_kv[li], st.enc_rows, st.enc_n, st.fill_of)
+            ao = ops.linear_fwd(ctx, arena.bf16(out.dense.weight), out.dense.bias)
+            x, _, _ = ops.layernorm_fwd(ao, x, out.LayerNorm.weight, out.LayerNorm.bias)
+            # ---- feed-forward ----
+            w1, w2 = arena.bf16(layer.intermediate.dense.weight), arena.bf16(layer.output.dense.weight)
+            pre = torch.empty(R, w1.shape[0], dtype=BF16, device=dev)
+            h = ops.linear_fwd(x, w1, layer.intermediate.dense.bias, epi=ops.EPI_GELU, aux_out=pre)
+            fo = ops.linear_fwd(h, w2, layer.output.dense.bias)
+            x, _, _ = ops.layernorm_fwd(fo, x, layer.output.LayerNorm.weight, layer.output.LayerNorm.bias)
+        st.hist.append(dec.classifier.cls.logits(x))
+        st.t += 1
+
+    def _gather(self, R):
+        """fp32 [R, t, vocab]: position p of row r is the logits its ancestor at position p was decoded with"""
+        st = self.state
+        V = st.hist[0].shape[1]
+        out = torch.empty((R, st.t, V), dtype=torch.float32, device=st.hist[0].device)
+        for p, h in enumerate(st.hist):
+            out[:, p] = h.index_select(0, st.slots[:, p])
+        return out
 
 
 @torch.no_grad()

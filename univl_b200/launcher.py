@@ -66,15 +66,21 @@ def install_numpy_aliases():
 
 def install_shadow(checkout):
     """`from modules.X import ...` resolves to univl_b200.modules.X for the hot-path modules and to the checkout's own
-    file for tokenization / beam."""
+    file for tokenization / beam.  Under UNIVL_DECODE_CACHE=prefix, `modules.beam` is univl_b200.modules.beam, whose
+    Beam keeps its hypotheses on the host."""
+    from .caption import decode_cache_mode
     checkout = os.path.abspath(checkout)
     if checkout not in sys.path:
         sys.path.insert(0, checkout)
     pkg = importlib.import_module("univl_b200.modules")
     sys.modules["modules"] = pkg
-    for name in _SHADOWED:
+    shadowed = _SHADOWED + (("beam",) if decode_cache_mode() == "prefix" else ())
+    for name in shadowed:
         sys.modules["modules." + name] = importlib.import_module("univl_b200.modules." + name)
     for name in ("tokenization", "beam"):
+        if name in shadowed:
+            setattr(pkg, name, sys.modules["modules." + name])
+            continue
         path = os.path.join(checkout, "modules", name + ".py")
         if not os.path.exists(path):
             continue

@@ -16,6 +16,7 @@ from torch import nn
 
 from .. import ops
 from .. import runtime as rt
+from ..caption import PrefixDecodeCache, decode_cache_mode
 from .module_bert import BertConfig, BertModel, BertOnlyMLMHead
 from .module_cross import CrossConfig, CrossModel
 from .module_decoder import DecoderConfig, DecoderModel
@@ -230,6 +231,12 @@ class UniVL(UniVLPreTrainedModel):
             self._pretrain_sim_loss_fct = margin
 
         self.apply(self.init_weights)
+
+    def train(self, mode=True):
+        """nn.Module.train; back in training mode the caption decoding cache (PrefixDecodeCache) is released"""
+        if mode:
+            PrefixDecodeCache.release(self)
+        return super(UniVL, self).train(mode)
 
     # ------------------------------------------------------------------------------------------------------
     # internals work on 2-D bf16 [rows, H] tensors plus the int64 masks
@@ -457,8 +464,14 @@ class UniVL(UniVLPreTrainedModel):
 
     def decoder_caption(self, sequence_output, visual_output, input_ids, attention_mask, video_mask,
                         input_caption_ids, decoder_mask, shaped=False, get_logits=False):
-        scores, _ = self._get_decoder_score(sequence_output, visual_output, input_ids, attention_mask, video_mask,
-                                            input_caption_ids, decoder_mask, shaped=shaped)
+        """UNIVL_DECODE_CACHE=prefix (caption.decode_cache_mode) serves the calls of a token-by-token decoding loop
+        incrementally through the model's caption.PrefixDecodeCache; the result is the same either way."""
+        if decode_cache_mode() == "prefix":
+            scores = PrefixDecodeCache.of(self).logits(sequence_output, visual_output, attention_mask, video_mask,
+                                                       input_caption_ids, decoder_mask, shaped=shaped)
+        else:
+            scores, _ = self._get_decoder_score(sequence_output, visual_output, input_ids, attention_mask, video_mask,
+                                                input_caption_ids, decoder_mask, shaped=shaped)
         if get_logits:
             return scores
         return torch.max(scores, -1)[1]

@@ -512,6 +512,23 @@ def gather_rows_varlen(a, b, seqs, q_first):
     return out
 
 
+def attention_decode_fwd(q, kv, key_rows, n_keys, list_of_query=None, out=None, lse=None):
+    """Single-token attention over indexed key rows (csrc/attention_decode.cu), no mask, no dropout.  q [n_q, 768];
+    kv [*, >= 1536] with k | v in its first 1536 columns; key_rows int32 [n_lists, >= max keys] (row-major, any row
+    stride); n_keys int32 [n_lists]; list_of_query int32 [n_q] or None (query r reads list r).  -> ctx [n_q, 768]
+    (into `out` when given); lse: optional fp32 [n_q, 12]"""
+    _check2d(q, "attention_decode q"); _check2d(kv, "attention_decode kv"); _check2d(key_rows, "attention_decode key_rows")
+    for t, name in ((key_rows, "key_rows"), (n_keys, "n_keys"), (list_of_query, "list_of_query")):
+        if t is not None and t.dtype != I32:
+            raise RuntimeError("univl_b200: attention_decode %s must be int32" % name)
+    o = _empty((q.shape[0], HEADS * 64), BF16, q) if out is None else out
+    _check2d(o, "attention_decode out")
+    call("univl_attention_decode_fwd", q.data_ptr(), q.stride(0), kv.data_ptr(), kv.stride(0), key_rows.data_ptr(),
+         key_rows.stride(0), n_keys.data_ptr(), ptr(list_of_query), q.shape[0], HEADS, o.data_ptr(), o.stride(0),
+         ptr(lse), 1.0 / math.sqrt(64.0))
+    return o
+
+
 def _split_qkv(qkv):
     H = qkv.shape[1] // 3
     return qkv[:, :H], qkv[:, H:2 * H], qkv[:, 2 * H:]
