@@ -161,6 +161,17 @@ int univl_attention_pair_fwd(const void* qa, long long ldqa, const void* ka, lon
                              const void* vb, long long ldvb, void* o, long long ldo, float* lse,
                              const long long* mask_a, const long long* mask_b, int Na, int Wa, int Nb, int Fb,
                              int heads, int Sq, float scale, void* stream);
+/* univl_attention_pair_fwd on a list of n_pairs pairs: sequence p = concat(a_i, b_j) with i = text_index[p] and
+ * j = video_index[p] (int32 [n_pairs], any order, repeats allowed, each in range of its source; not checked here),
+ * its rows read from the two sources as above.  mask_a [n_pairs, Wa] and mask_b [n_pairs, Fb] are the listed pairs'
+ * own mask rows (row p of each), both needed, Fb > 0.  The context is [n_pairs * Sq, heads * 64]; the same kernels
+ * run for the same Wa + Fb, so a listed pair's context equals the all-pairs entry's for (i, j) bit for bit. */
+int univl_attention_pair_list_fwd(const void* qa, long long ldqa, const void* ka, long long ldka, const void* va,
+                                  long long ldva, const void* qb, long long ldqb, const void* kb, long long ldkb,
+                                  const void* vb, long long ldvb, void* o, long long ldo, float* lse,
+                                  const int* text_index, const int* video_index, const long long* mask_a,
+                                  const long long* mask_b, int n_pairs, int Wa, int Fb, int heads, int Sq,
+                                  float scale, void* stream);
 /* Forward only, no dropout, no mask: the attention core of n_seq variable-length sequences in one launch.  Sequence p
  * has Sk_p = cu_seqlens[p + 1] - cu_seqlens[p] keys (int32 [n_seq + 1], ascending), all of them real.  Two row
  * addressings of q/k/v:
@@ -286,6 +297,14 @@ int univl_vocab_xent_fwd(const void* x, long long ldx, const void* w, long long 
 int univl_vocab_xent_bwd(const void* x, long long ldx, const void* w, long long ldw, const float* bias,
                          const long long* labels, const float* lse, const float* sum_count, const float* gscale,
                          void* dlogits, long long ld_d, int T, int V, int Kc, int groups, void* stream);
+/* Exact top-k of sim = t v^T per text row, the matrix never written (retrieval shortlists): t [Nt, H], v [Nv, H]
+ * fp32 row-major, 16-byte aligned, H a multiple of 4.  scores fp32 [Nt, k] and index int32 [Nt, k] hold row i's k
+ * best videos in one strict order: score descending, then video index ascending.  Every score has the bits
+ * univl_sim_matmul_fwd (groups = 1) gives the same entry, and the result does not depend on how the kernel tiles or
+ * splits the gallery: repeated launches write the same bytes.  1 <= k <= min(256, Nv); otherwise UNIVL_ERR_ARG.
+ * Inputs are expected finite (a NaN score has no place in the order). */
+int univl_sim_topk(const float* t, const float* v, float* scores, int* index, int Nt, int Nv, int H, int k,
+                   void* stream);
 /* cross pooler tanh + similarity_dense (module_cross.py:281-287; modeling.py:371): out[r] = tanh(u[r,:]).w + b */
 int univl_pooler_sim_fwd(const void* u, const float* w, const float* b, float* out, int N, int H, void* stream);
 int univl_pooler_sim_bwd(const void* u, const float* w, const float* dout, void* du, float* dw, float* db, int N,

@@ -84,10 +84,10 @@ attention_fwd_kernel(const AttnParams p_in, const PairSrc pb, const VarlenSrc vl
     load_varlen_q(sQ, p.q, p.ldq, pb.q, pb.ldq, vl, seq, h, 0, p.Sq, Sq16);
     load_varlen_tile(sK, p.k, p.ldk, pb.k, pb.ldk, vl, seq, h, 0, p.Sk, Sk16);
     load_varlen_tile(sV, p.v, p.ldv, pb.v, pb.ldv, vl, seq, h, 0, p.Sk, Sk16);
-  } else if constexpr (ADDR == ADDR_PAIR) {
-    load_pair_tile(sQ, p.q, p.ldq, pb.q, pb.ldq, p, seq, h, 0, p.Sq, Sq16);
-    load_pair_tile(sK, p.k, p.ldk, pb.k, pb.ldk, p, seq, h, 0, p.Sk, Sk16);
-    load_pair_tile(sV, p.v, p.ldv, pb.v, pb.ldv, p, seq, h, 0, p.Sk, Sk16);
+  } else if constexpr (ADDR == ADDR_PAIR || ADDR == ADDR_PAIR_LIST) {
+    load_pair_tile<ADDR>(sQ, p.q, p.ldq, pb.q, pb.ldq, p, vl, seq, h, 0, p.Sq, Sq16);
+    load_pair_tile<ADDR>(sK, p.k, p.ldk, pb.k, pb.ldk, p, vl, seq, h, 0, p.Sk, Sk16);
+    load_pair_tile<ADDR>(sV, p.v, p.ldv, pb.v, pb.ldv, p, vl, seq, h, 0, p.Sk, Sk16);
   } else {
     load_head_tile(sQ, p.q + (long long)seq * p.Sq * p.ldq + h * HD, p.ldq, p.Sq, Sq16);
     load_head_tile(sK, p.k + (long long)seq * p.Sk * p.ldk + h * HD, p.ldk, p.Sk, Sk16);
@@ -628,6 +628,7 @@ int attention_fwd_launch(const AttnParams& p, Addr addr, const PairSrc& pb, cons
   const int nkb = Sk16 / 16;
   void (*kern)(const AttnParams, const PairSrc, const VarlenSrc) =
       addr == ADDR_PAIR ? fwd_kernel_for<ADDR_PAIR>(nkb)
+      : addr == ADDR_PAIR_LIST ? fwd_kernel_for<ADDR_PAIR_LIST>(nkb)
       : addr == ADDR_VARLEN_PAIR ? fwd_kernel_for<ADDR_VARLEN_PAIR>(nkb)
       : addr == ADDR_VARLEN_PACKED ? fwd_kernel_for<ADDR_VARLEN_PACKED>(nkb) : fwd_kernel_for<ADDR_DENSE>(nkb);
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

@@ -49,7 +49,9 @@ struct PairSrc {
 //   ADDR_PAIR           all-pairs concat(a_i, b_j) of two sources (load_pair_tile, univl_attention_pair_fwd)
 //   ADDR_VARLEN_PAIR    varlen sequences whose rows are picked from two sources by index lists (VarlenSrc)
 //   ADDR_VARLEN_PACKED  varlen sequences stored back to back (VarlenSrc)
-enum Addr : int { ADDR_DENSE = 0, ADDR_PAIR = 1, ADDR_VARLEN_PAIR = 2, ADDR_VARLEN_PACKED = 3 };
+//   ADDR_PAIR_LIST      listed pairs concat(a_i, b_j), (i, j) = (VarlenSrc idx_a[s], idx_b[s]), rows as ADDR_PAIR
+//                       (univl_attention_pair_list_fwd)
+enum Addr : int { ADDR_DENSE = 0, ADDR_PAIR = 1, ADDR_VARLEN_PAIR = 2, ADDR_VARLEN_PACKED = 3, ADDR_PAIR_LIST = 4 };
 
 // The varlen forward's sequences (univl_attention_varlen_fwd, univl_gather_rows_varlen).  Sequence p has
 // Sk_p = cu[p + 1] - cu[p] rows, every one of them a real key (no mask).  Pair addressing (idx_a != null): row r < len_a[p]
@@ -91,12 +93,20 @@ __device__ __forceinline__ void load_head_tile(bf16* dst, const bf16* src, long 
 }
 
 // load_head_tile for the pair forward: rows [r0, r0 + rows) of sequence `seq` = concat(text i, video j) (all-pairs
-// pairing), whose row s is row i * Wa + s of the first source a (s < Wa) or row j * Fb + s - Wa of the second source b.
-// a / b point at column 0 of the q, k or v projections of each source.
+// pairing under ADDR_PAIR, the pair list vl.idx_a / vl.idx_b under ADDR_PAIR_LIST), whose row s is row i * Wa + s of
+// the first source a (s < Wa) or row j * Fb + s - Wa of the second source b.  a / b point at column 0 of the q, k or v
+// projections of each source.
+template <int ADDR>
 __device__ __forceinline__ void load_pair_tile(bf16* dst, const bf16* a, long long lda, const bf16* b, long long ldb,
-                                               const AttnParams& p, int seq, int h, int r0, int rows, int rows16) {
+                                               const AttnParams& p, const VarlenSrc& vl, int seq, int h, int r0,
+                                               int rows, int rows16) {
   long long i, j;
-  pair_sources(seq, 1, p.n_seq, p.Nb, i, j);
+  if constexpr (ADDR == ADDR_PAIR_LIST) {
+    i = vl.idx_a[seq];
+    j = vl.idx_b[seq];
+  } else {
+    pair_sources(seq, 1, p.n_seq, p.Nb, i, j);
+  }
   const bf16* ra = a + i * p.Wa * lda + h * HD;
   const bf16* rb = b + j * p.Fb * ldb + h * HD;
   for (int idx = threadIdx.x; idx < rows16 * 8; idx += blockDim.x) {

@@ -69,7 +69,7 @@ __device__ __forceinline__ void write_partial_row(const float* slots, int nwarps
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// forward (ADDR: the row addressing of Q/K/V, attention_common.cuh Addr; under ADDR_PAIR and ADDR_VARLEN_PAIR a key tile
+// forward (ADDR: the row addressing of Q/K/V, attention_common.cuh Addr; under the pair addressings a key tile
 // may straddle the boundary between the two sources.  Under the varlen addressings each CTA takes its own sequence's
 // Sq / Sk, the query blocks past its Sq exit at once, and output / lse go to VarlenSrc's rows.)
 // ------------------------------------------------------------------------------------------------------------
@@ -105,16 +105,17 @@ attention_long_fwd_kernel(const AttnParams p_in, const PairSrc pb, const VarlenS
     if constexpr (VARLEN) {
       load_varlen_tile(sK, p.k, p.ldk, pb.k, pb.ldk, vl, seq, h, k0, min(LT, p.Sk - k0), LT);
       load_varlen_tile(sK + LT * LDS, p.v, p.ldv, pb.v, pb.ldv, vl, seq, h, k0, min(LT, p.Sk - k0), LT);
-    } else if constexpr (ADDR == ADDR_PAIR) {
-      load_pair_tile(sK, p.k, p.ldk, pb.k, pb.ldk, p, seq, h, k0, min(LT, p.Sk - k0), LT);
-      load_pair_tile(sK + LT * LDS, p.v, p.ldv, pb.v, pb.ldv, p, seq, h, k0, min(LT, p.Sk - k0), LT);
+    } else if constexpr (ADDR == ADDR_PAIR || ADDR == ADDR_PAIR_LIST) {
+      load_pair_tile<ADDR>(sK, p.k, p.ldk, pb.k, pb.ldk, p, vl, seq, h, k0, min(LT, p.Sk - k0), LT);
+      load_pair_tile<ADDR>(sK + LT * LDS, p.v, p.ldv, pb.v, pb.ldv, p, vl, seq, h, k0, min(LT, p.Sk - k0), LT);
     } else {
       load_head_tile(sK, p.k + ((long long)seq * p.Sk + k0) * p.ldk + h * HD, p.ldk, min(LT, p.Sk - k0), LT);
       load_head_tile(sK + LT * LDS, p.v + ((long long)seq * p.Sk + k0) * p.ldv + h * HD, p.ldv, min(LT, p.Sk - k0), LT);
     }
   };
   if constexpr (VARLEN) load_varlen_q(sQ, p.q, p.ldq, pb.q, pb.ldq, vl, seq, h, qbase, qrows, qrows16);
-  else if constexpr (ADDR == ADDR_PAIR) load_pair_tile(sQ, p.q, p.ldq, pb.q, pb.ldq, p, seq, h, qbase, qrows, qrows16);
+  else if constexpr (ADDR == ADDR_PAIR || ADDR == ADDR_PAIR_LIST)
+    load_pair_tile<ADDR>(sQ, p.q, p.ldq, pb.q, pb.ldq, p, vl, seq, h, qbase, qrows, qrows16);
   else load_head_tile(sQ, p.q + ((long long)seq * p.Sq + qbase) * p.ldq + h * HD, p.ldq, qrows, qrows16);
   build_key_mask(madd, p, seq, Sk16);
   load_kv(0, 0);
@@ -529,6 +530,7 @@ int attention_long_fwd_launch(const AttnParams& p, Addr addr, const PairSrc& pb,
   const size_t smem = (size_t)(LB + 4 * LT) * LDS * 2 + (size_t)Sk16 * 4;
   void (*kern)(const AttnParams, const PairSrc, const VarlenSrc) =
       addr == ADDR_PAIR ? attention_long_fwd_kernel<ADDR_PAIR>
+      : addr == ADDR_PAIR_LIST ? attention_long_fwd_kernel<ADDR_PAIR_LIST>
       : addr == ADDR_VARLEN_PAIR ? attention_long_fwd_kernel<ADDR_VARLEN_PAIR>
       : addr == ADDR_VARLEN_PACKED ? attention_long_fwd_kernel<ADDR_VARLEN_PACKED> : attention_long_fwd_kernel<ADDR_DENSE>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

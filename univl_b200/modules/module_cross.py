@@ -154,6 +154,33 @@ class CrossModel(PreTrainedModel):
             x = ops.encoder_layer_eval_fp8(x, n_seq, S, mask, _layer_params(layers[i]), qw[i])
         return ops.cls_layer_eval_fp8(x, n_seq, S, mask, _layer_params(layers[-1]), qw[-1])
 
+    def encode_pairs_first_token_eval_list(self, x, qkv, text_mask, video_mask, text_index, video_index, qw=None):
+        """encode_pairs_first_token_eval (qw None) or _fp8 (qw = fp8_eval_weights()) on a list of pairs instead of a
+        grid, each pair at all W + F tokens: sequence p = (text row text_index[p], video row video_index[p]) (int32
+        device tensors).  x, qkv: first_layer_source_rows of the call.  The first layer reads Q/K/V from qkv through
+        the list (ops.attention_pair_fwd), its residual rows are gathered from x, and every layer reads the listed
+        pairs' own mask rows, so a pair's result equals the grid's -> [P, H]"""
+        Nt, W = text_mask.shape
+        Nv, F = video_mask.shape
+        S, P, rows_t = W + F, text_index.numel(), Nt * W
+        pairs = (text_index, video_index)
+        mask = ops.MaskSpec(text_mask.index_select(0, text_index.long()),
+                            video_mask.index_select(0, video_index.long()), all_pairs=0)
+        h = ops.gather_rows_varlen(x[:rows_t], x[rows_t:], ops.padded_pair_seqs(text_index, video_index, Nt, W, Nv, F),
+                                   False)
+        layers = self.encoder.layer
+        if qw is not None:
+            h = ops.pair_layer_eval_fp8(h, qkv[:rows_t], qkv[rows_t:], P, 1, S, mask, _layer_params(layers[0]), qw[0],
+                                        pairs)
+            for i in range(1, len(layers) - 1):
+                h = ops.encoder_layer_eval_fp8(h, P, S, mask, _layer_params(layers[i]), qw[i])
+            return ops.cls_layer_eval_fp8(h, P, S, mask, _layer_params(layers[-1]), qw[-1])
+        h = ops.pair_layer_eval(h, qkv[:rows_t], qkv[rows_t:], P, 1, S, mask, _layer_params(layers[0]),
+                                len(layers) == 1, pairs)
+        if len(layers) == 1:
+            return h
+        return self.encoder.run_first_token(h, P, S, mask, start=1)
+
     def encode_pairs_first_token_eval_packed(self, x, qkv, rows_t, seqs, qw=None):
         """encode_pairs_first_token_eval (qw None) or _fp8 (qw = fp8_eval_weights()) on the packed layout: every pair
         of one tile on its valid tokens alone.  x, qkv: first_layer_source_rows of the call, whose first rows_t rows are

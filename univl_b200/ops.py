@@ -238,11 +238,22 @@ def attention_bwd(q, k, v, o, lse, d_o, dq, dk, dv, n_seq, Sq, Sk, mask, p=0.0, 
          stream, int(rng_layout), ptr(dbq), ptr(dbk), ptr(dbv))
 
 
-def attention_pair_fwd(qkv_a, qkv_b, Na, Nb, Sq, mask):
+def attention_pair_fwd(qkv_a, qkv_b, Na, Nb, Sq, mask, pairs=None):
     """Attention core of the Na x Nb sequences concat(a_i, b_j), p = i * Nb + j, reading Q/K/V from per-source
     projections (csrc/attention_pair.cu): qkv_a [Na*Wa, 3H] and qkv_b [Nb*Fb, 3H] hold q | k | v of every source row.
-    Sq = Wa + Fb, or 1 for token 0 only.  No dropout.  -> ctx [Na*Nb*Sq, H]"""
+    Sq = Wa + Fb, or 1 for token 0 only.  No dropout.  -> ctx [Na*Nb*Sq, H].
+    pairs: (text_index, video_index) int32 [P] on the device — the listed sequences p = (text_index[p], video_index[p])
+    instead of the grid (univl_attention_pair_list_fwd), with mask holding the listed pairs' own rows -> [P*Sq, H]"""
     H = HEADS * 64
+    if pairs is not None:
+        ti, vi = pairs
+        o = _empty((ti.numel() * Sq, H), BF16, qkv_a)
+        call("univl_attention_pair_list_fwd", qkv_a.data_ptr(), qkv_a.stride(0), qkv_a[:, H:].data_ptr(),
+             qkv_a.stride(0), qkv_a[:, 2 * H:].data_ptr(), qkv_a.stride(0), qkv_b.data_ptr(), qkv_b.stride(0),
+             qkv_b[:, H:].data_ptr(), qkv_b.stride(0), qkv_b[:, 2 * H:].data_ptr(), qkv_b.stride(0), o.data_ptr(),
+             o.stride(0), None, ti.data_ptr(), vi.data_ptr(), ptr(mask.a), ptr(mask.b), ti.numel(), mask.Wa, mask.Fb,
+             HEADS, Sq, 1.0 / math.sqrt(64.0))
+        return o
     o = _empty((Na * Nb * Sq, H), BF16, qkv_a)
     call("univl_attention_pair_fwd", qkv_a.data_ptr(), qkv_a.stride(0), qkv_a[:, H:].data_ptr(), qkv_a.stride(0),
          qkv_a[:, 2 * H:].data_ptr(), qkv_a.stride(0), qkv_b.data_ptr(), qkv_b.stride(0), qkv_b[:, H:].data_ptr(),
@@ -263,18 +274,19 @@ def embed_src_rows_eval(a, N, W, pos, type_w, gamma, beta, out):
     return out
 
 
-def pair_layer_eval(x, qkv_a, qkv_b, Na, Nb, S, mask, params, first_token):
+def pair_layer_eval(x, qkv_a, qkv_b, Na, Nb, S, mask, params, first_token, pairs=None):
     """An encoder layer over the Na x Nb pair sequences in evaluation (no dropout, no autograd) whose Q/K/V
     projections are given per source row, computed once per text row and once per video row instead of once per pair.
     x: the pair inputs [Na*Nb*S, H] (the residual of the attention block); params as EncoderLayerFn.  first_token: the
     layer is the stack's last and produces token 0 of every sequence only, as EncoderLayerClsFn -> [Na*Nb, H].
-    Same arithmetic as EncoderLayerFn / EncoderLayerClsFn on the QKV-GEMM + attention-core path."""
+    Same arithmetic as EncoderLayerFn / EncoderLayerClsFn on the QKV-GEMM + attention-core path.  pairs: the listed
+    sequences of attention_pair_fwd instead of the grid (x then holds their P*S rows)."""
     arena = rt.current()
     wa = dict(zip(ATT_KEYS, params[:10]))
     wf = dict(zip(FFN_KEYS, params[10:16]))
     drop = _Drop(0.0, 0.0, False)
-    n_seq = Na * Nb
-    ctx = attention_pair_fwd(qkv_a, qkv_b, Na, Nb, 1 if first_token else S, mask)
+    n_seq = pairs[0].numel() if pairs is not None else Na * Nb
+    ctx = attention_pair_fwd(qkv_a, qkv_b, Na, Nb, 1 if first_token else S, mask, pairs)
     xq = x.view(n_seq, S, -1)[:, 0].contiguous() if first_token else x
     ao = linear_fwd(ctx, arena.bf16(wa["o"]), wa["bo"])
     y, _, _ = layernorm_fwd(ao, xq, wa["gamma"], wa["beta"], 0.0, 1, drop.seed, drop.stream())
@@ -362,10 +374,10 @@ def _fp8_layer_tail(ctx, x, params, qw):
     return out
 
 
-def pair_layer_eval_fp8(x, qkv_a, qkv_b, Na, Nb, S, mask, params, qw):
+def pair_layer_eval_fp8(x, qkv_a, qkv_b, Na, Nb, S, mask, params, qw, pairs=None):
     """pair_layer_eval for a layer that is not the stack's last, its dense GEMMs over the pair tokens in FP8
     (qw holds "o", "w1", "w2" of fp8_layer_weights).  The attention core and the LayerNorms stay bf16."""
-    ctx = attention_pair_fwd(qkv_a, qkv_b, Na, Nb, S, mask)
+    ctx = attention_pair_fwd(qkv_a, qkv_b, Na, Nb, S, mask, pairs)
     return _fp8_layer_tail(ctx, x, params, qw)
 
 
@@ -481,6 +493,29 @@ class PairPacking:
         cu = _exclusive_cumsum(len_a.long() + len_b.long()).to(I32)
         return VarlenSeqs(cu, self.tokens(t0, t1, v0, v1), self.max_sk, self.idx_t, self.idx_v,
                           self.start_t[t0:t1].repeat_interleave(nv), self.start_v[v0:v1].repeat(nt), len_a)
+
+    def pairs(self, text_index, video_index):
+        """VarlenSeqs (pair addressing) of the listed pairs p = (text_index[p], video_index[p]) (int64 or int32
+        tensors on the masks' device, in range), in list order.  max_sk stays the call's, so each pair runs on the
+        attention kernel the grid would run it on.  `total` costs one device-to-host copy."""
+        ti, vi = text_index.long(), video_index.long()
+        len_a = self.n_t[ti]
+        cu = _exclusive_cumsum(len_a.long() + self.n_v[vi].long())
+        return VarlenSeqs(cu.to(I32), int(cu[-1]), self.max_sk, self.idx_t, self.idx_v, self.start_t[ti],
+                          self.start_v[vi], len_a)
+
+
+def padded_pair_seqs(text_index, video_index, Nt, W, Nv, F):
+    """VarlenSeqs (pair addressing) of the listed pairs at all W + F tokens, over the rows of the per-source sources
+    [Nt*W, *] (text) and [Nv*F, *] (video): pair p's rows are text rows text_index[p] * W + [0, W) then video rows
+    video_index[p] * F + [0, F) — the padded layout's pair sequence, for gather_rows_varlen"""
+    dev = text_index.device
+    P, S = text_index.numel(), W + F
+    cu = torch.arange(P + 1, dtype=I32, device=dev) * S
+    idx_a = torch.arange(Nt * W, dtype=I32, device=dev)
+    idx_b = torch.arange(Nv * F, dtype=I32, device=dev)
+    return VarlenSeqs(cu, P * S, S, idx_a, idx_b, (text_index.long() * W).to(I32), (video_index.long() * F).to(I32),
+                      torch.full((P,), W, dtype=I32, device=dev))
 
 
 def attention_varlen_fwd(q, k, v, seqs, q_first, qb=None, kb=None, vb=None):
@@ -1247,6 +1282,18 @@ class SimMatmulFn(torch.autograd.Function):
         call("univl_sim_matmul_bwd", ds.data_ptr(), t.data_ptr(), v.data_ptr(), dt.data_ptr(), dv.data_ptr(),
              t.shape[0] // G, v.shape[0] // G, t.shape[1], G)
         return dt, dv, None
+
+
+def sim_topk(t, v, k):
+    """Exact top-k of t v^T per row (csrc/retrieval.cu): t [Nt, H], v [Nv, H] fp32 -> (scores fp32 [Nt, k], index int32
+    [Nt, k]), score descending then index ascending; each score has SimMatmulFn's bits.  1 <= k <= min(256, Nv)."""
+    t, v = t.contiguous(), v.contiguous()
+    _check2d(t, "sim_topk t"); _check2d(v, "sim_topk v")
+    Nt, H = t.shape
+    scores = _empty((Nt, max(int(k), 0)), F32, t)
+    index = _empty((Nt, max(int(k), 0)), I32, t)
+    call("univl_sim_topk", t.data_ptr(), v.data_ptr(), scores.data_ptr(), index.data_ptr(), Nt, v.shape[0], H, int(k))
+    return scores, index
 
 
 class SimLossFn(torch.autograd.Function):
