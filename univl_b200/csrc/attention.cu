@@ -12,8 +12,6 @@
 // dK/dV pass of backward) at a time.  Backward recomputes P from Q, K and the saved log-sum-exp, flash-style, with
 // no atomics: dQ is produced by query-row tasks, dK/dV by key-row tasks that recompute the transposed tiles.
 // Dropout masks are Philox(seed, stream, element) and regenerated identically in every pass.
-#include <stdlib.h>
-
 #include "attention_common.cuh"
 
 namespace univl {
@@ -58,16 +56,8 @@ __global__ void __launch_bounds__(ATT_FWD_WARPS * 32)  // (capping S=96 at 112 r
 attention_fwd_kernel(const AttnParams p_in, const PairSrc pb, const VarlenSrc vl) {
   pdl_trigger();
   pdl_wait();
-  AttnParams p = p_in;
-  if (p.drop_on && p.rng != nullptr) {
-    p.seed = p.rng[0];
-    p.stream += p.rng[1] << 20;
-  }
-  constexpr bool VARLEN = ADDR == ADDR_VARLEN_PAIR || ADDR == ADDR_VARLEN_PACKED;
-  if constexpr (VARLEN) {
-    varlen_shape(p, vl, blockIdx.x / p.heads);
-    if (p.Sk <= 0) return;
-  }
+  AttnParams p = resolve_rng(p_in);
+  if (!seq_shape<ADDR>(p, vl, blockIdx.x / p.heads)) return;
   extern __shared__ __align__(16) uint8_t smem_att[];
   const int Sq16 = (p.Sq + 15) & ~15, Sk16 = (p.Sk + 15) & ~15;
   bf16* sQ = reinterpret_cast<bf16*>(smem_att);
@@ -78,21 +68,11 @@ attention_fwd_kernel(const AttnParams p_in, const PairSrc pb, const VarlenSrc vl
   const int seq = blockIdx.x / p.heads, h = blockIdx.x % p.heads;
   const long long bh = blockIdx.x;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int g = lane >> 2, t = lane & 3;
+  const int g = lane >> 2;
 
-  if constexpr (VARLEN) {
-    load_varlen_q(sQ, p.q, p.ldq, pb.q, pb.ldq, vl, seq, h, 0, p.Sq, Sq16);
-    load_varlen_tile(sK, p.k, p.ldk, pb.k, pb.ldk, vl, seq, h, 0, p.Sk, Sk16);
-    load_varlen_tile(sV, p.v, p.ldv, pb.v, pb.ldv, vl, seq, h, 0, p.Sk, Sk16);
-  } else if constexpr (ADDR == ADDR_PAIR || ADDR == ADDR_PAIR_LIST) {
-    load_pair_tile<ADDR>(sQ, p.q, p.ldq, pb.q, pb.ldq, p, vl, seq, h, 0, p.Sq, Sq16);
-    load_pair_tile<ADDR>(sK, p.k, p.ldk, pb.k, pb.ldk, p, vl, seq, h, 0, p.Sk, Sk16);
-    load_pair_tile<ADDR>(sV, p.v, p.ldv, pb.v, pb.ldv, p, vl, seq, h, 0, p.Sk, Sk16);
-  } else {
-    load_head_tile(sQ, p.q + (long long)seq * p.Sq * p.ldq + h * HD, p.ldq, p.Sq, Sq16);
-    load_head_tile(sK, p.k + (long long)seq * p.Sk * p.ldk + h * HD, p.ldk, p.Sk, Sk16);
-    load_head_tile(sV, p.v + (long long)seq * p.Sk * p.ldv + h * HD, p.ldv, p.Sk, Sk16);
-  }
+  load_rows<ADDR, OP_Q>(sQ, p, pb, vl, seq, h, 0, p.Sq, Sq16);
+  load_rows<ADDR, OP_K>(sK, p, pb, vl, seq, h, 0, p.Sk, Sk16);
+  load_rows<ADDR, OP_V>(sV, p, pb, vl, seq, h, 0, p.Sk, Sk16);
   build_key_mask(madd, p, seq, Sk16);
   cp_async_wait_all();
   __syncthreads();
@@ -101,13 +81,22 @@ attention_fwd_kernel(const AttnParams p_in, const PairSrc pb, const VarlenSrc vl
     uint32_t qa[4][4];
     load_a_frags(sQ, q0, lane, qa);
     const int i0 = q0 + g, i1 = q0 + g + 8;
+    float o[8][4];
+    float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
     if constexpr (NKB > 0) {
       const int nkb = Sk16 >> 4;
       float s[NKB][2][4];
 #pragma unroll
       for (int kb = 0; kb < NKB; ++kb)
         if (kb < nkb) mma_a_yT(qa, sK, kb * 16, lane, s[kb]);
-      float mx0 = -INFINITY, mx1 = -INFINITY;
+#pragma unroll
+      for (int kb = 0; kb < NKB; ++kb)
+        if (kb < nkb) {
+          scale_mask(p, madd, kb * 16, i0, i1, lane, s[kb]);
+          row_max(s[kb], m0, m1);
+        }
+      m0 = quad_max(m0);
+      m1 = quad_max(m1);
 #pragma unroll
       for (int kb = 0; kb < NKB; ++kb)
         if (kb < nkb) {
@@ -115,43 +104,15 @@ attention_fwd_kernel(const AttnParams p_in, const PairSrc pb, const VarlenSrc vl
           for (int nb = 0; nb < 2; ++nb)
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
-              const int j = kb * 16 + nb * 8 + 2 * t + e;
-              const float ma = madd[j];
-              float a0 = ma, a1 = ma;
-              if (p.causal) {
-                if (j > i0 && a0 == 0.f) a0 = -10000.f;
-                if (j > i1 && a1 == 0.f) a1 = -10000.f;
-              }
-              s[kb][nb][e] = s[kb][nb][e] * p.scale + a0;
-              s[kb][nb][2 + e] = s[kb][nb][2 + e] * p.scale + a1;
-              mx0 = fmaxf(mx0, s[kb][nb][e]);
-              mx1 = fmaxf(mx1, s[kb][nb][2 + e]);
+              s[kb][nb][e] = __expf(s[kb][nb][e] - m0);
+              s[kb][nb][2 + e] = __expf(s[kb][nb][2 + e] - m1);
+              l0 += s[kb][nb][e];
+              l1 += s[kb][nb][2 + e];
             }
         }
-      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
-      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
-      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
-      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
-      float sum0 = 0.f, sum1 = 0.f;
-#pragma unroll
-      for (int kb = 0; kb < NKB; ++kb)
-        if (kb < nkb) {
-#pragma unroll
-          for (int nb = 0; nb < 2; ++nb)
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              s[kb][nb][e] = __expf(s[kb][nb][e] - mx0);
-              s[kb][nb][2 + e] = __expf(s[kb][nb][2 + e] - mx1);
-              sum0 += s[kb][nb][e];
-              sum1 += s[kb][nb][2 + e];
-            }
-        }
-      sum0 += __shfl_xor_sync(0xffffffffu, sum0, 1);
-      sum0 += __shfl_xor_sync(0xffffffffu, sum0, 2);
-      sum1 += __shfl_xor_sync(0xffffffffu, sum1, 1);
-      sum1 += __shfl_xor_sync(0xffffffffu, sum1, 2);
-      const float r0 = 1.0f / sum0, r1 = 1.0f / sum1;
-      float o[8][4];
+      l0 = quad_sum(l0);
+      l1 = quad_sum(l1);
+      const float r0 = 1.0f / l0, r1 = 1.0f / l1;
 #pragma unroll
       for (int nb = 0; nb < 8; ++nb)
 #pragma unroll
@@ -167,132 +128,70 @@ attention_fwd_kernel(const AttnParams p_in, const PairSrc pb, const VarlenSrc vl
             for (int e = 0; e < 2; ++e) {
               float p0 = s[kb][nb][e] * r0, p1 = s[kb][nb][2 + e] * r1;
               if (p.drop_on) {
-                p0 = philox_u16(rnd, e | (nb << 2)) < p.drop_threshold ? p0 * p.drop_scale : 0.f;
-                p1 = philox_u16(rnd, e | 2 | (nb << 2)) < p.drop_threshold ? p1 * p.drop_scale : 0.f;
+                p0 = dropout(p, philox_u16(rnd, e | (nb << 2)), p0);
+                p1 = dropout(p, philox_u16(rnd, e | 2 | (nb << 2)), p1);
               }
               s[kb][nb][e] = p0;
               s[kb][nb][2 + e] = p1;
             }
           uint32_t pa[4];
-          pa[0] = pack_bf16x2(s[kb][0][0], s[kb][0][1]);
-          pa[1] = pack_bf16x2(s[kb][0][2], s[kb][0][3]);
-          pa[2] = pack_bf16x2(s[kb][1][0], s[kb][1][1]);
-          pa[3] = pack_bf16x2(s[kb][1][2], s[kb][1][3]);
+          pack_a(s[kb], pa);
           mma_p_z(pa, sV, kb * 16, lane, o);
         }
-      // output row of query 0; lse [n_seq, heads, Sq], or [rows, heads] under the varlen addressings
-      const long long ob = VARLEN ? varlen_out_row(vl, seq) : (long long)seq * p.Sq;
-      bf16* orow0 = p.o + (ob + i0) * p.ldo + h * HD;
-      bf16* orow1 = p.o + (ob + i1) * p.ldo + h * HD;
+    } else {
+      // pass 1: row max and sum of exponentials
+      for (int j0 = 0; j0 < Sk16; j0 += 16) {
+        float s[2][4];
+        mma_a_yT(qa, sK, j0, lane, s);
+        scale_mask(p, madd, j0, i0, i1, lane, s);
+        float cm0 = -INFINITY, cm1 = -INFINITY;
+        row_max(s, cm0, cm1);
+        const float n0 = fmaxf(m0, quad_max(cm0)), n1 = fmaxf(m1, quad_max(cm1));
+        float e0 = 0.f, e1 = 0.f;
 #pragma unroll
-      for (int nb = 0; nb < 8; ++nb) {
-        if (i0 < p.Sq) *reinterpret_cast<uint32_t*>(orow0 + nb * 8 + 2 * t) = pack_bf16x2(o[nb][0], o[nb][1]);
-        if (i1 < p.Sq) *reinterpret_cast<uint32_t*>(orow1 + nb * 8 + 2 * t) = pack_bf16x2(o[nb][2], o[nb][3]);
-      }
-      if (t == 0 && p.lse != nullptr) {
-        if (i0 < p.Sq) p.lse[VARLEN ? (ob + i0) * p.heads + h : bh * p.Sq + i0] = mx0 + __logf(sum0);
-        if (i1 < p.Sq) p.lse[VARLEN ? (ob + i1) * p.heads + h : bh * p.Sq + i1] = mx1 + __logf(sum1);
-      }
-      continue;
-    }
-    float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
-    // pass 1: row max and sum of exponentials
-    for (int j0 = 0; j0 < Sk16; j0 += 16) {
-      float s[2][4];
-      mma_a_yT(qa, sK, j0, lane, s);
-      float cm0 = -INFINITY, cm1 = -INFINITY;
+        for (int nb = 0; nb < 2; ++nb)
 #pragma unroll
-      for (int nb = 0; nb < 2; ++nb)
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int j = j0 + nb * 8 + 2 * t + e;
-          float ma = madd[j];
-          float a0 = ma, a1 = ma;
-          if (p.causal) {
-            if (j > i0 && a0 == 0.f) a0 = -10000.f;
-            if (j > i1 && a1 == 0.f) a1 = -10000.f;
+          for (int e = 0; e < 2; ++e) {
+            e0 += __expf(s[nb][e] - n0);
+            e1 += __expf(s[nb][2 + e] - n1);
           }
-          s[nb][e] = s[nb][e] * p.scale + a0;
-          s[nb][2 + e] = s[nb][2 + e] * p.scale + a1;
-          cm0 = fmaxf(cm0, s[nb][e]);
-          cm1 = fmaxf(cm1, s[nb][2 + e]);
-        }
-      cm0 = fmaxf(cm0, __shfl_xor_sync(0xffffffffu, cm0, 1));
-      cm0 = fmaxf(cm0, __shfl_xor_sync(0xffffffffu, cm0, 2));
-      cm1 = fmaxf(cm1, __shfl_xor_sync(0xffffffffu, cm1, 1));
-      cm1 = fmaxf(cm1, __shfl_xor_sync(0xffffffffu, cm1, 2));
-      const float n0 = fmaxf(m0, cm0), n1 = fmaxf(m1, cm1);
-      float e0 = 0.f, e1 = 0.f;
-#pragma unroll
-      for (int nb = 0; nb < 2; ++nb)
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          e0 += __expf(s[nb][e] - n0);
-          e1 += __expf(s[nb][2 + e] - n1);
-        }
-      e0 += __shfl_xor_sync(0xffffffffu, e0, 1);
-      e0 += __shfl_xor_sync(0xffffffffu, e0, 2);
-      e1 += __shfl_xor_sync(0xffffffffu, e1, 1);
-      e1 += __shfl_xor_sync(0xffffffffu, e1, 2);
-      l0 = l0 * __expf(m0 - n0) + e0;
-      l1 = l1 * __expf(m1 - n1) + e1;
-      m0 = n0;
-      m1 = n1;
-    }
-    const float inv0 = 1.0f / l0, inv1 = 1.0f / l1;
-    // pass 2: normalised probabilities -> P V
-    float o[8][4];
-#pragma unroll
-    for (int nb = 0; nb < 8; ++nb)
-#pragma unroll
-      for (int e = 0; e < 4; ++e) o[nb][e] = 0.f;
-    for (int j0 = 0; j0 < Sk16; j0 += 16) {
-      float s[2][4];
-      mma_a_yT(qa, sK, j0, lane, s);
-      uint4 rnd = make_uint4(0, 0, 0, 0);
-      if (p.drop_on) rnd = tile_rng(p, bh, q0 >> 4, j0 >> 4, Sq16 >> 4, Sk16 >> 4, lane);
-#pragma unroll
-      for (int nb = 0; nb < 2; ++nb) {
-        const int jb = j0 + nb * 8 + 2 * t;
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int j = jb + e;
-          float ma = madd[j];
-          float a0 = ma, a1 = ma;
-          if (p.causal) {
-            if (j > i0 && a0 == 0.f) a0 = -10000.f;
-            if (j > i1 && a1 == 0.f) a1 = -10000.f;
-          }
-          float p0 = __expf(s[nb][e] * p.scale + a0 - m0) * inv0;
-          float p1 = __expf(s[nb][2 + e] * p.scale + a1 - m1) * inv1;
-          if (p.drop_on) {
-            p0 = philox_u16(rnd, e | (nb << 2)) < p.drop_threshold ? p0 * p.drop_scale : 0.f;
-            p1 = philox_u16(rnd, e | 2 | (nb << 2)) < p.drop_threshold ? p1 * p.drop_scale : 0.f;
-          }
-          s[nb][e] = p0;
-          s[nb][2 + e] = p1;
-        }
+        l0 = l0 * __expf(m0 - n0) + quad_sum(e0);
+        l1 = l1 * __expf(m1 - n1) + quad_sum(e1);
+        m0 = n0;
+        m1 = n1;
       }
-      uint32_t pa[4];
-      pa[0] = pack_bf16x2(s[0][0], s[0][1]);
-      pa[1] = pack_bf16x2(s[0][2], s[0][3]);
-      pa[2] = pack_bf16x2(s[1][0], s[1][1]);
-      pa[3] = pack_bf16x2(s[1][2], s[1][3]);
-      mma_p_z(pa, sV, j0, lane, o);
-    }
-    // store context rows (heads merged: column h*64 + d) and the row log-sum-exp
-    const long long ob = VARLEN ? varlen_out_row(vl, seq) : (long long)seq * p.Sq;
-    bf16* orow0 = p.o + (ob + i0) * p.ldo + h * HD;
-    bf16* orow1 = p.o + (ob + i1) * p.ldo + h * HD;
+      const float inv0 = 1.0f / l0, inv1 = 1.0f / l1;
+      // pass 2: normalised probabilities -> P V
 #pragma unroll
-    for (int nb = 0; nb < 8; ++nb) {
-      if (i0 < p.Sq) *reinterpret_cast<uint32_t*>(orow0 + nb * 8 + 2 * t) = pack_bf16x2(o[nb][0], o[nb][1]);
-      if (i1 < p.Sq) *reinterpret_cast<uint32_t*>(orow1 + nb * 8 + 2 * t) = pack_bf16x2(o[nb][2], o[nb][3]);
+      for (int nb = 0; nb < 8; ++nb)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) o[nb][e] = 0.f;
+      for (int j0 = 0; j0 < Sk16; j0 += 16) {
+        float s[2][4];
+        mma_a_yT(qa, sK, j0, lane, s);
+        uint4 rnd = make_uint4(0, 0, 0, 0);
+        if (p.drop_on) rnd = tile_rng(p, bh, q0 >> 4, j0 >> 4, Sq16 >> 4, Sk16 >> 4, lane);
+#pragma unroll
+        for (int nb = 0; nb < 2; ++nb)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int j = j0 + nb * 8 + 2 * (lane & 3) + e;
+            const float2 a = mask_add(p, madd[j], i0, j, madd[j], i1, j);
+            float p0 = __expf(s[nb][e] * p.scale + a.x - m0) * inv0;
+            float p1 = __expf(s[nb][2 + e] * p.scale + a.y - m1) * inv1;
+            if (p.drop_on) {
+              p0 = dropout(p, philox_u16(rnd, e | (nb << 2)), p0);
+              p1 = dropout(p, philox_u16(rnd, e | 2 | (nb << 2)), p1);
+            }
+            s[nb][e] = p0;
+            s[nb][2 + e] = p1;
+          }
+        uint32_t pa[4];
+        pack_a(s, pa);
+        mma_p_z(pa, sV, j0, lane, o);
+      }
     }
-    if (t == 0 && p.lse != nullptr) {
-      if (i0 < p.Sq) p.lse[VARLEN ? (ob + i0) * p.heads + h : bh * p.Sq + i0] = m0 + __logf(l0);
-      if (i1 < p.Sq) p.lse[VARLEN ? (ob + i1) * p.heads + h : bh * p.Sq + i1] = m1 + __logf(l1);
-    }
+    store_fwd_rows<ADDR>(p, vl, seq, h, q0, lane, o, m0, l0, m1, l1);
   }
 }
 
@@ -309,19 +208,14 @@ struct BwdSmem {
 template <bool SHARE>
 __device__ __forceinline__ void bwd_dq_task(const AttnParams& p, const BwdSmem& sm, int task, int lane, int seq, int h,
                                             long long bh, int Sq16, int Sk16) {
-  const bf16 *sQ = sm.sQ, *sdO = sm.sdO, *sK = sm.sK, *sV = sm.sV;
-  const float *madd = sm.madd, *sLse = sm.sLse, *sD = sm.sD;
-  bf16 *sP = sm.sP, *sdS = sm.sdS;
-  const int ldp = sm.ldp;
-  (void)sP; (void)sdS; (void)ldp;  // used only when SHARE
   // ---------------- dQ for 16 query rows ----------------
   const int q0 = task * 16;
   const int g = lane >> 2, t = lane & 3;
   uint32_t qa[4][4], da[4][4];
-  load_a_frags(sQ, q0, lane, qa);
-  load_a_frags(sdO, q0, lane, da);
+  load_a_frags(sm.sQ, q0, lane, qa);
+  load_a_frags(sm.sdO, q0, lane, da);
   const int i0 = q0 + g, i1 = q0 + g + 8;
-  const float lse0 = sLse[i0], lse1 = sLse[i1], D0 = sD[i0], D1 = sD[i1];
+  const float lse0 = sm.sLse[i0], lse1 = sm.sLse[i1], D0 = sm.sD[i0], D1 = sm.sD[i1];
   float acc[8][4];
 #pragma unroll
   for (int nb = 0; nb < 8; ++nb)
@@ -329,158 +223,70 @@ __device__ __forceinline__ void bwd_dq_task(const AttnParams& p, const BwdSmem& 
     for (int e = 0; e < 4; ++e) acc[nb][e] = 0.f;
   for (int j0 = 0; j0 < Sk16; j0 += 16) {
     float s[2][4], dp[2][4];
-    mma_a_yT(qa, sK, j0, lane, s);
-    mma_a_yT(da, sV, j0, lane, dp);
+    mma_a_yT(qa, sm.sK, j0, lane, s);
+    mma_a_yT(da, sm.sV, j0, lane, dp);
     uint4 rnd = make_uint4(0, 0, 0, 0);
     uint32_t rw[4] = {0, 0, 0, 0};
     if (p.drop_on) {
       if (p.rng_rowmajor) tile_rng_rowmajor(p, bh, q0, j0 >> 4, lane, rw);
       else rnd = tile_rng(p, bh, q0 >> 4, j0 >> 4, Sq16 >> 4, Sk16 >> 4, lane);
     }
+    scale_mask(p, sm.madd, j0, i0, i1, lane, s);
 #pragma unroll
     for (int nb = 0; nb < 2; ++nb) {
       const int jb = j0 + nb * 8 + 2 * t;
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
-        const int j = jb + e;
-        float ma = madd[j];
-        float a0 = ma, a1 = ma;
-        if (p.causal) {
-          if (j > i0 && a0 == 0.f) a0 = -10000.f;
-          if (j > i1 && a1 == 0.f) a1 = -10000.f;
-        }
-        const float p0 = __expf(s[nb][e] * p.scale + a0 - lse0);
-        const float p1 = __expf(s[nb][2 + e] * p.scale + a1 - lse1);
-        float g0 = dp[nb][e], g1 = dp[nb][2 + e];
-        float pk0 = p0, pk1 = p1;
-        if (p.drop_on) {
-          const uint32_t u0 = p.rng_rowmajor ? (e ? rw[nb] >> 16 : rw[nb] & 0xFFFFu) : philox_u16(rnd, e | (nb << 2));
-          const uint32_t u1 = p.rng_rowmajor ? (e ? rw[2 + nb] >> 16 : rw[2 + nb] & 0xFFFFu)
-                                             : philox_u16(rnd, e | 2 | (nb << 2));
-          const bool kp0 = u0 < p.drop_threshold;
-          const bool kp1 = u1 < p.drop_threshold;
-          g0 = kp0 ? g0 * p.drop_scale : 0.f;
-          g1 = kp1 ? g1 * p.drop_scale : 0.f;
-          pk0 = kp0 ? p0 * p.drop_scale : 0.f;
-          pk1 = kp1 ? p1 * p.drop_scale : 0.f;
-        }
-        s[nb][e] = p0 * (g0 - D0) * p.scale;
-        s[nb][2 + e] = p1 * (g1 - D1) * p.scale;
-        dp[nb][e] = pk0;  // dP is consumed: reuse its registers for the dropped probabilities
-        dp[nb][2 + e] = pk1;
+        const uint32_t u0 = p.rng_rowmajor ? (e ? rw[nb] >> 16 : rw[nb] & 0xFFFFu) : philox_u16(rnd, e | (nb << 2));
+        const uint32_t u1 = p.rng_rowmajor ? (e ? rw[2 + nb] >> 16 : rw[2 + nb] & 0xFFFFu)
+                                           : philox_u16(rnd, e | 2 | (nb << 2));
+        // dP is consumed: its registers take the dropped probabilities
+        bwd_pair(p, s[nb][e], s[nb][2 + e], dp[nb][e], dp[nb][2 + e], lse0, lse1, D0, D1, u0, u1);
       }
       if (SHARE) {
-        *reinterpret_cast<uint32_t*>(sP + i0 * ldp + jb) = pack_bf16x2(dp[nb][0], dp[nb][1]);
-        *reinterpret_cast<uint32_t*>(sP + i1 * ldp + jb) = pack_bf16x2(dp[nb][2], dp[nb][3]);
-        *reinterpret_cast<uint32_t*>(sdS + i0 * ldp + jb) = pack_bf16x2(s[nb][0], s[nb][1]);
-        *reinterpret_cast<uint32_t*>(sdS + i1 * ldp + jb) = pack_bf16x2(s[nb][2], s[nb][3]);
+        *reinterpret_cast<uint32_t*>(sm.sP + i0 * sm.ldp + jb) = pack_bf16x2(dp[nb][0], dp[nb][1]);
+        *reinterpret_cast<uint32_t*>(sm.sP + i1 * sm.ldp + jb) = pack_bf16x2(dp[nb][2], dp[nb][3]);
+        *reinterpret_cast<uint32_t*>(sm.sdS + i0 * sm.ldp + jb) = pack_bf16x2(s[nb][0], s[nb][1]);
+        *reinterpret_cast<uint32_t*>(sm.sdS + i1 * sm.ldp + jb) = pack_bf16x2(s[nb][2], s[nb][3]);
       }
     }
     uint32_t pa[4];
-    pa[0] = pack_bf16x2(s[0][0], s[0][1]);
-    pa[1] = pack_bf16x2(s[0][2], s[0][3]);
-    pa[2] = pack_bf16x2(s[1][0], s[1][1]);
-    pa[3] = pack_bf16x2(s[1][2], s[1][3]);
-    mma_p_z(pa, sK, j0, lane, acc);
+    pack_a(s, pa);
+    mma_p_z(pa, sm.sK, j0, lane, acc);
   }
   if (sm.csum != nullptr) tile_colsum(acc, sm.csum + task * 64, lane);
-  bf16* r0 = p.dq + ((long long)seq * p.Sq + i0) * p.lddq + h * HD;
-  bf16* r1 = p.dq + ((long long)seq * p.Sq + i1) * p.lddq + h * HD;
-#pragma unroll
-  for (int nb = 0; nb < 8; ++nb) {
-    if (i0 < p.Sq) *reinterpret_cast<uint32_t*>(r0 + nb * 8 + 2 * t) = pack_bf16x2(acc[nb][0], acc[nb][1]);
-    if (i1 < p.Sq) *reinterpret_cast<uint32_t*>(r1 + nb * 8 + 2 * t) = pack_bf16x2(acc[nb][2], acc[nb][3]);
+  store_rows(p.dq + h * HD, p.lddq, (long long)seq * p.Sq, q0, p.Sq, lane, acc);
+}
+
+// the key-major tasks' epilogue: bias-gradient column sums and the dK / dV rows of this task's 16 keys
+__device__ __forceinline__ void store_dkdv(const AttnParams& p, const BwdSmem& sm, int task, int lane, int seq, int h,
+                                           const float (&dk)[8][4], const float (&dv)[8][4]) {
+  if (sm.csum != nullptr) {
+    tile_colsum(dk, sm.csum + (sm.nQ + task) * 64, lane);
+    tile_colsum(dv, sm.csum + (sm.nQ + sm.nK + task) * 64, lane);
   }
+  store_rows(p.dk + h * HD, p.lddk, (long long)seq * p.Sk, task * 16, p.Sk, lane, dk);
+  store_rows(p.dv + h * HD, p.lddv, (long long)seq * p.Sk, task * 16, p.Sk, lane, dv);
 }
 
 // key-major pass that recomputes the transposed score / dP tiles (any S <= 256)
 __device__ __forceinline__ void bwd_dkdv_task_recompute(const AttnParams& p, const BwdSmem& sm, int task, int lane,
                                                         int seq, int h, long long bh, int Sq16, int Sk16) {
-  const bf16 *sQ = sm.sQ, *sdO = sm.sdO, *sK = sm.sK, *sV = sm.sV;
-  const float *madd = sm.madd, *sLse = sm.sLse, *sD = sm.sD;
   // ---------------- dK, dV for 16 key rows (transposed tiles) ----------------
   const int k0 = task * 16;
-  const int g = lane >> 2, t = lane & 3;
+  const int g = lane >> 2;
   uint32_t ka[4][4], va[4][4];
-  load_a_frags(sK, k0, lane, ka);
-  load_a_frags(sV, k0, lane, va);
-  const int j0r = k0 + g, j1r = k0 + g + 8;
-  const float ma0 = madd[j0r], ma1 = madd[j1r];
+  load_a_frags(sm.sK, k0, lane, ka);
+  load_a_frags(sm.sV, k0, lane, va);
+  const float ma0 = sm.madd[k0 + g], ma1 = sm.madd[k0 + g + 8];
   float dk[8][4], dv[8][4];
 #pragma unroll
   for (int nb = 0; nb < 8; ++nb)
 #pragma unroll
     for (int e = 0; e < 4; ++e) dk[nb][e] = dv[nb][e] = 0.f;
-  for (int q0 = 0; q0 < Sq16; q0 += 16) {
-    float st[2][4], dpt[2][4];
-    mma_a_yT(ka, sQ, q0, lane, st);    // S^T tile: rows = keys, cols = queries
-    mma_a_yT(va, sdO, q0, lane, dpt);  // dP^T tile
-    float pd[2][4];
-    uint4 rnd[2] = {make_uint4(0, 0, 0, 0), make_uint4(0, 0, 0, 0)};
-    if (p.drop_on) {
-      rnd[0] = tile_rng(p, bh, q0 >> 4, k0 >> 4, Sq16 >> 4, Sk16 >> 4, ((2 * t) << 2) | (g >> 1));
-      rnd[1] = tile_rng(p, bh, q0 >> 4, k0 >> 4, Sq16 >> 4, Sk16 >> 4, ((2 * t + 1) << 2) | (g >> 1));
-    }
-#pragma unroll
-    for (int nb = 0; nb < 2; ++nb)
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int i = q0 + nb * 8 + 2 * t + e;
-        const float lse = sLse[i], D = sD[i];
-        float a0 = ma0, a1 = ma1;
-        if (p.causal) {
-          if (j0r > i && a0 == 0.f) a0 = -10000.f;
-          if (j1r > i && a1 == 0.f) a1 = -10000.f;
-        }
-        const float p0 = __expf(st[nb][e] * p.scale + a0 - lse);
-        const float p1 = __expf(st[nb][2 + e] * p.scale + a1 - lse);
-        float g0 = dpt[nb][e], g1 = dpt[nb][2 + e];
-        float pk0 = p0, pk1 = p1;
-        if (p.drop_on) {
-          // element (query i, key j): word (j & 1) | ((i >> 3) & 1) << 1 | ((j >> 3) & 1) << 2 ; j = g (+8)
-          const bool kp0 = philox_u16(rnd[e], (g & 1) | (nb << 1)) < p.drop_threshold;
-          const bool kp1 = philox_u16(rnd[e], (g & 1) | (nb << 1) | 4) < p.drop_threshold;
-          g0 = kp0 ? g0 * p.drop_scale : 0.f;
-          g1 = kp1 ? g1 * p.drop_scale : 0.f;
-          pk0 = kp0 ? p0 * p.drop_scale : 0.f;
-          pk1 = kp1 ? p1 * p.drop_scale : 0.f;
-        }
-        pd[nb][e] = pk0;
-        pd[nb][2 + e] = pk1;
-        st[nb][e] = p0 * (g0 - D) * p.scale;
-        st[nb][2 + e] = p1 * (g1 - D) * p.scale;
-      }
-    uint32_t pa[4], sa[4];
-    pa[0] = pack_bf16x2(pd[0][0], pd[0][1]);
-    pa[1] = pack_bf16x2(pd[0][2], pd[0][3]);
-    pa[2] = pack_bf16x2(pd[1][0], pd[1][1]);
-    pa[3] = pack_bf16x2(pd[1][2], pd[1][3]);
-    sa[0] = pack_bf16x2(st[0][0], st[0][1]);
-    sa[1] = pack_bf16x2(st[0][2], st[0][3]);
-    sa[2] = pack_bf16x2(st[1][0], st[1][1]);
-    sa[3] = pack_bf16x2(st[1][2], st[1][3]);
-    mma_p_z(pa, sdO, q0, lane, dv);
-    mma_p_z(sa, sQ, q0, lane, dk);
-  }
-  if (sm.csum != nullptr) {
-    tile_colsum(dk, sm.csum + (sm.nQ + task) * 64, lane);
-    tile_colsum(dv, sm.csum + (sm.nQ + sm.nK + task) * 64, lane);
-  }
-  bf16* kr0 = p.dk + ((long long)seq * p.Sk + j0r) * p.lddk + h * HD;
-  bf16* kr1 = p.dk + ((long long)seq * p.Sk + j1r) * p.lddk + h * HD;
-  bf16* vr0 = p.dv + ((long long)seq * p.Sk + j0r) * p.lddv + h * HD;
-  bf16* vr1 = p.dv + ((long long)seq * p.Sk + j1r) * p.lddv + h * HD;
-#pragma unroll
-  for (int nb = 0; nb < 8; ++nb) {
-    if (j0r < p.Sk) {
-      *reinterpret_cast<uint32_t*>(kr0 + nb * 8 + 2 * t) = pack_bf16x2(dk[nb][0], dk[nb][1]);
-      *reinterpret_cast<uint32_t*>(vr0 + nb * 8 + 2 * t) = pack_bf16x2(dv[nb][0], dv[nb][1]);
-    }
-    if (j1r < p.Sk) {
-      *reinterpret_cast<uint32_t*>(kr1 + nb * 8 + 2 * t) = pack_bf16x2(dk[nb][2], dk[nb][3]);
-      *reinterpret_cast<uint32_t*>(vr1 + nb * 8 + 2 * t) = pack_bf16x2(dv[nb][2], dv[nb][3]);
-    }
-  }
+  for (int q0 = 0; q0 < Sq16; q0 += 16)
+    dkdv_tile(p, ka, va, ma0, ma1, k0, sm.sQ, sm.sdO, sm.sLse, sm.sD, q0, q0, bh, Sq16 >> 4, Sk16 >> 4, lane, dk, dv);
+  store_dkdv(p, sm, task, lane, seq, h, dk, dv);
 }
 
 // key-major pass on the tiles the query-major pass left in shared memory: dV = P_drop^T dO, dK = dS^T Q.  The A
@@ -488,7 +294,6 @@ __device__ __forceinline__ void bwd_dkdv_task_recompute(const AttnParams& p, con
 __device__ __forceinline__ void bwd_dkdv_task_shared(const AttnParams& p, const BwdSmem& sm, int task, int lane, int seq,
                                                      int h, int Sq16) {
   const int k0 = task * 16;
-  const int g = lane >> 2, t = lane & 3;
   float dk[8][4], dv[8][4];
 #pragma unroll
   for (int nb = 0; nb < 8; ++nb)
@@ -504,26 +309,7 @@ __device__ __forceinline__ void bwd_dkdv_task_shared(const AttnParams& p, const 
     mma_p_z(pa, sm.sdO, q0, lane, dv);
     mma_p_z(sa, sm.sQ, q0, lane, dk);
   }
-  const int j0r = k0 + g, j1r = k0 + g + 8;
-  if (sm.csum != nullptr) {
-    tile_colsum(dk, sm.csum + (sm.nQ + task) * 64, lane);
-    tile_colsum(dv, sm.csum + (sm.nQ + sm.nK + task) * 64, lane);
-  }
-  bf16* kr0 = p.dk + ((long long)seq * p.Sk + j0r) * p.lddk + h * HD;
-  bf16* kr1 = p.dk + ((long long)seq * p.Sk + j1r) * p.lddk + h * HD;
-  bf16* vr0 = p.dv + ((long long)seq * p.Sk + j0r) * p.lddv + h * HD;
-  bf16* vr1 = p.dv + ((long long)seq * p.Sk + j1r) * p.lddv + h * HD;
-#pragma unroll
-  for (int nb = 0; nb < 8; ++nb) {
-    if (j0r < p.Sk) {
-      *reinterpret_cast<uint32_t*>(kr0 + nb * 8 + 2 * t) = pack_bf16x2(dk[nb][0], dk[nb][1]);
-      *reinterpret_cast<uint32_t*>(vr0 + nb * 8 + 2 * t) = pack_bf16x2(dv[nb][0], dv[nb][1]);
-    }
-    if (j1r < p.Sk) {
-      *reinterpret_cast<uint32_t*>(kr1 + nb * 8 + 2 * t) = pack_bf16x2(dk[nb][2], dk[nb][3]);
-      *reinterpret_cast<uint32_t*>(vr1 + nb * 8 + 2 * t) = pack_bf16x2(dv[nb][2], dv[nb][3]);
-    }
-  }
+  store_dkdv(p, sm, task, lane, seq, h, dk, dv);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -533,11 +319,7 @@ __global__ void __launch_bounds__(ATT_BWD_WARPS * 32)
 attention_bwd_kernel(const AttnParams p_in) {
   pdl_trigger();
   pdl_wait();
-  AttnParams p = p_in;
-  if (p.drop_on && p.rng != nullptr) {
-    p.seed = p.rng[0];
-    p.stream += p.rng[1] << 20;
-  }
+  AttnParams p = resolve_rng(p_in);
   extern __shared__ __align__(16) uint8_t smem_att[];
   const int Sq16 = (p.Sq + 15) & ~15, Sk16 = (p.Sk + 15) & ~15;
   bf16* sQ = reinterpret_cast<bf16*>(smem_att);
@@ -552,37 +334,15 @@ attention_bwd_kernel(const AttnParams p_in) {
   const int seq = blockIdx.x / p.heads, h = blockIdx.x % p.heads;
   const long long bh = blockIdx.x;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  (void)lane;
 
-  load_head_tile(sQ, p.q + (long long)seq * p.Sq * p.ldq + h * HD, p.ldq, p.Sq, Sq16);
-  load_head_tile(sdO, p.d_o + (long long)seq * p.Sq * p.lddo + h * HD, p.lddo, p.Sq, Sq16);
-  load_head_tile(sK, p.k + (long long)seq * p.Sk * p.ldk + h * HD, p.ldk, p.Sk, Sk16);
-  load_head_tile(sV, p.v + (long long)seq * p.Sk * p.ldv + h * HD, p.ldv, p.Sk, Sk16);
+  load_rows<ADDR_DENSE, OP_Q>(sQ, p, {}, {}, seq, h, 0, p.Sq, Sq16);
+  load_rows<ADDR_DENSE, OP_DO>(sdO, p, {}, {}, seq, h, 0, p.Sq, Sq16);
+  load_rows<ADDR_DENSE, OP_K>(sK, p, {}, {}, seq, h, 0, p.Sk, Sk16);
+  load_rows<ADDR_DENSE, OP_V>(sV, p, {}, {}, seq, h, 0, p.Sk, Sk16);
   build_key_mask(madd, p, seq, Sk16);
   cp_async_wait_all();
   __syncthreads();
-  // D_i = sum_d dO[i,d] * O[i,d]   (8 lanes per row, 8 dims each); LSE rows (+inf on padding -> P = 0)
-  for (int idx = threadIdx.x; idx < Sq16 * 8; idx += blockDim.x) {
-    const int r = idx >> 3, c = idx & 7;
-    float part = 0.f;
-    if (r < p.Sq) {
-      const uint4 uo = *reinterpret_cast<const uint4*>(p.o + ((long long)seq * p.Sq + r) * p.ldo + h * HD + c * 8);
-      const uint4 ud = *reinterpret_cast<const uint4*>(sdO + r * LDS + c * 8);
-      const uint32_t wo[4] = {uo.x, uo.y, uo.z, uo.w}, wd[4] = {ud.x, ud.y, ud.z, ud.w};
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 a = unpack_bf16x2(wo[j]), b = unpack_bf16x2(wd[j]);
-        part += a.x * b.x + a.y * b.y;
-      }
-    }
-    part += __shfl_xor_sync(0xffffffffu, part, 1);
-    part += __shfl_xor_sync(0xffffffffu, part, 2);
-    part += __shfl_xor_sync(0xffffffffu, part, 4);
-    if (c == 0) {
-      sD[r] = part;
-      sLse[r] = r < p.Sq ? p.lse[bh * p.Sq + r] : INFINITY;
-    }
-  }
+  stage_d_lse(p, sdO, seq, h, bh, 0, p.Sq, Sq16, sD, sLse, nullptr);
   __syncthreads();
 
   const int nQ = Sq16 >> 4, nK = Sk16 >> 4;
@@ -615,22 +375,16 @@ attention_bwd_kernel(const AttnParams p_in) {
   }
 }
 
-template <int ADDR>
-static void (*fwd_kernel_for(int nkb))(const AttnParams, const PairSrc, const VarlenSrc) {
-  return nkb <= 3 ? attention_fwd_kernel<3, ADDR>
-         : nkb <= 6 ? attention_fwd_kernel<6, ADDR>
-         : nkb <= 8 ? attention_fwd_kernel<8, ADDR> : attention_fwd_kernel<0, ADDR>;
-}
-
 int attention_fwd_launch(const AttnParams& p, Addr addr, const PairSrc& pb, const VarlenSrc& vl, cudaStream_t stream) {
   const int Sq16 = (p.Sq + 15) & ~15, Sk16 = (p.Sk + 15) & ~15;
   const size_t smem = (size_t)(Sq16 + 2 * Sk16) * LDS * 2 + (size_t)Sk16 * 4;
   const int nkb = Sk16 / 16;
-  void (*kern)(const AttnParams, const PairSrc, const VarlenSrc) =
-      addr == ADDR_PAIR ? fwd_kernel_for<ADDR_PAIR>(nkb)
-      : addr == ADDR_PAIR_LIST ? fwd_kernel_for<ADDR_PAIR_LIST>(nkb)
-      : addr == ADDR_VARLEN_PAIR ? fwd_kernel_for<ADDR_VARLEN_PAIR>(nkb)
-      : addr == ADDR_VARLEN_PACKED ? fwd_kernel_for<ADDR_VARLEN_PACKED>(nkb) : fwd_kernel_for<ADDR_DENSE>(nkb);
+  const FwdKernel kern = with_addr(addr, [nkb](auto addr_c) -> FwdKernel {
+    constexpr int ADDR = decltype(addr_c)::value;
+    return nkb <= 3 ? attention_fwd_kernel<3, ADDR>
+           : nkb <= 6 ? attention_fwd_kernel<6, ADDR>
+           : nkb <= 8 ? attention_fwd_kernel<8, ADDR> : attention_fwd_kernel<0, ADDR>;
+  });
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "attention_fwd smem attribute: %s", cudaGetErrorString(e));
   // warps per CTA: one per 16-row task up to 3, else two tasks per warp — smaller CTAs, more of them resident per SM, so
@@ -638,14 +392,6 @@ int attention_fwd_launch(const AttnParams& p, Addr addr, const PairSrc& pb, cons
   const int fwd_tasks = Sq16 / 16;
   int fwd_warps = fwd_tasks <= 3 ? fwd_tasks : (fwd_tasks + 1) / 2;
   if (fwd_warps > ATT_FWD_WARPS) fwd_warps = ATT_FWD_WARPS;
-  {
-    static int cap = -1;  // tuning: UNIVL_ATT_FWD_WARPS=n caps the warps per CTA (more, smaller CTAs per SM)
-    if (cap < 0) {
-      const char* e = getenv("UNIVL_ATT_FWD_WARPS");
-      cap = e ? atoi(e) : 0;
-    }
-    if (cap > 0 && fwd_warps > cap) fwd_warps = cap;
-  }
   launch_kernel(kern, dim3(p.n_seq * p.heads), dim3(fwd_warps * 32), smem, stream, p, pb, vl);
   UNIVL_CHECK_LAUNCH("attention_fwd");
   return UNIVL_OK;

@@ -36,29 +36,6 @@ __device__ __forceinline__ void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
 
-__device__ __forceinline__ void resolve_rng(AttnParams& p) {
-  if (p.drop_on && p.rng != nullptr) {
-    p.seed = p.rng[0];
-    p.stream += p.rng[1] << 20;
-  }
-}
-
-// additive mask of (query i, key j): the key's padding mask, or -10000 once for a future key of a causal row
-__device__ __forceinline__ float mask_add(const AttnParams& p, float ma, int i, int j) {
-  return (p.causal && j > i && ma == 0.f) ? -10000.f : ma;
-}
-
-// store a warp's 16 x 64 accumulator (fragment rows r0 + g and r0 + g + 8) as bf16 into base[row * ld + col], rows < `rows`
-__device__ __forceinline__ void store_rows(bf16* base, long long ld, int r0, int rows, int lane, const float (&acc)[8][4]) {
-  const int g = lane >> 2, t = lane & 3;
-  const int i0 = r0 + g, i1 = i0 + 8;
-#pragma unroll
-  for (int nb = 0; nb < 8; ++nb) {
-    if (i0 < rows) *reinterpret_cast<uint32_t*>(base + i0 * ld + nb * 8 + 2 * t) = pack_bf16x2(acc[nb][0], acc[nb][1]);
-    if (i1 < rows) *reinterpret_cast<uint32_t*>(base + i1 * ld + nb * 8 + 2 * t) = pack_bf16x2(acc[nb][2], acc[nb][3]);
-  }
-}
-
 // this CTA's partial bias-gradient row: the sum of its warps' column-sum slots in warp order
 __device__ __forceinline__ void write_partial_row(const float* slots, int nwarps, float* dst) {
   for (int col = threadIdx.x; col < HD; col += blockDim.x) {
@@ -78,16 +55,12 @@ __global__ void __launch_bounds__(LONG_WARPS * 32)
 attention_long_fwd_kernel(const AttnParams p_in, const PairSrc pb, const VarlenSrc vl) {
   pdl_trigger();
   pdl_wait();
-  AttnParams p = p_in;
-  resolve_rng(p);
-  constexpr bool VARLEN = ADDR == ADDR_VARLEN_PAIR || ADDR == ADDR_VARLEN_PACKED;
+  AttnParams p = resolve_rng(p_in);
   const int seq = blockIdx.x / p.heads, h = blockIdx.x % p.heads;
   const long long bh = blockIdx.x;
   const int qbase = blockIdx.y * LB;
-  if constexpr (VARLEN) {
-    varlen_shape(p, vl, seq);
-    if (p.Sk <= 0 || qbase >= p.Sq) return;  // the whole CTA leaves before any barrier
-  }
+  // under the varlen addressings a CTA may have no query rows; the whole CTA leaves before any barrier
+  if (!seq_shape<ADDR>(p, vl, seq) || qbase >= p.Sq) return;
   extern __shared__ __align__(16) uint8_t smem_att[];
   const int Sq16 = (p.Sq + 15) & ~15, Sk16 = (p.Sk + 15) & ~15;
   bf16* sQ = reinterpret_cast<bf16*>(smem_att);                 // [LB][LDS]
@@ -95,28 +68,17 @@ attention_long_fwd_kernel(const AttnParams p_in, const PairSrc pb, const VarlenS
   float* madd = reinterpret_cast<float*>(sKV + 4 * LT * LDS);  // [Sk16]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int g = lane >> 2, t = lane & 3;
+  const int g = lane >> 2;
   const int qrows = min(LB, p.Sq - qbase), qrows16 = min(LB, Sq16 - qbase);
   const int nT = (Sk16 + LT - 1) / LT;
 
   auto load_kv = [&](int tile, int stage) {
     const int k0 = tile * LT;
     bf16* sK = sKV + stage * 2 * LT * LDS;
-    if constexpr (VARLEN) {
-      load_varlen_tile(sK, p.k, p.ldk, pb.k, pb.ldk, vl, seq, h, k0, min(LT, p.Sk - k0), LT);
-      load_varlen_tile(sK + LT * LDS, p.v, p.ldv, pb.v, pb.ldv, vl, seq, h, k0, min(LT, p.Sk - k0), LT);
-    } else if constexpr (ADDR == ADDR_PAIR || ADDR == ADDR_PAIR_LIST) {
-      load_pair_tile<ADDR>(sK, p.k, p.ldk, pb.k, pb.ldk, p, vl, seq, h, k0, min(LT, p.Sk - k0), LT);
-      load_pair_tile<ADDR>(sK + LT * LDS, p.v, p.ldv, pb.v, pb.ldv, p, vl, seq, h, k0, min(LT, p.Sk - k0), LT);
-    } else {
-      load_head_tile(sK, p.k + ((long long)seq * p.Sk + k0) * p.ldk + h * HD, p.ldk, min(LT, p.Sk - k0), LT);
-      load_head_tile(sK + LT * LDS, p.v + ((long long)seq * p.Sk + k0) * p.ldv + h * HD, p.ldv, min(LT, p.Sk - k0), LT);
-    }
+    load_rows<ADDR, OP_K>(sK, p, pb, vl, seq, h, k0, min(LT, p.Sk - k0), LT);
+    load_rows<ADDR, OP_V>(sK + LT * LDS, p, pb, vl, seq, h, k0, min(LT, p.Sk - k0), LT);
   };
-  if constexpr (VARLEN) load_varlen_q(sQ, p.q, p.ldq, pb.q, pb.ldq, vl, seq, h, qbase, qrows, qrows16);
-  else if constexpr (ADDR == ADDR_PAIR || ADDR == ADDR_PAIR_LIST)
-    load_pair_tile<ADDR>(sQ, p.q, p.ldq, pb.q, pb.ldq, p, vl, seq, h, qbase, qrows, qrows16);
-  else load_head_tile(sQ, p.q + ((long long)seq * p.Sq + qbase) * p.ldq + h * HD, p.ldq, qrows, qrows16);
+  load_rows<ADDR, OP_Q>(sQ, p, pb, vl, seq, h, qbase, qrows, qrows16);
   build_key_mask(madd, p, seq, Sk16);
   load_kv(0, 0);
   cp_async_commit();
@@ -155,24 +117,11 @@ attention_long_fwd_kernel(const AttnParams p_in, const PairSrc pb, const VarlenS
 #pragma unroll
       for (int kb = 0; kb < LT / 16; ++kb)
         if (kb < nkb) {
-#pragma unroll
-          for (int nb = 0; nb < 2; ++nb)
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              const int j = k0 + kb * 16 + nb * 8 + 2 * t + e;
-              const float ma = madd[j];
-              s[kb][nb][e] = s[kb][nb][e] * p.scale + mask_add(p, ma, i0, j);
-              s[kb][nb][2 + e] = s[kb][nb][2 + e] * p.scale + mask_add(p, ma, i1, j);
-              cm0 = fmaxf(cm0, s[kb][nb][e]);
-              cm1 = fmaxf(cm1, s[kb][nb][2 + e]);
-            }
+          scale_mask(p, madd, k0 + kb * 16, i0, i1, lane, s[kb]);
+          row_max(s[kb], cm0, cm1);
         }
-      cm0 = fmaxf(cm0, __shfl_xor_sync(0xffffffffu, cm0, 1));
-      cm0 = fmaxf(cm0, __shfl_xor_sync(0xffffffffu, cm0, 2));
-      cm1 = fmaxf(cm1, __shfl_xor_sync(0xffffffffu, cm1, 1));
-      cm1 = fmaxf(cm1, __shfl_xor_sync(0xffffffffu, cm1, 2));
       // every processed 16-key block holds a real key, so the running max is finite after the first tile
-      const float n0 = fmaxf(m0, cm0), n1 = fmaxf(m1, cm1);
+      const float n0 = fmaxf(m0, quad_max(cm0)), n1 = fmaxf(m1, quad_max(cm1));
       const float c0 = __expf(m0 - n0), c1 = __expf(m1 - n1);
       m0 = n0;
       m1 = n1;
@@ -198,27 +147,22 @@ attention_long_fwd_kernel(const AttnParams p_in, const PairSrc pb, const VarlenS
               l0 += p0;
               l1 += p1;
               if (p.drop_on) {
-                p0 = philox_u16(rnd, e | (nb << 2)) < p.drop_threshold ? p0 * p.drop_scale : 0.f;
-                p1 = philox_u16(rnd, e | 2 | (nb << 2)) < p.drop_threshold ? p1 * p.drop_scale : 0.f;
+                p0 = dropout(p, philox_u16(rnd, e | (nb << 2)), p0);
+                p1 = dropout(p, philox_u16(rnd, e | 2 | (nb << 2)), p1);
               }
               s[kb][nb][e] = p0;
               s[kb][nb][2 + e] = p1;
             }
           uint32_t pa[4];
-          pa[0] = pack_bf16x2(s[kb][0][0], s[kb][0][1]);
-          pa[1] = pack_bf16x2(s[kb][0][2], s[kb][0][3]);
-          pa[2] = pack_bf16x2(s[kb][1][0], s[kb][1][1]);
-          pa[3] = pack_bf16x2(s[kb][1][2], s[kb][1][3]);
+          pack_a(s[kb], pa);
           mma_p_z(pa, sV, kb * 16, lane, o);
         }
     }
     __syncthreads();  // the next iteration refills this stage
   }
   if (!active) return;
-  l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
-  l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
-  l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
-  l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+  l0 = quad_sum(l0);
+  l1 = quad_sum(l1);
   const float r0 = 1.0f / l0, r1 = 1.0f / l1;
 #pragma unroll
   for (int nb = 0; nb < 8; ++nb) {
@@ -227,13 +171,7 @@ attention_long_fwd_kernel(const AttnParams p_in, const PairSrc pb, const VarlenS
     o[nb][2] *= r1;
     o[nb][3] *= r1;
   }
-  const long long obase = VARLEN ? varlen_out_row(vl, seq) : (long long)seq * p.Sq;  // output row of query 0
-  store_rows(p.o + (obase + qbase) * p.ldo + h * HD, p.ldo, warp * 16, qrows, lane, o);
-  if (t == 0 && p.lse != nullptr) {
-    // lse: [n_seq, heads, Sq], or [rows, heads] under the varlen addressings
-    if (i0 < p.Sq) p.lse[VARLEN ? (obase + i0) * p.heads + h : bh * p.Sq + i0] = m0 + __logf(l0);
-    if (i1 < p.Sq) p.lse[VARLEN ? (obase + i1) * p.heads + h : bh * p.Sq + i1] = m1 + __logf(l1);
-  }
+  store_fwd_rows<ADDR>(p, vl, seq, h, q0, lane, o, m0, l0, m1, l1);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -243,8 +181,7 @@ __global__ void __launch_bounds__(LONG_WARPS * 32)
 attention_long_bwd_dq_kernel(const AttnParams p_in, float* __restrict__ Dg, float* __restrict__ part_q) {
   pdl_trigger();
   pdl_wait();
-  AttnParams p = p_in;
-  resolve_rng(p);
+  AttnParams p = resolve_rng(p_in);
   extern __shared__ __align__(16) uint8_t smem_att[];
   const int Sq16 = (p.Sq + 15) & ~15, Sk16 = (p.Sk + 15) & ~15;
   bf16* sQ = reinterpret_cast<bf16*>(smem_att);                 // [LB][LDS]
@@ -259,48 +196,25 @@ attention_long_bwd_dq_kernel(const AttnParams p_in, float* __restrict__ Dg, floa
   const long long bh = blockIdx.x;
   const int qbase = blockIdx.y * LB;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int g = lane >> 2, t = lane & 3;
+  const int g = lane >> 2;
   const int qrows = min(LB, p.Sq - qbase), qrows16 = min(LB, Sq16 - qbase);
   const int nT = (Sk16 + LT - 1) / LT;
 
   auto load_kv = [&](int tile, int stage) {
     const int k0 = tile * LT;
     bf16* sK = sKV + stage * 2 * LT * LDS;
-    load_head_tile(sK, p.k + ((long long)seq * p.Sk + k0) * p.ldk + h * HD, p.ldk, min(LT, p.Sk - k0), LT);
-    load_head_tile(sK + LT * LDS, p.v + ((long long)seq * p.Sk + k0) * p.ldv + h * HD, p.ldv, min(LT, p.Sk - k0), LT);
+    load_rows<ADDR_DENSE, OP_K>(sK, p, {}, {}, seq, h, k0, min(LT, p.Sk - k0), LT);
+    load_rows<ADDR_DENSE, OP_V>(sK + LT * LDS, p, {}, {}, seq, h, k0, min(LT, p.Sk - k0), LT);
   };
-  load_head_tile(sQ, p.q + ((long long)seq * p.Sq + qbase) * p.ldq + h * HD, p.ldq, qrows, qrows16);
-  load_head_tile(sdO, p.d_o + ((long long)seq * p.Sq + qbase) * p.lddo + h * HD, p.lddo, qrows, qrows16);
+  load_rows<ADDR_DENSE, OP_Q>(sQ, p, {}, {}, seq, h, qbase, qrows, qrows16);
+  load_rows<ADDR_DENSE, OP_DO>(sdO, p, {}, {}, seq, h, qbase, qrows, qrows16);
   cp_async_commit();
   load_kv(0, 0);
   cp_async_commit();
   build_key_mask(madd, p, seq, Sk16);
   cp_async_wait<1>();
   __syncthreads();
-  // D_i (8 lanes per row, 8 dims each) and the LSE rows (+inf past Sq -> P = 0), as attention.cu computes them
-  for (int idx = threadIdx.x; idx < qrows16 * 8; idx += blockDim.x) {
-    const int r = idx >> 3, c = idx & 7;
-    float part = 0.f;
-    if (r < qrows) {
-      const uint4 uo =
-          *reinterpret_cast<const uint4*>(p.o + ((long long)seq * p.Sq + qbase + r) * p.ldo + h * HD + c * 8);
-      const uint4 ud = *reinterpret_cast<const uint4*>(sdO + r * LDS + c * 8);
-      const uint32_t wo[4] = {uo.x, uo.y, uo.z, uo.w}, wd[4] = {ud.x, ud.y, ud.z, ud.w};
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 a = unpack_bf16x2(wo[j]), b = unpack_bf16x2(wd[j]);
-        part += a.x * b.x + a.y * b.y;
-      }
-    }
-    part += __shfl_xor_sync(0xffffffffu, part, 1);
-    part += __shfl_xor_sync(0xffffffffu, part, 2);
-    part += __shfl_xor_sync(0xffffffffu, part, 4);
-    if (c == 0) {
-      sD[r] = part;
-      sLse[r] = r < qrows ? p.lse[bh * p.Sq + qbase + r] : INFINITY;
-      if (r < qrows) Dg[bh * p.Sq + qbase + r] = part;
-    }
-  }
+  stage_d_lse(p, sdO, seq, h, bh, qbase, qrows, qrows16, sD, sLse, Dg);
 
   const int q0 = qbase + warp * 16;
   const bool active = warp * 16 < qrows16;
@@ -341,27 +255,15 @@ attention_long_bwd_dq_kernel(const AttnParams p_in, float* __restrict__ Dg, floa
         mma_a_yT(da, sV, kb * 16, lane, dp);
         uint4 rnd = make_uint4(0, 0, 0, 0);
         if (p.drop_on) rnd = tile_rng(p, bh, q0 >> 4, (k0 >> 4) + kb, Sq16 >> 4, Sk16 >> 4, lane);
+        scale_mask(p, madd, k0 + kb * 16, i0, i1, lane, s);
 #pragma unroll
         for (int nb = 0; nb < 2; ++nb)
 #pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int j = k0 + kb * 16 + nb * 8 + 2 * t + e;
-            const float ma = madd[j];
-            const float p0 = __expf(s[nb][e] * p.scale + mask_add(p, ma, i0, j) - lse0);
-            const float p1 = __expf(s[nb][2 + e] * p.scale + mask_add(p, ma, i1, j) - lse1);
-            float g0 = dp[nb][e], g1 = dp[nb][2 + e];
-            if (p.drop_on) {
-              g0 = philox_u16(rnd, e | (nb << 2)) < p.drop_threshold ? g0 * p.drop_scale : 0.f;
-              g1 = philox_u16(rnd, e | 2 | (nb << 2)) < p.drop_threshold ? g1 * p.drop_scale : 0.f;
-            }
-            s[nb][e] = p0 * (g0 - D0) * p.scale;
-            s[nb][2 + e] = p1 * (g1 - D1) * p.scale;
-          }
+          for (int e = 0; e < 2; ++e)
+            bwd_pair(p, s[nb][e], s[nb][2 + e], dp[nb][e], dp[nb][2 + e], lse0, lse1, D0, D1,
+                     philox_u16(rnd, e | (nb << 2)), philox_u16(rnd, e | 2 | (nb << 2)));
         uint32_t pa[4];
-        pa[0] = pack_bf16x2(s[0][0], s[0][1]);
-        pa[1] = pack_bf16x2(s[0][2], s[0][3]);
-        pa[2] = pack_bf16x2(s[1][0], s[1][1]);
-        pa[3] = pack_bf16x2(s[1][2], s[1][3]);
+        pack_a(s, pa);
         mma_p_z(pa, sK, kb * 16, lane, acc);
       }
     }
@@ -370,7 +272,7 @@ attention_long_bwd_dq_kernel(const AttnParams p_in, float* __restrict__ Dg, floa
   const int nw = (int)(blockDim.x >> 5);
   if (active) {
     if (part_q != nullptr) tile_colsum(acc, csum + warp * HD, lane);
-    store_rows(p.dq + ((long long)seq * p.Sq + qbase) * p.lddq + h * HD, p.lddq, warp * 16, qrows, lane, acc);
+    store_rows(p.dq + h * HD, p.lddq, (long long)seq * p.Sq + qbase, warp * 16, qrows, lane, acc);
   }
   if (part_q != nullptr) {
     __syncthreads();
@@ -387,8 +289,7 @@ attention_long_bwd_dkdv_kernel(const AttnParams p_in, const float* __restrict__ 
                                float* __restrict__ part_v) {
   pdl_trigger();
   pdl_wait();
-  AttnParams p = p_in;
-  resolve_rng(p);
+  AttnParams p = resolve_rng(p_in);
   extern __shared__ __align__(16) uint8_t smem_att[];
   const int Sq16 = (p.Sq + 15) & ~15, Sk16 = (p.Sk + 15) & ~15;
   bf16* sK = reinterpret_cast<bf16*>(smem_att);                 // [LB][LDS]
@@ -402,7 +303,7 @@ attention_long_bwd_dkdv_kernel(const AttnParams p_in, const float* __restrict__ 
   const long long bh = blockIdx.x;
   const int kbase = blockIdx.y * LB;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int g = lane >> 2, t = lane & 3;
+  const int g = lane >> 2;
   const int krows = min(LB, p.Sk - kbase), krows16 = min(LB, Sk16 - kbase);
   const int nT = (Sq16 + LT - 1) / LT;
 
@@ -410,23 +311,22 @@ attention_long_bwd_dkdv_kernel(const AttnParams p_in, const float* __restrict__ 
     const int q0 = tile * LT;
     const int rows = min(LT, p.Sq - q0);
     bf16* sQ = sQdO + stage * 2 * LT * LDS;
-    load_head_tile(sQ, p.q + ((long long)seq * p.Sq + q0) * p.ldq + h * HD, p.ldq, rows, LT);
-    load_head_tile(sQ + LT * LDS, p.d_o + ((long long)seq * p.Sq + q0) * p.lddo + h * HD, p.lddo, rows, LT);
+    load_rows<ADDR_DENSE, OP_Q>(sQ, p, {}, {}, seq, h, q0, rows, LT);
+    load_rows<ADDR_DENSE, OP_DO>(sQ + LT * LDS, p, {}, {}, seq, h, q0, rows, LT);
     float* ld = sLD + stage * 2 * LT;
     for (int r = threadIdx.x; r < LT; r += blockDim.x) {
       ld[r] = r < rows ? p.lse[bh * p.Sq + q0 + r] : INFINITY;  // +inf: P = 0 on the padding rows
       ld[LT + r] = r < rows ? Dg[bh * p.Sq + q0 + r] : 0.f;
     }
   };
-  load_head_tile(sK, p.k + ((long long)seq * p.Sk + kbase) * p.ldk + h * HD, p.ldk, krows, krows16);
-  load_head_tile(sV, p.v + ((long long)seq * p.Sk + kbase) * p.ldv + h * HD, p.ldv, krows, krows16);
+  load_rows<ADDR_DENSE, OP_K>(sK, p, {}, {}, seq, h, kbase, krows, krows16);
+  load_rows<ADDR_DENSE, OP_V>(sV, p, {}, {}, seq, h, kbase, krows, krows16);
   build_key_mask(madd, p, seq, Sk16);
   load_qdo(0, 0);
   cp_async_commit();
 
   const int k0 = kbase + warp * 16;  // this warp's first key row
   const bool active = warp * 16 < krows16;
-  const int j0r = k0 + g, j1r = j0r + 8;
   uint32_t ka[4][4], va[4][4];
   float dk[8][4], dv[8][4];
 #pragma unroll
@@ -448,8 +348,8 @@ attention_long_bwd_dkdv_kernel(const AttnParams p_in, const float* __restrict__ 
       if (tile == 0) {
         load_a_frags(sK, warp * 16, lane, ka);
         load_a_frags(sV, warp * 16, lane, va);
-        ma0 = madd[j0r];
-        ma1 = madd[j1r];
+        ma0 = madd[k0 + g];
+        ma1 = madd[k0 + g + 8];
       }
       const bf16* sQ = sQdO + (tile & 1) * 2 * LT * LDS;
       const bf16* sdO = sQ + LT * LDS;
@@ -457,53 +357,9 @@ attention_long_bwd_dkdv_kernel(const AttnParams p_in, const float* __restrict__ 
       const float* sD = sLse + LT;
       const int q0t = tile * LT;
       const int nqb = min(LT, Sq16 - q0t) >> 4;
-      for (int qb = 0; qb < nqb; ++qb) {
-        const int q0 = q0t + qb * 16;  // global first query row of this 16 x 16 tile
-        float st[2][4], dpt[2][4];
-        mma_a_yT(ka, sQ, qb * 16, lane, st);    // S^T tile: rows = keys, cols = queries
-        mma_a_yT(va, sdO, qb * 16, lane, dpt);  // dP^T tile
-        float pd[2][4];
-        uint4 rnd[2] = {make_uint4(0, 0, 0, 0), make_uint4(0, 0, 0, 0)};
-        if (p.drop_on) {
-          rnd[0] = tile_rng(p, bh, q0 >> 4, k0 >> 4, Sq16 >> 4, Sk16 >> 4, ((2 * t) << 2) | (g >> 1));
-          rnd[1] = tile_rng(p, bh, q0 >> 4, k0 >> 4, Sq16 >> 4, Sk16 >> 4, ((2 * t + 1) << 2) | (g >> 1));
-        }
-#pragma unroll
-        for (int nb = 0; nb < 2; ++nb)
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int il = qb * 16 + nb * 8 + 2 * t + e, i = q0t + il;
-            const float lse = sLse[il], D = sD[il];
-            const float p0 = __expf(st[nb][e] * p.scale + mask_add(p, ma0, i, j0r) - lse);
-            const float p1 = __expf(st[nb][2 + e] * p.scale + mask_add(p, ma1, i, j1r) - lse);
-            float g0 = dpt[nb][e], g1 = dpt[nb][2 + e];
-            float pk0 = p0, pk1 = p1;
-            if (p.drop_on) {
-              // element (query i, key j): word (j & 1) | ((i >> 3) & 1) << 1 | ((j >> 3) & 1) << 2 ; j = g (+8)
-              const bool kp0 = philox_u16(rnd[e], (g & 1) | (nb << 1)) < p.drop_threshold;
-              const bool kp1 = philox_u16(rnd[e], (g & 1) | (nb << 1) | 4) < p.drop_threshold;
-              g0 = kp0 ? g0 * p.drop_scale : 0.f;
-              g1 = kp1 ? g1 * p.drop_scale : 0.f;
-              pk0 = kp0 ? p0 * p.drop_scale : 0.f;
-              pk1 = kp1 ? p1 * p.drop_scale : 0.f;
-            }
-            pd[nb][e] = pk0;
-            pd[nb][2 + e] = pk1;
-            st[nb][e] = p0 * (g0 - D) * p.scale;
-            st[nb][2 + e] = p1 * (g1 - D) * p.scale;
-          }
-        uint32_t pa[4], sa[4];
-        pa[0] = pack_bf16x2(pd[0][0], pd[0][1]);
-        pa[1] = pack_bf16x2(pd[0][2], pd[0][3]);
-        pa[2] = pack_bf16x2(pd[1][0], pd[1][1]);
-        pa[3] = pack_bf16x2(pd[1][2], pd[1][3]);
-        sa[0] = pack_bf16x2(st[0][0], st[0][1]);
-        sa[1] = pack_bf16x2(st[0][2], st[0][3]);
-        sa[2] = pack_bf16x2(st[1][0], st[1][1]);
-        sa[3] = pack_bf16x2(st[1][2], st[1][3]);
-        mma_p_z(pa, sdO, qb * 16, lane, dv);
-        mma_p_z(sa, sQ, qb * 16, lane, dk);
-      }
+      for (int qb = 0; qb < nqb; ++qb)
+        dkdv_tile(p, ka, va, ma0, ma1, k0, sQ, sdO, sLse, sD, qb * 16, q0t + qb * 16, bh, Sq16 >> 4, Sk16 >> 4, lane,
+                  dk, dv);
     }
     __syncthreads();  // the next iteration refills this stage
   }
@@ -513,8 +369,8 @@ attention_long_bwd_dkdv_kernel(const AttnParams p_in, const float* __restrict__ 
       tile_colsum(dk, csum + warp * HD, lane);
       tile_colsum(dv, csum + (LONG_WARPS + warp) * HD, lane);
     }
-    store_rows(p.dk + ((long long)seq * p.Sk + kbase) * p.lddk + h * HD, p.lddk, warp * 16, krows, lane, dk);
-    store_rows(p.dv + ((long long)seq * p.Sk + kbase) * p.lddv + h * HD, p.lddv, warp * 16, krows, lane, dv);
+    store_rows(p.dk + h * HD, p.lddk, (long long)seq * p.Sk + kbase, warp * 16, krows, lane, dk);
+    store_rows(p.dv + h * HD, p.lddv, (long long)seq * p.Sk + kbase, warp * 16, krows, lane, dv);
   }
   if (part_k != nullptr) {
     __syncthreads();
@@ -528,11 +384,8 @@ int attention_long_fwd_launch(const AttnParams& p, Addr addr, const PairSrc& pb,
                               cudaStream_t stream) {
   const int Sq16 = (p.Sq + 15) & ~15, Sk16 = (p.Sk + 15) & ~15;
   const size_t smem = (size_t)(LB + 4 * LT) * LDS * 2 + (size_t)Sk16 * 4;
-  void (*kern)(const AttnParams, const PairSrc, const VarlenSrc) =
-      addr == ADDR_PAIR ? attention_long_fwd_kernel<ADDR_PAIR>
-      : addr == ADDR_PAIR_LIST ? attention_long_fwd_kernel<ADDR_PAIR_LIST>
-      : addr == ADDR_VARLEN_PAIR ? attention_long_fwd_kernel<ADDR_VARLEN_PAIR>
-      : addr == ADDR_VARLEN_PACKED ? attention_long_fwd_kernel<ADDR_VARLEN_PACKED> : attention_long_fwd_kernel<ADDR_DENSE>;
+  const FwdKernel kern =
+      with_addr(addr, [](auto addr_c) -> FwdKernel { return attention_long_fwd_kernel<decltype(addr_c)::value>; });
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "attention_long_fwd smem attribute: %s", cudaGetErrorString(e));
   const int warps = Sq16 / 16 < LONG_WARPS ? Sq16 / 16 : LONG_WARPS;

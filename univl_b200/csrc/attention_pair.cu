@@ -5,7 +5,7 @@
 // computed once per source row, and this entry reads them in place: sequence p = i * Nb + j (the all-pairs pairing of
 // common.cuh pair_sources) takes rows r < Wa from the text source at row i * Wa + r and rows r >= Wa from the video
 // source at row j * Fb + r - Wa.  The kernels are attention.cu's (S <= 256) and attention_long.cu's (S <= 1024) forward
-// kernels with the pair row addressing (load_pair_tile) as a compile-time variant, so the context equals that of
+// kernels with the pair row addressing (load_rows) as a compile-time variant, so the context equals that of
 // univl_attention_fwd / univl_attention_long_fwd on the materialised per-pair q/k/v bit for bit.
 //
 // univl_attention_pair_list_fwd runs the same kernels on a list of pairs (sequence p = (text_index[p],
@@ -30,13 +30,9 @@ extern "C" int univl_attention_pair_fwd(const void* qa, long long ldqa, const vo
   UNIVL_CHECK_ARG((long long)Na * Nb * heads <= INT_MAX, "attention_pair_fwd: too many pairs (%d x %d)", Na, Nb);
   UNIVL_CHECK_ARG(Fb == 0 || (mask_a != nullptr && mask_b != nullptr),
                   "attention_pair_fwd: both mask parts are needed when Fb > 0");
-  if (Fb > 0) {
-    UNIVL_CHECK_ARG(qb && kb && vb, "attention_pair_fwd: null second-source q/k/v");
-    UNIVL_CHECK_ARG((ldqb % 8) == 0 && (ldkb % 8) == 0 && (ldvb % 8) == 0,
-                    "attention_pair_fwd: second-source row strides must be multiples of 8");
-    UNIVL_CHECK_ARG(((uintptr_t)qb & 15) == 0 && ((uintptr_t)kb & 15) == 0 && ((uintptr_t)vb & 15) == 0,
-                    "attention_pair_fwd: second-source q/k/v must be 16-byte aligned");
-  }
+  PairSrc pb{};
+  if (Fb > 0)
+    if (int rc = fill_pair_src(pb, qb, ldqb, kb, ldkb, vb, ldvb, "attention_pair_fwd")) return rc;
   const int n_seq = Na * Nb;
   AttnParams p = {};
   if (int rc = fill_common(p, qa, ldqa, ka, ldka, va, ldva, mask_a, mask_b, Wa, Fb, Nb, 1, n_seq, heads, Sq, S, 0,
@@ -44,10 +40,8 @@ extern "C" int univl_attention_pair_fwd(const void* qa, long long ldqa, const vo
     return rc;
   UNIVL_CHECK_ARG(o != nullptr && (ldo % 2) == 0, "attention_pair_fwd: bad output");
   if (n_seq == 0) return UNIVL_OK;
-  const PairSrc pb{(const bf16*)qb, (const bf16*)kb, (const bf16*)vb, ldqb, ldkb, ldvb};
   p.o = (bf16*)o; p.ldo = ldo; p.lse = lse;
-  if (S <= 256) return attention_fwd_launch(p, ADDR_PAIR, pb, VarlenSrc{}, (cudaStream_t)stream);
-  return attention_long_fwd_launch(p, ADDR_PAIR, pb, VarlenSrc{}, (cudaStream_t)stream);
+  return attention_fwd_any_launch(p, ADDR_PAIR, pb, VarlenSrc{}, (cudaStream_t)stream);
 }
 
 extern "C" int univl_attention_pair_list_fwd(const void* qa, long long ldqa, const void* ka, long long ldka,
@@ -64,11 +58,8 @@ extern "C" int univl_attention_pair_list_fwd(const void* qa, long long ldqa, con
   UNIVL_CHECK_ARG((long long)n_pairs * heads <= INT_MAX, "attention_pair_list_fwd: too many pairs (%d)", n_pairs);
   UNIVL_CHECK_ARG(text_index && video_index && mask_a && mask_b,
                   "attention_pair_list_fwd: the index lists and both mask parts are needed");
-  UNIVL_CHECK_ARG(qb && kb && vb, "attention_pair_list_fwd: null second-source q/k/v");
-  UNIVL_CHECK_ARG((ldqb % 8) == 0 && (ldkb % 8) == 0 && (ldvb % 8) == 0,
-                  "attention_pair_list_fwd: second-source row strides must be multiples of 8");
-  UNIVL_CHECK_ARG(((uintptr_t)qb & 15) == 0 && ((uintptr_t)kb & 15) == 0 && ((uintptr_t)vb & 15) == 0,
-                  "attention_pair_list_fwd: second-source q/k/v must be 16-byte aligned");
+  PairSrc pb;
+  if (int rc = fill_pair_src(pb, qb, ldqb, kb, ldkb, vb, ldvb, "attention_pair_list_fwd")) return rc;
   AttnParams p = {};
   // masks [n_pairs, Wa] / [n_pairs, Fb]: aligned pairing (row p of each part)
   if (int rc = fill_common(p, qa, ldqa, ka, ldka, va, ldva, mask_a, mask_b, Wa, Fb, n_pairs, 0, n_pairs, heads, Sq, S,
@@ -76,11 +67,9 @@ extern "C" int univl_attention_pair_list_fwd(const void* qa, long long ldqa, con
     return rc;
   UNIVL_CHECK_ARG(o != nullptr && (ldo % 2) == 0, "attention_pair_list_fwd: bad output");
   if (n_pairs == 0) return UNIVL_OK;
-  const PairSrc pb{(const bf16*)qb, (const bf16*)kb, (const bf16*)vb, ldqb, ldkb, ldvb};
   VarlenSrc vl{};
   vl.idx_a = text_index;
   vl.idx_b = video_index;
   p.o = (bf16*)o; p.ldo = ldo; p.lse = lse;
-  if (S <= 256) return attention_fwd_launch(p, ADDR_PAIR_LIST, pb, vl, (cudaStream_t)stream);
-  return attention_long_fwd_launch(p, ADDR_PAIR_LIST, pb, vl, (cudaStream_t)stream);
+  return attention_fwd_any_launch(p, ADDR_PAIR_LIST, pb, vl, (cudaStream_t)stream);
 }

@@ -77,20 +77,13 @@ extern "C" int univl_attention_varlen_fwd(const void* qa, long long ldqa, const 
                            q_first ? 1 : max_sk, max_sk, 0, scale, 0.f, nullptr, 0, 1024))
     return rc;
   PairSrc pb{};
-  if (idx_a != nullptr) {
-    UNIVL_CHECK_ARG(qb && kb && vb, "attention_varlen_fwd: null second-source q/k/v");
-    UNIVL_CHECK_ARG((ldqb % 8) == 0 && (ldkb % 8) == 0 && (ldvb % 8) == 0,
-                    "attention_varlen_fwd: second-source row strides must be multiples of 8");
-    UNIVL_CHECK_ARG(((uintptr_t)qb & 15) == 0 && ((uintptr_t)kb & 15) == 0 && ((uintptr_t)vb & 15) == 0,
-                    "attention_varlen_fwd: second-source q/k/v must be 16-byte aligned");
-    pb = PairSrc{(const bf16*)qb, (const bf16*)kb, (const bf16*)vb, ldqb, ldkb, ldvb};
-  }
+  if (idx_a != nullptr)
+    if (int rc = fill_pair_src(pb, qb, ldqb, kb, ldkb, vb, ldvb, "attention_varlen_fwd")) return rc;
   UNIVL_CHECK_ARG(o != nullptr && (ldo % 2) == 0, "attention_varlen_fwd: bad output");
   if (n_seq == 0) return UNIVL_OK;
   p.o = (bf16*)o; p.ldo = ldo; p.lse = lse;
   const Addr addr = idx_a != nullptr ? ADDR_VARLEN_PAIR : ADDR_VARLEN_PACKED;
-  if (max_sk <= 256) return attention_fwd_launch(p, addr, pb, vl, (cudaStream_t)stream);
-  return attention_long_fwd_launch(p, addr, pb, vl, (cudaStream_t)stream);
+  return attention_fwd_any_launch(p, addr, pb, vl, (cudaStream_t)stream);
 }
 
 extern "C" int univl_gather_rows_varlen(const void* a, long long lda, const void* b, long long ldb, const int* idx_a,
