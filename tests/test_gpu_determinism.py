@@ -1,7 +1,9 @@
 """GPU: a retrieval fine-tuning (FT-Align) training step computes the same bits every time it runs.
 
 No cross-CTA floating-point atomic is on this path: split-K weight gradients, LayerNorm / embedding / bias / attention
-bias gradients, the similarity head and the optimizer's norms all add partial rows in a fixed order.  So two identical
+bias gradients, the similarity head and the optimizer's norms all add partial rows in a fixed order.  (The other
+training modes' softmax cross-entropy sums its rows in row order too; the one float atomic left on a training path is
+MIL-NCE's dsim, whose cells each take at most two addends onto zero, which commute.)  So two identical
 models and optimizers fed the same batch agree bit for bit in the loss, every gradient, every parameter and the Adam
 moments — with or without SMs reserved for a concurrent collective, and between an eager step and a CUDA-graph replay
 of it.  bench.py's --dump-outputs files, the README's statement of that claim, are compared byte for byte."""

@@ -10,6 +10,7 @@ pytestmark = pytest.mark.gpu
 
 from tests import attn_check as ac  # noqa: E402
 from tests import gemm_check as gc  # noqa: E402
+from tests.row_check import ln_bwd64 as _ln_bwd64  # noqa: E402
 from univl_b200 import ops  # noqa: E402
 from univl_b200 import runtime as rt  # noqa: E402
 
@@ -573,23 +574,6 @@ def _within(got, ref, bound, what):
         i = tuple(int(v) for v in (~ok).nonzero()[0])
         raise AssertionError("%s: %d elements outside the bound; first %s: got %r ref %r bound %r"
                              % (what, int((~ok).sum()), i, float(got[i]), float(ref[i]), float(bound[i])))
-
-
-def _ln_bwd64(z, d, gamma):
-    """fp64 LayerNorm backward of rows z [R, C] for upstream d: (xhat, dz, e_xhat, e_dz) where e_* bound the fp32
-    kernels' per-element error (C-term row sums for the mean, variance and the two backward row sums)"""
-    C = z.shape[1]
-    mean = z.mean(1, keepdim=True)
-    rstd = 1.0 / torch.sqrt(((z - mean) ** 2).mean(1, keepdim=True) + 1e-12)
-    xhat = (z - mean) * rstd
-    g = d * gamma.double()
-    gx = (g * xhat).mean(1, keepdim=True)
-    dz = rstd * (g - g.mean(1, keepdim=True) - xhat * gx)
-    k = (C + 16) * U32
-    e_xhat = k * (rstd * (z.abs().mean(1, keepdim=True) + z.abs()) + xhat.abs())
-    e_dz = 2 * k * (rstd * (g.abs() + g.abs().mean(1, keepdim=True) + (1 + xhat.abs()) * (g * xhat).abs().mean(1, keepdim=True))
-                    + dz.abs()) + rstd * (g * xhat).abs().mean(1, keepdim=True) * e_xhat
-    return xhat, dz, e_xhat, e_dz
 
 
 @pytest.mark.parametrize("rows,cols", [(1536, 768), (98304, 3072), (1, 768), (1000, 771)])

@@ -160,17 +160,20 @@ __device__ __forceinline__ void erf_exp_terms(float x, float& w, float& gauss) {
   poly = fmaf(poly, t, 0.5f * 0.254829592f);
   w = (poly * t) * gauss;
 }
+// At x = +-inf, w and gauss are 0: |x| is capped at 1e30 where it multiplies them, so the results are the limits
+// (gelu: +inf / -0, gelu': 1 / 0) rather than inf * 0 = NaN.  A NaN x still gives NaN through w.  gelu takes the sign
+// of x, which no finite result changes (x - x w > 0 for x > 0, -|x| w <= 0 for x < 0) but keeps gelu(-0) = -0.
 __device__ __forceinline__ float gelu_erf(float x) {
   float w, g;
   erf_exp_terms(x, w, g);
-  return fmaf(-fabsf(x), w, fmaxf(x, 0.f));
+  return copysignf(fmaf(-fminf(fabsf(x), 1e30f), w, fmaxf(x, 0.f)), x);
 }
 // d/dx gelu_erf(x) = Phi(x) + x * phi(x)
 __device__ __forceinline__ float gelu_erf_grad(float x) {
   float w, g;
   erf_exp_terms(x, w, g);
   const float cdf = x >= 0.f ? 1.0f - w : w;
-  return fmaf(x * 0.39894228040143267794f, g, cdf);
+  return fmaf(fminf(fmaxf(x, -1e30f), 1e30f) * 0.39894228040143267794f, g, cdf);
 }
 
 // ----------------------------------------------------------------------------

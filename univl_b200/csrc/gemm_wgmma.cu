@@ -1056,7 +1056,7 @@ vocab_xent_group_kernel(const float* __restrict__ nll, const long long* __restri
   }
 }
 
-// finalize_mean_kernel's arithmetic: mean over groups of sum / count, 0 / 0 = NaN for a group without a scored row
+// xent_sum_kernel's arithmetic (csrc/loss.cu): mean over groups of sum / count, 0 / 0 = NaN for a group without a scored row
 __global__ void vocab_xent_mean_kernel(const float* __restrict__ sum_count, int groups, float* __restrict__ out) {
   float acc = sum_count[0] / sum_count[groups];
   for (int g = 1; g < groups; ++g) acc += sum_count[g] / sum_count[groups + g];

@@ -260,6 +260,8 @@ milnce_kernel(const float* __restrict__ sim, float* __restrict__ loss, float* __
       float gr = expf(x - lse);
       if (first && same) gr -= expf(x - lsep);
       gr /= (float)bs;
+      // Order-independent: a cell receives at most two addends onto its 0 — (r, r) from both halves of row r, and
+      // (r1, r2) from the picked rows r1 and r2 — and 0 + a + b has the same bits as 0 + b + a.
       atomicAdd(first ? &dsim[cc * N + r] : &dsim[r * N + cc], gr);
     }
   }
@@ -273,18 +275,18 @@ milnce_kernel(const float* __restrict__ sim, float* __restrict__ loss, float* __
 // ------------------------------------------------------------------------------------------------------------
 // target_mode 0: target = labels[r]; 1: target = r.  Row is scored iff labels[r] != ignore_index.
 // Optional pairwise mask (MFM): logit += (1 - vm[r] * vm[c]) * -1e8   (modeling.py:286-288).
-// G groups of R = T / G consecutive rows (micro-batches) keep their own sum and count: loss_sum[g], count[g].  In
+// G groups of R = T / G consecutive rows (micro-batches) keep their own sum and count (xent_sum_kernel).  In
 // target_mode 1 a row of group g holds logits against its own group's R frames only (the MFM NCE of one micro-batch):
 // its target is r - g R and its mask columns are vm[g R + c].
 __global__ void __launch_bounds__(256)
 xent_fwd_kernel(const float* __restrict__ logits, long long ld, const long long* __restrict__ labels,
-                const long long* __restrict__ vm, float* __restrict__ lse_out, float* __restrict__ loss_sum,
-                float* __restrict__ count, int V, int target_mode, long long ignore_index, int rows_per_group) {
+                const long long* __restrict__ vm, float* __restrict__ lse_out, float* __restrict__ term, int V,
+                int target_mode, long long ignore_index, int rows_per_group) {
   __shared__ float red[32];
   const int r = blockIdx.x;
   const long long lab = labels[r];
   if (lab == ignore_index) {
-    if (threadIdx.x == 0) lse_out[r] = 0.f;
+    if (threadIdx.x == 0) lse_out[r] = term[r] = 0.f;
     return;
   }
   const int g = r / rows_per_group;
@@ -312,8 +314,7 @@ xent_fwd_kernel(const float* __restrict__ logits, long long ld, const long long*
     const long long tgt = target_mode == 0 ? lab : r - off;
     float xt = row[tgt];
     if (vm) xt += (1.0f - vr * (vm[tgt] != 0 ? 1.f : 0.f)) * -1e8f;
-    atomicAdd(loss_sum + g, lse - xt);
-    atomicAdd(count + g, 1.f);
+    term[r] = lse - xt;
   }
 }
 
@@ -351,13 +352,32 @@ xent_bwd_kernel(const float* __restrict__ logits, long long ld, const long long*
   }
 }
 
-// mean over groups of sum[g] / count[g]; 0/0 -> NaN exactly like the reference's mean of an empty selection
-// (modeling.py:295-296), so a group without a scored row makes the loss NaN, as that micro-batch's loss would be
-__global__ void finalize_mean_kernel(const float* __restrict__ sum, const float* __restrict__ count, int groups,
-                                     float* __restrict__ out) {
-  float acc = sum[0] / count[0];
-  for (int g = 1; g < groups; ++g) acc += sum[g] / count[g];
-  *out = groups > 1 ? acc / (float)groups : acc;
+// One CTA: sum[g] and count[g] of each group's per-row terms (xent_fwd_kernel), each thread adding its rows in row order
+// and block_sum combining the threads in a fixed order, so the loss has the same bits on every launch.  Then the mean
+// over groups of sum[g] / count[g]; 0/0 -> NaN exactly like the reference's mean of an empty selection
+// (modeling.py:295-296), so a group without a scored row makes the loss NaN, as that micro-batch's loss would be.
+__global__ void __launch_bounds__(256)
+xent_sum_kernel(const float* __restrict__ term, const long long* __restrict__ labels, long long ignore_index,
+                int rows_per_group, int groups, float* __restrict__ sum, float* __restrict__ count,
+                float* __restrict__ out) {
+  __shared__ float red[32];
+  float acc = 0.f;
+  for (int g = 0; g < groups; ++g) {
+    const long long r0 = (long long)g * rows_per_group;
+    float s = 0.f, n = 0.f;
+    for (int r = threadIdx.x; r < rows_per_group; r += blockDim.x) {
+      s += term[r0 + r];
+      n += labels[r0 + r] != ignore_index ? 1.f : 0.f;
+    }
+    s = block_sum(s, red);
+    n = block_sum(n, red);
+    if (threadIdx.x == 0) {
+      sum[g] = s;
+      count[g] = n;
+      acc = g == 0 ? s / n : acc + s / n;
+    }
+  }
+  if (threadIdx.x == 0) *out = groups > 1 ? acc / (float)groups : acc;
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -485,7 +505,7 @@ extern "C" int univl_milnce_loss(const float* sim, float* loss, float* dsim, int
   });
 }
 // loss = mean over groups of the mean over the group's scored rows of (logsumexp(row) - row[target]);
-// scratch: lse[T], sum_count[2 * groups] (sums, then counts; zeroed here)
+// outputs besides the loss: lse[T], sum_count[2 * groups] (sums, then counts)
 extern "C" int univl_softmax_xent_fwd(const float* logits, long long ld, const long long* labels,
                                       const long long* pair_mask, float* lse, float* sum_count, float* loss, int T,
                                       int V, int target_mode, long long ignore_index, int groups, void* stream) {
@@ -496,12 +516,16 @@ extern "C" int univl_softmax_xent_fwd(const float* logits, long long ld, const l
   UNIVL_CHECK_ARG(target_mode == 0 || groups == 1 || V == T / groups,
                   "softmax_xent_fwd: grouped target_mode 1 needs V = T / groups");
   cudaStream_t st = (cudaStream_t)stream;
-  cudaError_t e = cudaMemsetAsync(sum_count, 0, 2 * (size_t)groups * sizeof(float), st);
-  if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "softmax_xent_fwd memset: %s", cudaGetErrorString(e));
-  xent_fwd_kernel<<<T, 256, 0, st>>>(logits, ld, labels, pair_mask, lse, sum_count, sum_count + groups, V, target_mode,
-                                     ignore_index, T / groups);
-  finalize_mean_kernel<<<1, 1, 0, st>>>(sum_count, sum_count + groups, groups, loss);
-  UNIVL_CHECK_LAUNCH("softmax_xent_fwd");
+  // per-row terms in scratch, not in lse: ProjXentFn keeps lse for the backward
+  float* term;
+  if (int rc = scratch_alloc((void**)&term, (size_t)T * sizeof(float), st)) return rc;
+  xent_fwd_kernel<<<T, 256, 0, st>>>(logits, ld, labels, pair_mask, lse, term, V, target_mode, ignore_index,
+                                     T / groups);
+  xent_sum_kernel<<<1, 256, 0, st>>>(term, labels, ignore_index, T / groups, groups, sum_count, sum_count + groups,
+                                     loss);
+  const cudaError_t e = cudaGetLastError();
+  cudaFreeAsync(term, st);
+  if (e != cudaSuccess) return set_error(UNIVL_ERR_CUDA, "softmax_xent_fwd launch: %s", cudaGetErrorString(e));
   return UNIVL_OK;
 }
 extern "C" int univl_softmax_xent_bwd(const float* logits, long long ld, const long long* labels,
