@@ -9,7 +9,10 @@
 //            update = m / (sqrt(v) + e) + weight_decay * p    (e OUTSIDE the sqrt, decoupled decay)
 //            p -= lr * schedule(step / t_total, warmup) * update ;  step += 1
 //   warmup_linear(x, w) = x / w if x < w else max((x - 1) / (w - 1), 0)      (optimization.py:37-43)
-// The step counter lives in device memory so the whole update is CUDA-graph capturable.
+// The step counter lives in device memory so the whole update is CUDA-graph capturable.  It is ONE counter for all
+// tensors, where the reference keeps a `step` per parameter and advances it only when that parameter has a gradient:
+// a tensor that is skipped on some steps (below) is scheduled here at the optimizer's step count, in the reference at
+// its own, smaller one.  Both agree whenever every tensor receives a gradient on every step.
 #include "common.cuh"
 
 namespace univl {
@@ -52,37 +55,51 @@ adam_sumsq_kernel(const G* __restrict__ g, const AdamSeg* __restrict__ segs, flo
   __shared__ float red[8];
   const AdamSeg s = segs[blockIdx.x];
   float acc = 0.f;
+  // OR of the gradients' bits: some element is nonzero iff the OR has a magnitude bit set (-0 counts as zero).  A bit
+  // test, not `x != 0.f`: under --use_fast_math comparisons flush denormals, and a denormal gradient is a gradient.
+  unsigned bits = 0u;
   for (int i = threadIdx.x * 4; i < s.count; i += blockDim.x * 4) {
     if (i + 4 <= s.count) {
       const float4 x = load_grad4(g, s.offset + i);
       acc += (x.x * x.x + x.y * x.y + x.z * x.z + x.w * x.w) * grad_scale * grad_scale;
+      bits |= __float_as_uint(x.x) | __float_as_uint(x.y) | __float_as_uint(x.z) | __float_as_uint(x.w);
     } else {
       for (int j = i; j < s.count; ++j) {
         const float x = load_grad(g, s.offset + j);
         acc += x * x * grad_scale * grad_scale;
+        bits |= __float_as_uint(x);
       }
     }
   }
   acc = warp_sum(acc);
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
-  __syncthreads();
+  const int any_nz = __syncthreads_or((bits & 0x7fffffffu) != 0u);
   if (threadIdx.x == 0) {
     float t = 0.f;
     for (int w = 0; w < 8; ++w) t += red[w];
-    part[blockIdx.x] = t;  // this chunk's share; adam_tensor_sums_kernel adds a tensor's chunks in order
+    // this chunk's share; adam_tensor_sums_kernel adds a tensor's chunks in order.  A chunk with a nonzero gradient
+    // whose squares all flushed stores -0: adding it changes no sum, and its sign bit still says "has a gradient".
+    part[blockIdx.x] = (any_nz && t == 0.f) ? -0.f : t;
   }
 }
 
-// per-chunk sums of squares -> sumsq[tensor], each tensor's chunks added in chunk order
+// per-chunk sums of squares -> sumsq[tensor], each tensor's chunks added in chunk order; tensor_nz[tensor] = some
+// chunk of it has a nonzero gradient (a partial that is not +0)
 __global__ void __launch_bounds__(256)
 adam_tensor_sums_kernel(const float* __restrict__ part, const AdamSeg* __restrict__ segs, int n_chunks,
-                        float* __restrict__ sumsq, int n_tensors) {
+                        float* __restrict__ sumsq, int* __restrict__ tensor_nz, int n_tensors) {
   const int i = blockIdx.x * 256 + threadIdx.x;
   if (i >= n_tensors) return;
   float t = 0.f;
+  unsigned nz = 0u;
   for (int c = 0; c < n_chunks; ++c)
-    if (segs[c].tensor == i) t += part[c];
+    if (segs[c].tensor == i) {
+      const float x = part[c];
+      t += x;
+      nz |= __float_as_uint(x);
+    }
   sumsq[i] = t;
+  tensor_nz[i] = nz != 0u;
 }
 
 // sumsq[n_tensors] -> sumsq[n_tensors] holds the total
@@ -104,11 +121,14 @@ template <typename G>
 __global__ void __launch_bounds__(256)
 adam_update_kernel(float* __restrict__ p, const G* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
                    bf16* __restrict__ p_bf16, const AdamSeg* __restrict__ segs, const float* __restrict__ sumsq,
-                   int n_tensors, const long long* __restrict__ step, AdamCfg cfg) {
+                   const int* __restrict__ tensor_nz, int n_tensors, const long long* __restrict__ step,
+                   AdamCfg cfg) {
   const AdamSeg s = segs[blockIdx.x];
   // a tensor whose gradient is identically zero received none this step (unused poolers etc.): the reference
-  // skips parameters with `p.grad is None` entirely — no moment update, no weight decay (optimization.py:115-116)
-  if (sumsq[s.tensor] == 0.f) return;
+  // skips parameters with `p.grad is None` entirely — no moment update, no weight decay (optimization.py:115-116).
+  // Decided from the nonzero flags, not from sumsq == 0: squares below the fp32 normal range flush to zero (fast-math
+  // FTZ), so gradients under ~1e-19 in magnitude sum to 0 yet must still move the moments and apply weight decay.
+  if (!tensor_nz[s.tensor]) return;
   float cg = 1.f;
   if (cfg.global_clip_norm > 0.f) cg = fminf(1.f, cfg.global_clip_norm / (sqrtf(sumsq[n_tensors]) + 1e-6f));
   float ct = 1.f;
@@ -168,7 +188,8 @@ using namespace univl;
 
 // One optimizer step over flat buffers.  segs: device array of n_chunks {int64 offset, int32 count, int32 tensor,
 // float lr, float weight_decay, -, -} — one CTA per chunk (chunks of <= 64K elements, offsets multiples of 64);
-// scratch: n_tensors + 1 floats; step: device int64 (incremented).  p_bf16 (same element offsets as p) may be null.
+// scratch: n_tensors + 1 floats (left holding each tensor's and the total sum of squares of the scaled gradients);
+// step: device int64 (incremented).  p_bf16 (same element offsets as p) may be null.
 template <typename G>
 static int adam_step(float* p, const G* g, float* m, float* v, void* p_bf16, const void* segs, int n_chunks,
                      int n_tensors, float* scratch, long long* step, const AdamCfg& cfg, void* stream) {
@@ -176,13 +197,16 @@ static int adam_step(float* p, const G* g, float* m, float* v, void* p_bf16, con
   UNIVL_CHECK_ARG(n_tensors > 0 && n_chunks >= n_tensors, "bert_adam_step: bad tensor / chunk count");
   cudaStream_t st = (cudaStream_t)stream;
   const AdamSeg* s = reinterpret_cast<const AdamSeg*>(segs);
+  // one allocation: per-chunk sums [n_chunks], then per-tensor "has a gradient" flags [n_tensors]
   float* part;
-  if (int rc = scratch_alloc((void**)&part, (size_t)n_chunks * sizeof(float), st)) return rc;
+  if (int rc = scratch_alloc((void**)&part, (size_t)(n_chunks + n_tensors) * sizeof(float), st)) return rc;
+  int* tensor_nz = reinterpret_cast<int*>(part + n_chunks);
   adam_sumsq_kernel<G><<<n_chunks, 256, 0, st>>>(g, s, part, cfg.grad_scale);
-  adam_tensor_sums_kernel<<<(n_tensors + 255) / 256, 256, 0, st>>>(part, s, n_chunks, scratch, n_tensors);
-  cudaFreeAsync(part, st);
+  adam_tensor_sums_kernel<<<(n_tensors + 255) / 256, 256, 0, st>>>(part, s, n_chunks, scratch, tensor_nz, n_tensors);
   adam_total_kernel<<<1, 256, 0, st>>>(scratch, n_tensors);
-  adam_update_kernel<G><<<n_chunks, 256, 0, st>>>(p, g, m, v, (bf16*)p_bf16, s, scratch, n_tensors, step, cfg);
+  adam_update_kernel<G><<<n_chunks, 256, 0, st>>>(p, g, m, v, (bf16*)p_bf16, s, scratch, tensor_nz, n_tensors, step,
+                                                  cfg);
+  cudaFreeAsync(part, st);
   adam_step_inc_kernel<<<1, 1, 0, st>>>(step);
   UNIVL_CHECK_LAUNCH("bert_adam_step");
   return UNIVL_OK;
