@@ -10,6 +10,7 @@ pytestmark = pytest.mark.gpu
 
 from tests import attn_check as ac  # noqa: E402
 from tests import gemm_check as gc  # noqa: E402
+from tests.layer_check import colsum_bound  # noqa: E402
 from tests.row_check import ln_bwd64 as _ln_bwd64  # noqa: E402
 from univl_b200 import ops  # noqa: E402
 from univl_b200 import runtime as rt  # noqa: E402
@@ -588,7 +589,7 @@ def test_colsum_fp64_and_repeatable(rows, cols):
         return [out]
     got = _same_bits(run)[0]
     xd = x.double()
-    _within(got - 1.0, xd.sum(0), (rows + 2) * U32 * xd.abs().sum(0) + 2 * U32, "colsum")
+    _within(got - 1.0, xd.sum(0), colsum_bound(x, torch.ones(cols, device=DEV)), "colsum")
 
 
 @pytest.mark.parametrize("rows,cols,p", [(1, 768, 0.0), (37, 1024, 0.0), (1536, 768, 0.1), (98304, 768, 0.1)])
