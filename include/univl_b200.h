@@ -297,6 +297,31 @@ int univl_vocab_xent_fwd(const void* x, long long ldx, const void* w, long long 
 int univl_vocab_xent_bwd(const void* x, long long ldx, const void* w, long long ldw, const float* bias,
                          const long long* labels, const float* lse, const float* sum_count, const float* gscale,
                          void* dlogits, long long ld_d, int T, int V, int Kc, int groups, void* stream);
+/* One step of caption beam search over the tied vocabulary projection, the logits never written (Beam.advance,
+ * modules/beam.py:63-87).  x bf16 [R, Kc] holds the prediction head's transform of R = n_inst * n_beam rows, the n_beam
+ * rows of an instance contiguous; W, bias, logit[r, c] and the chunking as univl_vocab_xent_fwd.  Two passes over the
+ * vocabulary: lse fp32 [R] gets every row's log-sum-exp (folded as univl_vocab_xent_fwd folds it), then the logits are
+ * recomputed and each column c < V gets key = (logit[r, c] - lse[r]) + score[r] in fp32.  Instance i's rows
+ * i n_beam + k, k < n_live[i] (int32 [n_inst], device; 1 at the first step, n_beam after) compete: out_key fp32 and
+ * out_index int32 [n_inst, n_beam] hold its n_beam best as (key, flat = k V + c) in one strict order, key descending,
+ * then flat ascending, so the result is exact and does not depend on chunking, grid or reserved SMs.  1 <= n_beam <= 8,
+ * n_beam <= V; otherwise UNIVL_ERR_ARG.  Inputs are expected finite.  workspace: at least
+ * univl_vocab_beam_topk_workspace(n_inst, n_beam, V) bytes, 16-byte aligned, used on `stream` only (graph-safe). */
+int univl_vocab_beam_topk_workspace(int n_inst, int n_beam, int V);
+int univl_vocab_beam_topk(const void* x, long long ldx, const void* w, long long ldw, const float* bias,
+                          const float* score, const int* n_live, int n_inst, int n_beam, int V, int Kc, float* lse,
+                          float* out_key, int* out_index, void* workspace, long long workspace_bytes, void* stream);
+/* The beam bookkeeping of step t after univl_vocab_beam_topk, one CTA per instance.  An instance whose done[i] (int32)
+ * is 0 takes its picks: hypothesis j continues row k = flat / V of the instance with word c = flat mod V;
+ * score[i n_beam + j] = key, prev_k[t][i][j] = k and word[t][i][j] = c (int32 step tables [max_words, n_inst, n_beam]),
+ * tokens[i n_beam + j] = c (int64, the row's next input), and done[i] = 1 when its top pick's word is eos.  A done
+ * instance changes none of these.  Ancestor tables anc_in / anc_out int32 [R, max_words] (distinct; swap them between
+ * steps): row r's list for step t + 1 is its parent's (row i n_beam + k, or r itself when done) first t + 1 entries
+ * of anc_in, then its own key slot (t + 1) R + r (when t + 1 < max_words) — univl_attention_decode_fwd's key rows over
+ * a K|V buffer with one plane of R rows per position.  0 <= t < max_words. */
+int univl_beam_advance(const float* key, const int* index, int n_inst, int n_beam, int V, int t, int max_words,
+                       long long eos, float* score, int* done, int* prev_k, int* word, long long* tokens,
+                       const int* anc_in, int* anc_out, void* stream);
 /* Exact top-k of sim = t v^T per text row, the matrix never written (retrieval shortlists): t [Nt, H], v [Nv, H]
  * fp32 row-major, 16-byte aligned, H a multiple of 4.  scores fp32 [Nt, k] and index int32 [Nt, k] hold row i's k
  * best videos in one strict order: score descending, then video index ascending.  Every score has the bits

@@ -5,7 +5,8 @@ through univl_b200.launcher) on synthetic batches, in three configurations alter
   cache      UNIVL_DECODE_CACHE=prefix with the checkout's Beam (one device read per token per hypothesis)
   cache+host UNIVL_DECODE_CACHE=prefix with univl_b200.modules.beam.Beam (hypotheses on the host)
 
-and, for comparison, univl_b200.caption.beam_search on the same inputs.  A randomly initialised model never ranks [SEP]
+and, for comparison, univl_b200.caption.beam_search and univl_b200.caption.GraphBeamSearch ("graph": the loop on the
+device, replayed as CUDA graphs; one searcher per cap, so its graphs are captured in the warm-up) on the same inputs.  A randomly initialised model never ranks [SEP]
 first, so the decode cap (the driver's --max_words loop bound) fixes the number of steps.  Reports ms per batch and
 the peak of torch allocations, with the card's name and power limit read in the same run; --profile adds a
 torch.profiler run of one batch per configuration: the summed time of its device events, and the rest of the profiled
@@ -29,7 +30,8 @@ import torch  # noqa: E402
 
 # the README's settings: YouCookII 12 text / 6 visual / 2 cross / 3 decoder layers, W = 128, F = 96; MSRVTT W = F = 48
 SHAPES = {"youcook": dict(W=128, F=96), "msrvtt": dict(W=48, F=48), "tiny": dict(W=16, F=16)}
-CONFIGS = ("off", "cache", "cache+host", "beam_search")
+CONFIGS = ("off", "cache", "cache+host", "beam_search", "graph")
+_SEARCHERS = {}
 
 
 class FakeTokenizer(object):
@@ -96,16 +98,21 @@ def run_config(name, drv, model, loader, cap, out_dir, ref_beam, host_beam):
     """-> hypotheses (list of strings) of one pass over the loader"""
     args = argparse.Namespace(max_words=cap, output_dir=out_dir, datatype="youcook")
     device = torch.device("cuda", 0)
-    if name == "beam_search":
-        from univl_b200.caption import beam_search
+    if name in ("beam_search", "graph"):
+        from univl_b200.caption import GraphBeamSearch, beam_search
+        if name == "graph":
+            if cap not in _SEARCHERS:
+                _SEARCHERS[cap] = GraphBeamSearch(model, n_beam=5, max_words=cap)
+            search = _SEARCHERS[cap]
+        else:
+            search = lambda seq, vis, am, vm: beam_search(model, seq, vis, am, vm, cap, n_beam=5)
         hyps = []
         os.environ["UNIVL_DECODE_CACHE"] = "off"
         for batch in loader:
             batch = [x.to(device) for x in batch]
             with torch.no_grad():
                 seq, vis = model.get_sequence_visual_output(batch[0], batch[2], batch[1], batch[3], batch[4])
-                h, _ = beam_search(model, seq, vis, batch[1].view(seq.shape[0], -1), batch[4].view(seq.shape[0], -1),
-                                   cap, n_beam=5)
+                h, _ = search(seq, vis, batch[1].view(seq.shape[0], -1), batch[4].view(seq.shape[0], -1))
             hyps += [" ".join(map(str, x)) for x in h]
         return hyps
     os.environ["UNIVL_DECODE_CACHE"] = "off" if name == "off" else "prefix"
@@ -153,9 +160,9 @@ def main():
     cfg, model = build(a.shape, layers, a.batch_size_val)
     loader = make_loader(cfg, a.batches * a.batch_size_val, a.batch_size_val, seed=5)
     configs = a.configs.split(",")
-    for name in configs:                                  # warm-up: one batch of every configuration
-        run_config(name, drv, model, make_loader(cfg, a.batch_size_val, a.batch_size_val, 6), min(a.cap, 3), tmp,
-                   ref_beam, host_beam)
+    for name in configs:  # warm-up: one batch of every configuration (graph: at the timed cap, which captures it)
+        run_config(name, drv, model, make_loader(cfg, a.batch_size_val, a.batch_size_val, 6),
+                   a.cap if name == "graph" else min(a.cap, 3), tmp, ref_beam, host_beam)
     times = {n: [] for n in configs}
     peaks, hyps = {}, {}
     for _ in range(a.repeats):
@@ -187,7 +194,9 @@ def main():
                           "host_gap_ms": round(max(0.0, wall - gpu), 1)}
             with open(os.path.join(a.profile, "%s.txt" % name.replace("+", "_")), "w") as fh:
                 fh.write(p.key_averages().table(sort_by="self_device_time_total", row_limit=25))
-    same = {n: hyps[n] == hyps[configs[0]] for n in configs if n != "beam_search"}
+    same = {n: hyps[n] == hyps[configs[0]] for n in configs if n not in ("beam_search", "graph")}
+    if "graph" in configs and "beam_search" in configs:
+        same["graph_vs_beam_search"] = hyps["graph"] == hyps["beam_search"]
     res = {"card": card(), "shape": a.shape, "layers": a.layers, "batch_size_val": a.batch_size_val, "cap": a.cap,
            "batches": a.batches, "ms_per_batch": {n: [round(x, 1) for x in v] for n, v in times.items()},
            "peak_gib": {n: round(v, 2) for n, v in peaks.items()}, "same_captions_as_first": same, "profile": prof}

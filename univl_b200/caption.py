@@ -493,3 +493,221 @@ def beam_search(model, sequence_output, visual_output, input_mask, video_mask, m
         hyps.append(hyp[::-1])
         outs.append(float(scores_c[i, int(order_c[i, 0])]))
     return hyps, outs
+
+
+# Tokens per captured graph of GraphBeamSearch: after each chunk the host reads "every instance done" once, so at most
+# GRAPH_STEP_CHUNK - 1 steps run after the last instance finished.
+GRAPH_STEP_CHUNK = 8
+
+
+class _BeamGraphs:
+    """GraphBeamSearch's static buffers and captured chunks for one (n_inst, W, F)"""
+
+    def __init__(self, n_inst, W, F, n_beam, max_words, H, n_layers, dev):
+        R = n_inst * n_beam
+        self.n_inst, self.R, self.Se = n_inst, R, W + F
+        self.am = torch.zeros(n_inst, W, dtype=torch.int64, device=dev)
+        self.vm = torch.zeros(n_inst, F, dtype=torch.int64, device=dev)
+        self.enc_mask = ops.MaskSpec(self.am, self.vm)
+        self.enc_kv = [torch.empty(n_inst * self.Se, 2 * H, dtype=BF16, device=dev) for _ in range(n_layers)]
+        # self-attention K|V: plane t holds the R rows decoded at position t (key slot t R + r)
+        self.planes = [torch.empty(max_words * R, 2 * H, dtype=BF16, device=dev) for _ in range(n_layers)]
+        self.anc = [torch.zeros(R, max_words, dtype=I32, device=dev) for _ in range(2)]
+        self.n_self = (torch.arange(1, max_words + 1, dtype=I32, device=dev)[:, None]).expand(max_words, R).contiguous()
+        self.live = [torch.ones(n_inst, dtype=I32, device=dev), torch.full((n_inst,), n_beam, dtype=I32, device=dev)]
+        self.tokens = torch.empty(R, dtype=torch.int64, device=dev)
+        self.score = torch.empty(R, dtype=torch.float32, device=dev)
+        self.done = torch.empty(n_inst, dtype=I32, device=dev)
+        self.tables = torch.empty(2, max_words, n_inst, n_beam, dtype=I32, device=dev)   # prev_k, word
+        self.lse = torch.empty(R, dtype=torch.float32, device=dev)
+        self.key = torch.empty(n_inst, n_beam, dtype=torch.float32, device=dev)
+        self.index = torch.empty(n_inst, n_beam, dtype=I32, device=dev)
+        self.ws = None
+        self.pool = torch.cuda.graph_pool_handle()
+        self.graphs = [None] * ((max_words + GRAPH_STEP_CHUNK - 1) // GRAPH_STEP_CHUNK)
+        self.warm = False
+
+
+class GraphBeamSearch:
+    """`beam_search` with the loop on the device: the same hypotheses and scores (up to the fp32 rounding of the
+    log-softmax), without a host round trip per token.
+
+    Per batch the cross encoder and every decoder layer's encoder K/V run once, into static buffers of the batch's
+    shape (n_inst, W, F).  Each token step then runs the decoder on all n_inst * n_beam rows: self-attention through
+    univl_attention_decode_fwd over the row's ancestor slots (t + 1 keys at step t; beams reorder by rewriting those
+    lists, no K/V is copied), encoder attention as CachedCaptionDecoder.step runs it, the FFN, the head transform, then
+    univl_vocab_beam_topk (no [rows, vocab] logits) and univl_beam_advance (scores, back-pointers, words, next tokens,
+    ancestor lists, done flags).  Steps are captured as CUDA graphs of GRAPH_STEP_CHUNK tokens, one set per shape, and
+    replayed for later batches; after each chunk the host reads once whether every instance is done.
+
+    An instance that is done stays in the batch frozen: its scores and step tables stop changing, and its rows keep
+    decoding valid inputs whose results are not used.  This equals `beam_search`, which drops finished instances,
+    because a decoder row's arithmetic does not depend on the other rows of the batch (tests/test_gpu_beam_graph.py
+    pins that on CachedCaptionDecoder).
+
+    The graphs hold the device pointers of the model's parameters and of its bf16 weight arena.  The arena is refreshed
+    in place from the parameters at every call (as every top-level entry does), so optimizer steps and load_state_dict
+    are seen; when any of those pointers changed, the graphs are captured again."""
+
+    def __init__(self, model, n_beam=5, max_words=20, bos=101, eos=102):
+        dec = model.decoder
+        n_pos = dec.embeddings.position_embeddings.weight.shape[0]
+        if not 1 <= int(n_beam) <= ops.BEAM_MAX:
+            raise ValueError("GraphBeamSearch: n_beam=%r must be in [1, %d]" % (n_beam, ops.BEAM_MAX))
+        if not 1 <= int(max_words) <= n_pos:
+            raise ValueError("GraphBeamSearch: max_words=%r must be in [1, %d] (the decoder's position table)"
+                             % (max_words, n_pos))
+        self.model = model
+        self.n_beam, self.max_words, self.bos, self.eos = int(n_beam), int(max_words), int(bos), int(eos)
+        self.H = dec.embeddings.word_embeddings.weight.shape[1]
+        self.n_cross_pos = model.cross.embeddings.position_embeddings.weight.shape[0]
+        self._shapes = {}
+        self._sig = None
+
+    def _check(self, seq, vis, am, vm):
+        if seq.dim() != 3 or vis.dim() != 3 or seq.shape[0] != vis.shape[0] or seq.shape[0] == 0:
+            raise ValueError("GraphBeamSearch: sequence_output [n, W, H] and visual_output [n, F, H] expected, got %s "
+                             "and %s" % (tuple(seq.shape), tuple(vis.shape)))
+        n, W, H = seq.shape
+        F = vis.shape[1]
+        if H != self.H or vis.shape[2] != self.H:
+            raise ValueError("GraphBeamSearch: hidden size %d / %d, the model's is %d" % (H, vis.shape[2], self.H))
+        if am.numel() != n * W or vm.numel() != n * F:
+            raise ValueError("GraphBeamSearch: input_mask %s / video_mask %s do not match W=%d, F=%d"
+                             % (tuple(am.shape), tuple(vm.shape), W, F))
+        if W + F > self.n_cross_pos:
+            raise ValueError("GraphBeamSearch: W + F = %d exceeds the cross encoder's %d positions"
+                             % (W + F, self.n_cross_pos))
+        return n, W, F
+
+    def _signature(self, arena):
+        return (arena.buf.data_ptr(), tuple(p.data_ptr() for p in self.model.decoder.parameters()))
+
+    @torch.no_grad()
+    def __call__(self, sequence_output, visual_output, input_mask, video_mask):
+        """-> (hypotheses: list over instances of the best token-id list (without [CLS]), scores: list of floats), as
+        `beam_search` returns them"""
+        model = self.model
+        if model.training:
+            raise RuntimeError("GraphBeamSearch: call model.eval() first")
+        n, W, F = self._check(sequence_output, visual_output, input_mask, video_mask)
+        dev = sequence_output.device
+        with rt.use_model(model, dev) as arena:
+            sig = self._signature(arena)
+            if sig != self._sig:
+                self._shapes = {}
+                self._sig = sig
+            g = self._shapes.get((n, W, F))
+            if g is None:
+                g = _BeamGraphs(n, W, F, self.n_beam, self.max_words, self.H, len(model.decoder.decoder.layer), dev)
+                self._shapes[(n, W, F)] = g
+            self._prologue(g, sequence_output, visual_output, input_mask, video_mask)
+            if not g.warm:
+                # one eager step first: every kernel's one-time set-up happens outside the capture
+                self._reset(g)
+                self._step(g, 0)
+                g.warm = True
+            self._reset(g)
+            steps = 0
+            for c in range(len(g.graphs)):
+                if g.graphs[c] is None:
+                    graph = torch.cuda.CUDAGraph()
+                    with torch.cuda.graph(graph, pool=g.pool):
+                        for t in range(c * GRAPH_STEP_CHUNK, min((c + 1) * GRAPH_STEP_CHUNK, self.max_words)):
+                            self._step(g, t)
+                    g.graphs[c] = graph
+                g.graphs[c].replay()
+                steps = min((c + 1) * GRAPH_STEP_CHUNK, self.max_words)
+                if bool(g.done.all()):
+                    break
+            scores = g.score.view(n, self.n_beam)
+            order = scores.argsort(dim=1, descending=True)
+            tables = g.tables[:, :steps].cpu()
+            order_c, scores_c = order.cpu(), scores.cpu()
+        return self._hypotheses(tables[0], tables[1], order_c, scores_c)
+
+    def _prologue(self, g, seq, vis, am, vm):
+        """the batch's encoder side into g's static buffers: the masks, the cross encoder once, each decoder layer's
+        encoder K/V once"""
+        model, H = self.model, self.H
+        g.am.copy_(am.reshape(g.n_inst, -1))
+        g.vm.copy_(vm.reshape(g.n_inst, -1))
+        seq2d = seq.to(BF16).reshape(-1, H).contiguous()
+        vis2d = vis.to(BF16).reshape(-1, H).contiguous()
+        enc2d, _, _ = model._cross_pairs(seq2d, vis2d, g.am, g.vm, False)
+        arena = rt.current()
+        for li, layer in enumerate(model.decoder.decoder.layer):
+            att = layer.enc_attn.att
+            wqkv = arena.bf16_qkv(att.query.weight, att.key.weight, att.value.weight)
+            ops.gemm(enc2d, wqkv[H:], enc2d.shape[0], 2 * H, H, g.enc_kv[li],
+                     bias=rt.packed_bias(att.key.bias, att.value.bias))
+
+    def _reset(self, g):
+        """the beam state before step 0: every row's input is [CLS], scores 0, nothing done, and row r's only
+        ancestor slot is its own position-0 row"""
+        g.tokens.fill_(self.bos)
+        g.score.zero_()
+        g.done.zero_()
+        g.tables.zero_()
+        g.anc[0][:, 0] = torch.arange(g.R, dtype=I32, device=g.anc[0].device)
+
+    def _step(self, g, t):
+        """decoder position t on all rows, then the beam top-k and bookkeeping of token t + 1 (graph-capturable: no
+        host read, no shape that depends on device data)"""
+        dec, H, R = self.model.decoder, self.H, g.R
+        arena = rt.current()
+        emb = dec.embeddings
+        x = ops.EmbedTextFn.apply(g.tokens.view(R, 1), None, emb.word_embeddings.weight,
+                                  emb.position_embeddings.weight[t:], None, emb.LayerNorm.weight, emb.LayerNorm.bias,
+                                  0.0, False)
+        anc = g.anc[t % 2]
+        for li, layer in enumerate(dec.decoder.layer):
+            att, out = layer.slf_attn.att, layer.slf_attn.output
+            wqkv = arena.bf16_qkv(att.query.weight, att.key.weight, att.value.weight)
+            qkv = ops.linear_fwd(x, wqkv, rt.packed_bias(att.query.bias, att.key.bias, att.value.bias))
+            plane = g.planes[li]
+            plane[t * R:(t + 1) * R] = qkv[:, H:]
+            ctx = ops.attention_decode_fwd(qkv[:, :H], plane, anc, g.n_self[t])
+            ao = ops.linear_fwd(ctx, arena.bf16(out.dense.weight), out.dense.bias)
+            x, _, _ = ops.layernorm_fwd(ao, x, out.LayerNorm.weight, out.LayerNorm.bias)
+            att, out = layer.enc_attn.att, layer.enc_attn.output
+            wqkv = arena.bf16_qkv(att.query.weight, att.key.weight, att.value.weight)
+            q = ops.linear_fwd(x, wqkv[:H], att.query.bias)
+            kv = g.enc_kv[li]
+            ctx, _ = ops.attention_fwd(q, kv[:, :H], kv[:, H:], g.n_inst, self.n_beam, g.Se, g.enc_mask)
+            ao = ops.linear_fwd(ctx, arena.bf16(out.dense.weight), out.dense.bias)
+            x, _, _ = ops.layernorm_fwd(ao, x, out.LayerNorm.weight, out.LayerNorm.bias)
+            w1, w2 = arena.bf16(layer.intermediate.dense.weight), arena.bf16(layer.output.dense.weight)
+            pre = torch.empty(R, w1.shape[0], dtype=BF16, device=x.device)
+            h = ops.linear_fwd(x, w1, layer.intermediate.dense.bias, epi=ops.EPI_GELU, aux_out=pre)
+            fo = ops.linear_fwd(h, w2, layer.output.dense.bias)
+            x, _, _ = ops.layernorm_fwd(fo, x, layer.output.LayerNorm.weight, layer.output.LayerNorm.bias)
+        head = dec.classifier.cls.predictions
+        w16 = arena.bf16(head.decoder.weight)
+        if g.ws is None:
+            g.ws = ops.vocab_beam_topk_workspace(g.n_inst, self.n_beam, w16.shape[0], x)
+        ops.vocab_beam_topk(head.transform.run(x), w16, head.bias, g.score, g.live[min(t, 1)], self.n_beam, g.ws,
+                            out=(g.lse, g.key, g.index))
+        ops.beam_advance(g.key, g.index, w16.shape[0], t, self.eos, g.score, g.done, g.tables[0], g.tables[1],
+                         g.tokens, anc, g.anc[(t + 1) % 2])
+
+    def _hypotheses(self, ks, ys, order, scores):
+        """walk the back-pointers from each instance's top-scoring beam, stopping at the step it finished, as
+        `beam_search` does"""
+        ks, ys, order, scores = ks.tolist(), ys.tolist(), order.tolist(), scores.tolist()   # no per-element tensor reads
+        hyps, outs = [], []
+        n_steps = len(ks)
+        for i in range(len(order)):
+            last = n_steps
+            for s in range(n_steps):
+                if ys[s][i][0] == self.eos:
+                    last = s + 1
+                    break
+            k = order[i][0]
+            hyp = []
+            for j in range(last - 1, -1, -1):
+                hyp.append(ys[j][i][k])
+                k = ks[j][i][k]
+            hyps.append(hyp[::-1])
+            outs.append(scores[i][order[i][0]])
+        return hyps, outs

@@ -36,6 +36,7 @@
 #include "pipeline.cuh"
 #include "tmap.cuh"
 
+#include <climits>
 #include <stdio.h>
 #include <type_traits>
 
@@ -827,16 +828,44 @@ static int launch_gemm_fp8(const CUtensorMap& ta, const CUtensorMap& tb, const G
 // The mainloop is the bf16 kernel's cooperative one on 128 x 128 tiles (both operands K-major), so every logit has the
 // bits EPI_BIAS_F32 gives it: the same k16 wgmma chain and the same fp32 bias add.  A work item is one 128-row tile x
 // a chunk of VX_CHUNK consecutive 128-column tiles; the CTA walks the chunk's tiles in column order.
-//   forward  (BWD = false): each thread keeps, per row of its fragment, a running max m and sum s of exp(logit - m)
+//   forward  (MODE = VX_FWD): each thread keeps, per row of its fragment, a running max m and sum s of exp(logit - m)
 //            over the columns it holds, updated tile by tile; at the end of the item the four lanes of a quad fold
 //            their (m, s) with two xor shuffles (symmetric, so every lane gets the same bits) and lane 0 writes the
 //            row's (m, s, label logit) for the chunk.  vocab_xent_rows_kernel folds the chunks in chunk order.
-//   backward (BWD = true):  dl[r, c] = (exp(logit - lse[r]) - [c == label]) * g(r) as bf16, the arithmetic of
+//            Without labels every row is scored (the beam search's lse pass) and no label logit is taken.
+//   backward (MODE = VX_BWD):  dl[r, c] = (exp(logit - lse[r]) - [c == label]) * g(r) as bf16, the arithmetic of
 //            xent_bwd_kernel; columns [V, ld_d) and rows with label -1 get 0.
+//   beam     (MODE = VX_BEAM): key = (logit - lse[r]) + score[r] for every column c < V (Beam.advance's word_prob +
+//            scores); each thread keeps its row's VX_BEAM_MAX best (key, c) in registers, in the order key descending
+//            then c ascending; at the end of the item the four lanes of a quad merge their lists with shuffles and
+//            lane 0 writes the row's list for the chunk.  vocab_beam_merge_kernel takes an instance's top n_beam from
+//            its live rows' lists.
 // The chunking is a pure function of (T, V) (vx_plan), never of the SMs in use, so the bits do not depend on the
 // grid, reserved SMs or which CTA runs an item.
 constexpr int VX_BLOCK_N = 128;
 constexpr int VX_STAGES = 6;
+constexpr int VX_FWD = 0, VX_BWD = 1, VX_BEAM = 2;
+constexpr int VX_BEAM_MAX = 8;  // candidates a beam work item keeps per row: the largest n_beam
+
+// (k1, i1) comes before (k2, i2) in the beam order: key descending, then index ascending (a total order on distinct
+// indices, so every selection by it is exact)
+__device__ __forceinline__ bool vb_before(float k1, int i1, float k2, int i2) {
+  return k1 > k2 || (k1 == k2 && i1 < i2);
+}
+
+// insert (key, idx) into the sorted list (k, ix) if it beats the last entry; the list stays sorted by vb_before
+__device__ __forceinline__ void vb_insert(float (&k)[VX_BEAM_MAX], int (&ix)[VX_BEAM_MAX], float key, int idx) {
+  if (!vb_before(key, idx, k[VX_BEAM_MAX - 1], ix[VX_BEAM_MAX - 1])) return;
+  k[VX_BEAM_MAX - 1] = key;
+  ix[VX_BEAM_MAX - 1] = idx;
+#pragma unroll
+  for (int i = VX_BEAM_MAX - 1; i > 0; --i) {
+    if (vb_before(k[i], ix[i], k[i - 1], ix[i - 1])) {
+      const float tk = k[i]; k[i] = k[i - 1]; k[i - 1] = tk;
+      const int ti = ix[i]; ix[i] = ix[i - 1]; ix[i - 1] = ti;
+    }
+  }
+}
 
 struct VocabXentParams {
   int T, V, Kc;
@@ -844,8 +873,11 @@ struct VocabXentParams {
   const float* bias;        // nullable
   const long long* labels;  // [T], -1 = not scored
   float4* part;             // forward: [T, chunks] (m, s, label logit, 0)
-  // backward
+  // backward and beam
   const float* lse;
+  // beam
+  const float* score;  // [T]
+  int2* cand;          // [T, chunks, VX_BEAM_MAX] (key bits, column); unfilled entries (-inf, INT_MAX)
   const float* count;   // [groups]
   const float* gscale;  // nullable: 1
   int rows_per_group, groups;
@@ -853,7 +885,7 @@ struct VocabXentParams {
   long long ld_d;
 };
 
-template <bool BWD>
+template <int MODE>
 __global__ void __launch_bounds__(PIPELINE_THREADS, 1)
 vocab_xent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                   const VocabXentParams p, const int num_work) {
@@ -891,15 +923,26 @@ vocab_xent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     const int chunk = w / p.m_tiles;
     const int row = (w - chunk * p.m_tiles) * BLOCK_M + c * 64 + warp * 16 + (lane >> 2);  // and row + 8
     long long lab[2];
-    float m[2], s[2], xt[2], lse[2], g[2];
+    float m[2], s[2], xt[2], lse[2], g[2], sc[2];
+    float bk[2][VX_BEAM_MAX];
+    int bi[2][VX_BEAM_MAX];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int r = row + 8 * h;
-      lab[h] = r < p.T ? __ldg(p.labels + r) : -1;
+      lab[h] = (r < p.T && p.labels != nullptr) ? __ldg(p.labels + r) : -1;
       m[h] = -INFINITY;
       s[h] = 0.f;
       xt[h] = 0.f;
-      if constexpr (BWD) {
+      if constexpr (MODE == VX_BEAM) {
+        lse[h] = r < p.T ? __ldg(p.lse + r) : 0.f;
+        sc[h] = r < p.T ? __ldg(p.score + r) : 0.f;
+#pragma unroll
+        for (int i = 0; i < VX_BEAM_MAX; ++i) {
+          bk[h][i] = -INFINITY;
+          bi[h][i] = INT_MAX;
+        }
+      }
+      if constexpr (MODE == VX_BWD) {
         lse[h] = 0.f;
         g[h] = 0.f;
         if (lab[h] != -1) {
@@ -930,7 +973,7 @@ vocab_xent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
           acc[4 * j + 2 + e] = __fadd_rn(acc[4 * j + 2 + e], b);
         }
       }
-      if constexpr (!BWD) {
+      if constexpr (MODE == VX_FWD) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           float tm = -INFINITY;
@@ -953,6 +996,17 @@ vocab_xent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
               if (col == lab[h]) xt[h] = v;
             }
         }
+      } else if constexpr (MODE == VX_BEAM) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int j = 0; j < VX_BLOCK_N / 8; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int col = col0 + 8 * j + e;
+              if (col < p.V)
+                vb_insert(bk[h], bi[h], __fadd_rn(__fsub_rn(acc[4 * j + 2 * h + e], lse[h]), sc[h]), col);
+            }
       } else {
         const int ncol = min(p.ld_d - (long long)nt * VX_BLOCK_N, (long long)VX_BLOCK_N);  // this tile's columns
 #pragma unroll
@@ -977,7 +1031,32 @@ vocab_xent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         }
       }
     }
-    if constexpr (!BWD) {
+    if constexpr (MODE == VX_BEAM) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        // merge with the partner lane's list: the top VX_BEAM_MAX of the union in the strict order, so both lanes of
+        // the pair (and then all four of the quad) hold the same list
+#pragma unroll
+        for (int o = 1; o <= 2; o <<= 1) {
+          float ok[VX_BEAM_MAX];
+          int oi[VX_BEAM_MAX];
+#pragma unroll
+          for (int i = 0; i < VX_BEAM_MAX; ++i) {
+            ok[i] = __shfl_xor_sync(0xffffffffu, bk[h][i], o);
+            oi[i] = __shfl_xor_sync(0xffffffffu, bi[h][i], o);
+          }
+#pragma unroll
+          for (int i = 0; i < VX_BEAM_MAX; ++i) vb_insert(bk[h], bi[h], ok[i], oi[i]);
+        }
+        const int r = row + 8 * h;
+        if (q == 0 && r < p.T) {
+          int2* out = p.cand + ((long long)r * p.chunks + chunk) * VX_BEAM_MAX;
+#pragma unroll
+          for (int i = 0; i < VX_BEAM_MAX; ++i) out[i] = make_int2(__float_as_int(bk[h][i]), bi[h][i]);
+        }
+      }
+    }
+    if constexpr (MODE == VX_FWD) {
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
 #pragma unroll
@@ -1000,13 +1079,14 @@ vocab_xent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
 }
 
 // Row r (one thread each): fold its chunk records in chunk order into lse[r] = m + log(s) and nll[r] = lse[r] - the
-// label logit, taken from the label's chunk.  Rows with label -1 get lse 0, as xent_fwd_kernel gives them.
+// label logit, taken from the label's chunk.  Rows with label -1 get lse 0, as xent_fwd_kernel gives them.  Without
+// labels (null) every row gets its lse and no nll is written.
 __global__ void __launch_bounds__(256)
 vocab_xent_rows_kernel(const float4* __restrict__ part, const long long* __restrict__ labels, int T, int V, int chunks,
                        int chunk_cols, float* __restrict__ lse_out, float* __restrict__ nll) {
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= T) return;
-  const long long lab = labels[r];
+  const long long lab = labels != nullptr ? labels[r] : 0;
   if (lab == -1) {
     lse_out[r] = 0.f;
     return;
@@ -1022,6 +1102,7 @@ vocab_xent_rows_kernel(const float4* __restrict__ part, const long long* __restr
   }
   const float lse = m + __logf(s);
   lse_out[r] = lse;
+  if (labels == nullptr) return;
   // a label outside [0, V) scores NaN instead of reading past the row
   nll[r] = (lab >= 0 && lab < V) ? lse - pr[lab / chunk_cols].z : __int_as_float(0x7fc00000);
 }
@@ -1063,13 +1144,120 @@ __global__ void vocab_xent_mean_kernel(const float* __restrict__ sum_count, int 
   *out = groups > 1 ? acc / (float)groups : acc;
 }
 
+// Instance i (one CTA each): its n_beam best candidates from the lists of its live rows i n_beam + k, k < n_live[i]
+// (clamped to [0, n_beam]), as (key, flat = k V + c) in the beam order.  Round j takes the best candidate after round
+// j - 1's in that order: each thread scans a fixed stride of the lists, then a fixed-shape tree picks the block's best,
+// so the result is the exact top n_beam whatever the chunking.  Slots without a candidate get (-inf, -1).
+constexpr int VB_MERGE_THREADS = 256;
+__global__ void __launch_bounds__(VB_MERGE_THREADS)
+vocab_beam_merge_kernel(const int2* __restrict__ cand, const int* __restrict__ n_live, int n_beam, int chunks, int V,
+                        float* __restrict__ out_key, int* __restrict__ out_index) {
+  __shared__ float sk[VB_MERGE_THREADS / 32];
+  __shared__ int si[VB_MERGE_THREADS / 32];
+  const int inst = blockIdx.x;
+  const int live = min(max(__ldg(n_live + inst), 0), n_beam);
+  const int per_row = chunks * VX_BEAM_MAX;
+  const int n = live * per_row;
+  const int2* base = cand + (long long)inst * n_beam * per_row;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  float pk = INFINITY;  // the previous round's pick (none yet: every candidate comes after (+inf, -1))
+  int pi = -1;
+  for (int j = 0; j < n_beam; ++j) {
+    float bk = -INFINITY;
+    int bi = INT_MAX;
+    for (int e = threadIdx.x; e < n; e += VB_MERGE_THREADS) {
+      const int2 c = base[e];
+      if (c.y == INT_MAX) continue;  // an unfilled slot
+      const float k = __int_as_float(c.x);
+      const int flat = (e / per_row) * V + c.y;
+      if (vb_before(pk, pi, k, flat) && vb_before(k, flat, bk, bi)) {
+        bk = k;
+        bi = flat;
+      }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float ok = __shfl_xor_sync(0xffffffffu, bk, o);
+      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+      if (vb_before(ok, oi, bk, bi)) {
+        bk = ok;
+        bi = oi;
+      }
+    }
+    if (lane == 0) {
+      sk[warp] = bk;
+      si[warp] = bi;
+    }
+    __syncthreads();
+    bk = sk[0];
+    bi = si[0];
+    for (int w = 1; w < VB_MERGE_THREADS / 32; ++w)
+      if (vb_before(sk[w], si[w], bk, bi)) {
+        bk = sk[w];
+        bi = si[w];
+      }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      out_key[inst * n_beam + j] = bk;
+      out_index[inst * n_beam + j] = bi == INT_MAX ? -1 : bi;
+    }
+    pk = bk;
+    pi = bi;
+  }
+}
+
+// One beam step's bookkeeping for instance i (one CTA each), after vocab_beam_merge_kernel (Beam.advance,
+// modules/beam.py:63-87).  A live instance takes its n_beam picks: hypothesis j continues row k = flat / V of the
+// instance with word c = flat mod V, score[i n_beam + j] = key, prev_k[t, i, j] = k, word[t, i, j] = c and the row's
+// next input token is c; the instance is done when its top pick's word is eos.  A done instance changes none of these.
+// Every row r = i n_beam + j then gets its ancestor list for step t + 1: its parent's (row i n_beam + k, or r itself
+// when the instance is done) first t + 1 entries, then its own slot (t + 1) R + r, R = n_inst n_beam.
+__global__ void __launch_bounds__(128)
+beam_advance_kernel(const float* __restrict__ key, const int* __restrict__ index, int n_beam, int V, int t,
+                    long long eos, float* __restrict__ score, int* __restrict__ done,
+                    int* __restrict__ prev_k, int* __restrict__ word, long long* __restrict__ tokens,
+                    const int* __restrict__ anc_in, int* __restrict__ anc_out, int ld_anc) {
+  __shared__ int parent[VX_BEAM_MAX];
+  const int inst = blockIdx.x, n_inst = gridDim.x;
+  const int R = n_inst * n_beam;
+  const bool frozen = done[inst] != 0;
+  if (threadIdx.x < n_beam) {
+    const int j = threadIdx.x, r = inst * n_beam + j;
+    int k = j;
+    if (!frozen) {
+      const int flat = index[r];
+      k = flat / V;
+      const int c = flat - k * V;
+      score[r] = key[r];
+      prev_k[((long long)t * n_inst + inst) * n_beam + j] = k;
+      word[((long long)t * n_inst + inst) * n_beam + j] = c;
+      tokens[r] = c;
+    }
+    parent[j] = inst * n_beam + k;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0 && !frozen && index[inst * n_beam] % V == eos) done[inst] = 1;
+  const int len = min(t + 2, ld_anc);
+  for (int e = threadIdx.x; e < n_beam * len; e += blockDim.x) {
+    const int j = e / len, pos = e - j * len;
+    const int r = inst * n_beam + j;
+    anc_out[(long long)r * ld_anc + pos] =
+        pos <= t ? anc_in[(long long)parent[j] * ld_anc + pos] : (t + 1) * R + r;
+  }
+}
+
 // after vx_params, which runs persistent_prepare
-template <bool BWD>
+template <int MODE>
+static const char* vx_name() {
+  return MODE == VX_FWD ? "univl_vocab_xent_fwd" : MODE == VX_BWD ? "univl_vocab_xent_bwd" : "univl_vocab_beam_topk";
+}
+
+template <int MODE>
 static int launch_vocab_xent(const CUtensorMap& ta, const CUtensorMap& tb, const VocabXentParams& p,
                              cudaStream_t stream) {
   const long long work = (long long)p.m_tiles * p.chunks;
-  return persistent_launch(vocab_xent_kernel<BWD>, BWD ? "univl_vocab_xent_bwd" : "univl_vocab_xent_fwd", work,
-                           GemmSmem<VX_BLOCK_N, VX_STAGES>::DYN_BYTES, stream, ta, tb, p, (int)work);
+  return persistent_launch(vocab_xent_kernel<MODE>, vx_name<MODE>(), work, GemmSmem<VX_BLOCK_N, VX_STAGES>::DYN_BYTES,
+                           stream, ta, tb, p, (int)work);
 }
 
 }  // namespace univl
@@ -1324,11 +1512,10 @@ int vx_check(const char* name, const void* x, long long ldx, const void* w, long
 // Runs persistent_prepare first: a runtime call, which also makes the device's primary context current on this thread
 // before the driver encodes the tensor maps (autograd runs backward on a thread of its own, where this may be the
 // first call of the process into CUDA).
-template <bool BWD>
+template <int MODE>
 int vx_params(const void* x, long long ldx, const void* w, long long ldw, int T, int V, int Kc, CUtensorMap* ta,
               CUtensorMap* tb, VocabXentParams* p) {
-  if (int rc = persistent_prepare(vocab_xent_kernel<BWD>, GemmSmem<VX_BLOCK_N, VX_STAGES>::DYN_BYTES,
-                                  BWD ? "univl_vocab_xent_bwd" : "univl_vocab_xent_fwd"))
+  if (int rc = persistent_prepare(vocab_xent_kernel<MODE>, GemmSmem<VX_BLOCK_N, VX_STAGES>::DYN_BYTES, vx_name<MODE>()))
     return rc;
   const VxPlan pl = vx_plan(T, V);
   int rc;
@@ -1370,11 +1557,11 @@ extern "C" int univl_vocab_xent_fwd(const void* x, long long ldx, const void* w,
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   CUtensorMap ta, tb;
   VocabXentParams p;
-  if (int rc = vx_params<false>(x, ldx, w, ldw, T, V, Kc, &ta, &tb, &p)) return rc;
+  if (int rc = vx_params<VX_FWD>(x, ldx, w, ldw, T, V, Kc, &ta, &tb, &p)) return rc;
   p.bias = bias;
   p.labels = labels;
   p.part = reinterpret_cast<float4*>(workspace);
-  if (int rc = launch_vocab_xent<false>(ta, tb, p, stream)) return rc;
+  if (int rc = launch_vocab_xent<VX_FWD>(ta, tb, p, stream)) return rc;
   float* nll = reinterpret_cast<float*>(p.part + (long long)T * p.chunks);
   vocab_xent_rows_kernel<<<(T + 255) / 256, 256, 0, stream>>>(p.part, labels, T, V, p.chunks,
                                                                p.chunk_tiles * VX_BLOCK_N, lse, nll);
@@ -1398,7 +1585,7 @@ extern "C" int univl_vocab_xent_bwd(const void* x, long long ldx, const void* w,
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   CUtensorMap ta, tb;
   VocabXentParams p;
-  if (int rc = vx_params<true>(x, ldx, w, ldw, T, V, Kc, &ta, &tb, &p)) return rc;
+  if (int rc = vx_params<VX_BWD>(x, ldx, w, ldw, T, V, Kc, &ta, &tb, &p)) return rc;
   p.bias = bias;
   p.labels = labels;
   p.lse = lse;
@@ -1408,5 +1595,82 @@ extern "C" int univl_vocab_xent_bwd(const void* x, long long ldx, const void* w,
   p.groups = groups;
   p.dl = reinterpret_cast<bf16*>(dlogits);
   p.ld_d = ld_d;
-  return launch_vocab_xent<true>(ta, tb, p, stream);
+  return launch_vocab_xent<VX_BWD>(ta, tb, p, stream);
+}
+
+namespace {
+// workspace of univl_vocab_beam_topk: the lse pass's 16-byte record per row and chunk, then the selection pass's
+// VX_BEAM_MAX 8-byte candidates per row and chunk
+long long vb_workspace_bytes(int R, int V) {
+  return (long long)R * vx_plan(R, V).chunks * (long long)(sizeof(float4) + VX_BEAM_MAX * sizeof(int2));
+}
+}  // namespace
+
+extern "C" int univl_vocab_beam_topk_workspace(int n_inst, int n_beam, int V) {
+  UNIVL_CHECK_ARG(n_inst > 0 && V > 0 && n_beam >= 1 && n_beam <= VX_BEAM_MAX,
+                  "univl_vocab_beam_topk_workspace: n_inst=%d V=%d n_beam=%d (1 <= n_beam <= %d)", n_inst, V, n_beam,
+                  VX_BEAM_MAX);
+  const long long bytes = vb_workspace_bytes(n_inst * n_beam, V);
+  UNIVL_CHECK_ARG(bytes <= 0x7fffffffLL, "univl_vocab_beam_topk_workspace: n_inst=%d V=%d needs over 2 GiB", n_inst, V);
+  return (int)bytes;
+}
+
+extern "C" int univl_vocab_beam_topk(const void* x, long long ldx, const void* w, long long ldw, const float* bias,
+                                     const float* score, const int* n_live, int n_inst, int n_beam, int V, int Kc,
+                                     float* lse, float* out_key, int* out_index, void* workspace,
+                                     long long workspace_bytes, void* stream_) {
+  const char* name = "univl_vocab_beam_topk";
+  UNIVL_CHECK_ARG(n_beam >= 1 && n_beam <= VX_BEAM_MAX, "%s: n_beam=%d outside [1, %d]", name, n_beam, VX_BEAM_MAX);
+  UNIVL_CHECK_ARG(n_inst > 0 && Kc > 0 && V >= n_beam && (long long)n_beam * V <= 0x7fffffffLL,
+                  "%s: n_inst=%d K=%d V=%d (n_beam <= V, n_beam V < 2^31)", name, n_inst, Kc, V);
+  UNIVL_CHECK_ARG(x && w && score && n_live && lse && out_key && out_index && workspace,
+                  "%s: null x, W, score, n_live, lse, out_key, out_index or workspace", name);
+  UNIVL_CHECK_ARG(ldx >= Kc && ldw >= Kc && (ldx % 8) == 0 && (ldw % 8) == 0,
+                  "%s: ldx/ldw must be >= K and multiples of 8 (got %lld, %lld, K=%d)", name, ldx, ldw, Kc);
+  UNIVL_CHECK_ARG(((uintptr_t)x & 15) == 0 && ((uintptr_t)w & 15) == 0 && ((uintptr_t)workspace & 15) == 0,
+                  "%s: x, W and the workspace must be 16-byte aligned", name);
+  const int R = n_inst * n_beam;
+  const long long need = vb_workspace_bytes(R, V);
+  UNIVL_CHECK_ARG(workspace_bytes >= need, "%s: workspace of %lld bytes, needs %lld (univl_vocab_beam_topk_workspace)",
+                  name, workspace_bytes, need);
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  CUtensorMap ta, tb;
+  VocabXentParams p;
+  // pass 1: every row's lse, folded as the cross-entropy forward folds it
+  if (int rc = vx_params<VX_FWD>(x, ldx, w, ldw, R, V, Kc, &ta, &tb, &p)) return rc;
+  p.bias = bias;
+  p.part = reinterpret_cast<float4*>(workspace);
+  if (int rc = launch_vocab_xent<VX_FWD>(ta, tb, p, stream)) return rc;
+  vocab_xent_rows_kernel<<<(R + 255) / 256, 256, 0, stream>>>(p.part, nullptr, R, V, p.chunks,
+                                                               p.chunk_tiles * VX_BLOCK_N, lse, nullptr);
+  UNIVL_CHECK_LAUNCH(name);
+  // pass 2: the logits again, each row's best keys per chunk, then each instance's top n_beam
+  float4* part = p.part;
+  if (int rc = vx_params<VX_BEAM>(x, ldx, w, ldw, R, V, Kc, &ta, &tb, &p)) return rc;
+  p.bias = bias;
+  p.lse = lse;
+  p.score = score;
+  p.cand = reinterpret_cast<int2*>(part + (long long)R * p.chunks);
+  if (int rc = launch_vocab_xent<VX_BEAM>(ta, tb, p, stream)) return rc;
+  vocab_beam_merge_kernel<<<n_inst, VB_MERGE_THREADS, 0, stream>>>(p.cand, n_live, n_beam, p.chunks, V, out_key,
+                                                                   out_index);
+  UNIVL_CHECK_LAUNCH(name);
+  return UNIVL_OK;
+}
+
+extern "C" int univl_beam_advance(const float* key, const int* index, int n_inst, int n_beam, int V, int t,
+                                  int max_words, long long eos, float* score, int* done, int* prev_k, int* word,
+                                  long long* tokens, const int* anc_in, int* anc_out, void* stream_) {
+  const char* name = "univl_beam_advance";
+  UNIVL_CHECK_ARG(n_beam >= 1 && n_beam <= VX_BEAM_MAX, "%s: n_beam=%d outside [1, %d]", name, n_beam, VX_BEAM_MAX);
+  UNIVL_CHECK_ARG(n_inst > 0 && V > 0 && t >= 0 && t < max_words, "%s: n_inst=%d V=%d t=%d max_words=%d", name, n_inst,
+                  V, t, max_words);
+  UNIVL_CHECK_ARG((long long)max_words * n_inst * n_beam <= 0x7fffffffLL, "%s: max_words x rows must be < 2^31", name);
+  UNIVL_CHECK_ARG(key && index && score && done && prev_k && word && tokens && anc_in && anc_out && anc_in != anc_out,
+                  "%s: null pointer, or anc_in == anc_out", name);
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  beam_advance_kernel<<<n_inst, 128, 0, stream>>>(key, index, n_beam, V, t, eos, score, done, prev_k, word,
+                                                  tokens, anc_in, anc_out, max_words);
+  UNIVL_CHECK_LAUNCH(name);
+  return UNIVL_OK;
 }

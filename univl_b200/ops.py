@@ -1137,6 +1137,49 @@ def vocab_xent_bwd(x, w16, bias, labels, lse, sc, g, groups):
     return dl
 
 
+BEAM_MAX = 8  # largest n_beam univl_vocab_beam_topk takes
+
+
+def vocab_beam_topk_workspace(n_inst, n_beam, V, like):
+    """uint8 workspace for vocab_beam_topk on like's device"""
+    nbytes = lib.load().univl_vocab_beam_topk_workspace(int(n_inst), int(n_beam), int(V))
+    if nbytes < 0:
+        raise RuntimeError("univl_vocab_beam_topk_workspace failed: %s" % lib.load().univl_last_error_string().decode())
+    return _empty((nbytes,), torch.uint8, like)
+
+
+def vocab_beam_topk(x, w16, bias, score, n_live, n_beam, workspace=None, out=None):
+    """One beam step's top n_beam per instance over the vocabulary, without logits (csrc/gemm_wgmma.cu): x bf16
+    [n_inst * n_beam, K] (the head transform), w16 [V, K], bias fp32 [V], score fp32 [n_inst * n_beam], n_live int32
+    [n_inst].  -> (lse fp32 [R], key fp32 [n_inst, n_beam], index int32 [n_inst, n_beam]); index = k * V + c for row k
+    of the instance and word c, ordered by key descending then index ascending.  `out` = (lse, key, index) to write."""
+    _check2d(x, "vocab_beam_topk x"); _check2d(w16, "vocab_beam_topk W")
+    R, K = x.shape
+    V = w16.shape[0]
+    if not 1 <= n_beam <= BEAM_MAX or R % n_beam:
+        raise ValueError("vocab_beam_topk: n_beam=%d must be in [1, %d] and divide the %d rows" % (n_beam, BEAM_MAX, R))
+    n_inst = R // n_beam
+    if workspace is None:
+        workspace = vocab_beam_topk_workspace(n_inst, n_beam, V, x)
+    if out is None:
+        out = (_empty((R,), F32, x), _empty((n_inst, n_beam), F32, x), _empty((n_inst, n_beam), I32, x))
+    lse, key, index = out
+    call("univl_vocab_beam_topk", x.data_ptr(), x.stride(0), w16.data_ptr(), w16.stride(0), ptr(bias),
+         score.data_ptr(), n_live.data_ptr(), n_inst, n_beam, V, K, lse.data_ptr(), key.data_ptr(), index.data_ptr(),
+         workspace.data_ptr(), workspace.numel())
+    return lse, key, index
+
+
+def beam_advance(key, index, V, t, eos, score, done, prev_k, word, tokens, anc_in, anc_out):
+    """The bookkeeping of beam step t (csrc/gemm_wgmma.cu, univl_beam_advance): in place on score fp32 [R], done int32
+    [n_inst], the step tables prev_k / word int32 [max_words, n_inst, n_beam], tokens int64 [R] and anc_out int32
+    [R, max_words] (row r's self-attention key slots for step t + 1, from anc_in)"""
+    n_inst, n_beam = key.shape
+    call("univl_beam_advance", key.data_ptr(), index.data_ptr(), n_inst, n_beam, int(V), int(t), prev_k.shape[0],
+         int(eos), score.data_ptr(), done.data_ptr(), prev_k.data_ptr(), word.data_ptr(), tokens.data_ptr(),
+         anc_in.data_ptr(), anc_out.data_ptr())
+
+
 class ProjXentFn(torch.autograd.Function):
     """loss = CrossEntropy(x W^T + bias, labels) without ever exposing logits to autograd: tied vocab projection
     (reference modules/module_bert.py:327-330) + CrossEntropyLoss(ignore_index=-1) (modeling.py:253, :275), or the MFM
