@@ -86,6 +86,10 @@ int univl_layernorm_bwd(const void* dy, const void* dy2, const void* x, const vo
 /* NormalizeVideo (modeling.py:88-92): fp32 rows in, bf16 out; backward yields parameter gradients only */
 int univl_layernorm_f32_fwd(const float* x, const float* gamma, const float* beta, void* y, float* mean, float* rstd,
                             int rows, int cols, float eps, void* stream);
+/* NormalizeVideo on gathered rows (packed evaluation): y bf16 [rows, cols] row r = LN(x[x_rows[r]]) (x_rows int32), with
+ * univl_layernorm_f32_fwd's kernel body, so each row has its bits; no statistics are written */
+int univl_layernorm_f32_rows_fwd(const float* x, const int* x_rows, const float* gamma, const float* beta, void* y,
+                                 int rows, int cols, float eps, void* stream);
 int univl_layernorm_f32_bwd(const void* dy, const float* x, const float* gamma, const float* mean, const float* rstd,
                             float* dgamma, float* dbeta, int rows, int cols, void* stream);
 
@@ -100,6 +104,12 @@ int univl_embed_text_bwd(const void* dy, const long long* ids, const long long* 
                          const float* rstd, float* dword, float* dpos, float* dtype, float* dgamma, float* dbeta,
                          int n_seq, int S, int H, int vocab, float p_drop, const unsigned long long* rng_state,
                          unsigned long long stream_id, void* stream);
+/* Evaluation on packed rows (no dropout, no statistics): row r of y is token idx[r] (int32, = i * S + s) of the
+ * [n_seq, S] id matrices, y[r] = LN(word[ids[idx[r]]] + pos[s] (+ type[type_ids[idx[r]]])) with univl_embed_text_fwd's
+ * arithmetic at p = 0, bit for bit. */
+int univl_embed_text_packed_fwd(const long long* ids, const long long* type_ids, const int* idx, int rows, int S,
+                                const float* word, const float* pos, const float* type, const float* gamma,
+                                const float* beta, void* y, int H, int vocab, float eps, void* stream);
 /* activation sources a[Na,Wa,H] (+ b[Nb,Fb,H]) + pos[s] (+ type[s>=Wa]) -> LN -> dropout
  * (module_visual.py:118-131; module_cross.py:123-138 with modeling.py:315-325).  `all_pairs` is the number of pairing
  * groups: 0 = aligned (sequence p reads a[p], b[p]; Na == Nb); 1 = the B x B text-video pairing of
@@ -111,6 +121,10 @@ int univl_embed_src_fwd(const void* a, const void* b, const float* pos, const fl
                         const float* beta, void* y, float* mean, float* rstd, int Na, int Wa, int Nb, int Fb,
                         int all_pairs, int H, float eps, float p_drop, const unsigned long long* rng_state,
                         unsigned long long stream_id, void* stream);
+/* Evaluation on packed rows: x bf16 [rows, H] holds token idx[r] (= j * S + s) of an aligned source, y[r] =
+ * LN(x[r] + pos[s]) as univl_embed_src_fwd (Fb = 0, visual embeddings) computes it at p = 0, bit for bit. */
+int univl_embed_src_packed_fwd(const void* x, const int* idx, int rows, int S, const float* pos, const float* gamma,
+                               const float* beta, void* y, int H, float eps, void* stream);
 int univl_embed_src_bwd(const void* dy, const void* a, const void* b, const float* pos, const float* type,
                         const float* gamma, const float* mean, const float* rstd, void* da, void* db, float* dpos,
                         float* dtype, float* dgamma, float* dbeta, int Na, int Wa, int Nb, int Fb, int all_pairs,
@@ -249,6 +263,11 @@ int univl_scale_f32(float* dst, const float* src, long long n, const float* gsca
  * masked mean pooling (modeling.py:327-339) [+ F.normalize, :386-388] */
 int univl_meanpool_fwd(const void* x, const long long* mask, float* out, float* norm_out, int N, int S, int H,
                        int skip_first, int guard_zero, int l2norm, void* stream);
+/* univl_meanpool_fwd on packed rows: sequence n is x rows [cu[n], cu[n + 1]) (int32 cu [N + 1]), row r holding token
+ * idx[r] = n' * S + s at position s (skip_first skips s = 0).  Fed the padded layout's valid rows in ascending position,
+ * out equals univl_meanpool_fwd's bit for bit, a sequence without pooled rows included. */
+int univl_meanpool_packed_fwd(const void* x, const int* cu, const int* idx, float* out, int N, int S, int H,
+                              int skip_first, int guard_zero, int l2norm, void* stream);
 int univl_meanpool_bwd(const float* dy, const float* y, const float* norm, const long long* mask, void* dx, int N,
                        int S, int H, int skip_first, int guard_zero, int l2norm, void* stream);
 /* sim = T V^T (modeling.py:389).  groups = G >= 1: t [G Bt, H], v [G Bv, H] and sim the block diagonal [G, Bt, Bv],

@@ -61,16 +61,16 @@ __device__ __forceinline__ void emb_keep8(const EmbDrop& d, uint64_t idx0, bool 
   for (int j = 0; j < 8; ++j) k[j] = (m >> j) & 1u;
 }
 
-// z (registers) -> mean/rstd -> y ; shared by both forward kernels
-__device__ __forceinline__ void ln_row_fwd(float (&z)[EMB_VEC][8], const float* gamma, const float* beta, bf16* yrow,
-                                           float* mean_out, float* rstd_out, long long row, float eps,
-                                           const EmbDrop& drop, int lane) {
+// z (registers) -> mean / rstd, and z <- gamma * ((z - mean) * rstd) + beta in place: the LayerNorm of every forward
+// kernel here, so the packed evaluation kernels give the bits of the padded ones at p = 0
+__device__ __forceinline__ void ln_affine(float (&z)[EMB_VEC][8], const float* gamma, const float* beta, float eps,
+                                          int lane, float& mean, float& rstd) {
   float s = 0.f;
 #pragma unroll
   for (int i = 0; i < EMB_VEC; ++i)
 #pragma unroll
     for (int j = 0; j < 8; ++j) s += z[i][j];
-  const float mean = warp_sum(s) * (1.0f / EMB_H);
+  mean = warp_sum(s) * (1.0f / EMB_H);
   float q = 0.f;
 #pragma unroll
   for (int i = 0; i < EMB_VEC; ++i)
@@ -79,7 +79,24 @@ __device__ __forceinline__ void ln_row_fwd(float (&z)[EMB_VEC][8], const float* 
       const float d = z[i][j] - mean;
       q += d * d;
     }
-  const float rstd = 1.0f / sqrtf(warp_sum(q) * (1.0f / EMB_H) + eps);
+  rstd = 1.0f / sqrtf(warp_sum(q) * (1.0f / EMB_H) + eps);
+#pragma unroll
+  for (int i = 0; i < EMB_VEC; ++i) {
+    const int c = (i * 32 + lane) * 8;
+    float g[8], b[8];
+    ld8f(gamma + c, g);
+    ld8f(beta + c, b);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) z[i][j] = g[j] * ((z[i][j] - mean) * rstd) + b[j];
+  }
+}
+
+// z (registers) -> LayerNorm -> dropout -> y ; the text forward kernel
+__device__ __forceinline__ void ln_row_fwd(float (&z)[EMB_VEC][8], const float* gamma, const float* beta, bf16* yrow,
+                                           float* mean_out, float* rstd_out, long long row, float eps,
+                                           const EmbDrop& drop, int lane) {
+  float mean, rstd;
+  ln_affine(z, gamma, beta, eps, lane, mean, rstd);
   if (lane == 0) {
     mean_out[row] = mean;
     rstd_out[row] = rstd;
@@ -87,18 +104,13 @@ __device__ __forceinline__ void ln_row_fwd(float (&z)[EMB_VEC][8], const float* 
 #pragma unroll
   for (int i = 0; i < EMB_VEC; ++i) {
     const int c = (i * 32 + lane) * 8;
-    float g[8], b[8], o[8];
-    ld8f(gamma + c, g);
-    ld8f(beta + c, b);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) o[j] = g[j] * ((z[i][j] - mean) * rstd) + b[j];
     if (drop.on) {
       bool k[8];
       emb_keep8(drop, (uint64_t)row * EMB_H + c, k);
 #pragma unroll
-      for (int j = 0; j < 8; ++j) o[j] = k[j] ? o[j] * drop.scale : 0.f;
+      for (int j = 0; j < 8; ++j) z[i][j] = k[j] ? z[i][j] * drop.scale : 0.f;
     }
-    st8h(yrow + c, o);
+    st8h(yrow + c, z[i]);
   }
 }
 
@@ -191,6 +203,30 @@ __device__ __forceinline__ long long period_stride(long long launched_warps, int
 // ------------------------------------------------------------------------------------------------------------
 // text embeddings
 // ------------------------------------------------------------------------------------------------------------
+// z = word[ids[tok]] + pos[s] (+ type[type_ids[tok]]) of token `tok` at position s; id / t: the table rows it read
+__device__ __forceinline__ void text_row_z(const long long* ids, const long long* type_ids, const float* word,
+                                           const float* pos, const float* type, int vocab, long long tok, int s,
+                                           int lane, float (&z)[EMB_VEC][8], long long& id, long long& t) {
+  id = ids[tok];
+  id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
+  t = (type != nullptr && type_ids != nullptr) ? (type_ids[tok] != 0 ? 1 : 0) : 0;
+#pragma unroll
+  for (int i = 0; i < EMB_VEC; ++i) {
+    const int c = (i * 32 + lane) * 8;
+    float a[8], b[8];
+    ld8f(word + id * EMB_H + c, a);
+    ld8f(pos + (long long)s * EMB_H + c, b);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) z[i][j] = a[j] + b[j];
+    if (type != nullptr) {
+      float tt[8];
+      ld8f(type + t * EMB_H + c, tt);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) z[i][j] += tt[j];
+    }
+  }
+}
+
 __global__ void __launch_bounds__(EMB_WARPS * 32)
 embed_text_fwd_kernel(const long long* __restrict__ ids, const long long* __restrict__ type_ids,
                       const float* __restrict__ word, const float* __restrict__ pos, const float* __restrict__ type,
@@ -201,27 +237,30 @@ embed_text_fwd_kernel(const long long* __restrict__ ids, const long long* __rest
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long long rows = (long long)n_seq * S;
   for (long long row = (long long)blockIdx.x * EMB_WARPS + warp; row < rows; row += (long long)gridDim.x * EMB_WARPS) {
-    const int s = (int)(row % S);
-    long long id = ids[row];
-    id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
-    const long long t = (type != nullptr && type_ids != nullptr) ? (type_ids[row] != 0 ? 1 : 0) : 0;
     float z[EMB_VEC][8];
-#pragma unroll
-    for (int i = 0; i < EMB_VEC; ++i) {
-      const int c = (i * 32 + lane) * 8;
-      float a[8], b[8];
-      ld8f(word + id * EMB_H + c, a);
-      ld8f(pos + (long long)s * EMB_H + c, b);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) z[i][j] = a[j] + b[j];
-      if (type != nullptr) {
-        float tt[8];
-        ld8f(type + t * EMB_H + c, tt);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) z[i][j] += tt[j];
-      }
-    }
+    long long id, t;
+    text_row_z(ids, type_ids, word, pos, type, vocab, row, (int)(row % S), lane, z, id, t);
     ln_row_fwd(z, gamma, beta, y + row * EMB_H, mean_out, rstd_out, row, eps, drop, lane);
+  }
+}
+
+// Evaluation on packed rows: row r is token idx[r] (= i * S + s) of the [n_seq, S] id matrix, LayerNorm without
+// dropout or statistics
+__global__ void __launch_bounds__(EMB_WARPS * 32)
+embed_text_packed_fwd_kernel(const long long* __restrict__ ids, const long long* __restrict__ type_ids,
+                             const int* __restrict__ idx, int rows, int S, const float* __restrict__ word,
+                             const float* __restrict__ pos, const float* __restrict__ type,
+                             const float* __restrict__ gamma, const float* __restrict__ beta, bf16* __restrict__ y,
+                             int vocab, float eps) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (long long row = (long long)blockIdx.x * EMB_WARPS + warp; row < rows; row += (long long)gridDim.x * EMB_WARPS) {
+    const long long tok = idx[row];
+    float z[EMB_VEC][8], mean, rstd;
+    long long id, t;
+    text_row_z(ids, type_ids, word, pos, type, vocab, tok, (int)(tok % S), lane, z, id, t);
+    ln_affine(z, gamma, beta, eps, lane, mean, rstd);
+#pragma unroll
+    for (int i = 0; i < EMB_VEC; ++i) st8h(y + row * EMB_H + (i * 32 + lane) * 8, z[i]);
   }
 }
 
@@ -246,25 +285,9 @@ embed_text_bwd_kernel(const bf16* __restrict__ dy, const long long* __restrict__
   if (row >= stride) row = rows;
   for (; row < rows; row += stride) {
     const int s = (int)(row % S);
-    long long id = ids[row];
-    id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
-    const long long t = (type != nullptr && type_ids != nullptr) ? (type_ids[row] != 0 ? 1 : 0) : 0;
     float z[EMB_VEC][8], dz[EMB_VEC][8];
-#pragma unroll
-    for (int i = 0; i < EMB_VEC; ++i) {
-      const int c = (i * 32 + lane) * 8;
-      float a[8], b[8];
-      ld8f(word + id * EMB_H + c, a);
-      ld8f(pos + (long long)s * EMB_H + c, b);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) z[i][j] = a[j] + b[j];
-      if (type != nullptr) {
-        float tt[8];
-        ld8f(type + t * EMB_H + c, tt);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) z[i][j] += tt[j];
-      }
-    }
+    long long id, t;
+    text_row_z(ids, type_ids, word, pos, type, vocab, row, s, lane, z, id, t);
     ln_row_bwd(z, dy + row * EMB_H, gamma, mean_in[row], rstd_in[row], row, drop, lane, dz, acc_g, acc_b);
 #pragma unroll
     for (int i = 0; i < EMB_VEC; ++i) st8f(zrows + row * EMB_H + (i * 32 + lane) * 8, dz[i]);
@@ -286,6 +309,9 @@ struct SrcCfg {
   const bf16* b;  // [Nb, Fb, H] or null (Fb = 0)
   int Na, Wa, Nb, Fb;
   int groups;  // pairing groups (common.cuh pair_sources): 0 = aligned, G = G groups of (Na/G) x (Nb/G) pairs
+  // packed evaluation rows (forward only; Wa = 1, Fb = 0): row r of a and y is token idx[r] = j * idx_len + s
+  const int* idx;
+  int idx_len;
 };
 
 // Shared by both source kernels: one warp owns one SOURCE row (text row of a, or video row of b; blockIdx.y selects).
@@ -298,6 +324,7 @@ struct SrcRow {
   int fan;          // number of output sequences reading this row
 };
 __device__ __forceinline__ SrcRow src_row_info(const SrcCfg& c, int which, long long sr) {
+  if (c.idx != nullptr) return SrcRow{sr, c.idx[sr] % c.idx_len, 1};
   const int len = which == 0 ? c.Wa : c.Fb;
   SrcRow r;
   r.owner = sr / len;
@@ -306,6 +333,7 @@ __device__ __forceinline__ SrcRow src_row_info(const SrcCfg& c, int which, long 
   return r;
 }
 __device__ __forceinline__ long long src_out_row(const SrcCfg& c, int which, const SrcRow& r, int f) {
+  if (c.idx != nullptr) return r.owner;
   const int G = c.groups ? c.groups : 1;
   const long long p = pair_sequence(which, r.owner, f, c.groups, c.Na / G, c.Nb / G);
   return p * (c.Wa + c.Fb) + r.s;
@@ -341,35 +369,12 @@ embed_src_fwd_kernel(SrcCfg src, const float* __restrict__ pos, const float* __r
   for (long long sr = (long long)blockIdx.x * EMB_WARPS + warp; sr < n_src_rows;
        sr += (long long)gridDim.x * EMB_WARPS) {
     const SrcRow r = src_row_info(src, which, sr);
-    float z[EMB_VEC][8];
+    float z[EMB_VEC][8], mean, rstd;
     src_load_z(src, which, sr, r, pos, type, lane, z);
-    float sum = 0.f;
-#pragma unroll
-    for (int i = 0; i < EMB_VEC; ++i)
-#pragma unroll
-      for (int j = 0; j < 8; ++j) sum += z[i][j];
-    const float mean = warp_sum(sum) * (1.0f / EMB_H);
-    float q = 0.f;
-#pragma unroll
-    for (int i = 0; i < EMB_VEC; ++i)
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float d = z[i][j] - mean;
-        q += d * d;
-      }
-    const float rstd = 1.0f / sqrtf(warp_sum(q) * (1.0f / EMB_H) + eps);
-#pragma unroll
-    for (int i = 0; i < EMB_VEC; ++i) {
-      const int col = (i * 32 + lane) * 8;
-      float g[8], b[8];
-      ld8f(gamma + col, g);
-      ld8f(beta + col, b);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) z[i][j] = g[j] * ((z[i][j] - mean) * rstd) + b[j];
-    }
+    ln_affine(z, gamma, beta, eps, lane, mean, rstd);
     for (int f = 0; f < r.fan; ++f) {
       const long long row = src_out_row(src, which, r, f);
-      if (lane == 0) {
+      if (lane == 0 && mean_out != nullptr) {
         mean_out[row] = mean;
         rstd_out[row] = rstd;
       }
@@ -597,7 +602,7 @@ extern "C" int univl_embed_src_fwd(const void* a, const void* b, const float* po
   UNIVL_CHECK_ARG(all_pairs || Fb == 0 || Na == Nb, "embed_src_fwd: aligned mode needs Na == Nb");
   UNIVL_CHECK_ARG(all_pairs >= 0 && (all_pairs <= 1 || Fb == 0 || (Na % all_pairs == 0 && Nb % all_pairs == 0)),
                   "embed_src_fwd: %d pairing groups must divide Na=%d and Nb=%d", all_pairs, Na, Nb);
-  SrcCfg src{(const bf16*)a, (const bf16*)b, Na, Wa, Fb == 0 ? 1 : Nb, Fb, Fb > 0 ? all_pairs : 0};
+  SrcCfg src{(const bf16*)a, (const bf16*)b, Na, Wa, Fb == 0 ? 1 : Nb, Fb, Fb > 0 ? all_pairs : 0, nullptr, 0};
   const long long n_seq = src.groups ? (long long)Na * Nb / src.groups : Na;
   if (n_seq == 0) return UNIVL_OK;
   const long long rows_a = (long long)Na * Wa, rows_b = (long long)(Fb == 0 ? 0 : Nb) * Fb;
@@ -618,7 +623,7 @@ extern "C" int univl_embed_src_bwd(const void* dy, const void* a, const void* b,
   UNIVL_CHECK_ARG(Fb == 0 || b != nullptr, "embed_src_bwd: missing second source");
   UNIVL_CHECK_ARG(all_pairs >= 0 && (all_pairs <= 1 || Fb == 0 || (Na % all_pairs == 0 && Nb % all_pairs == 0)),
                   "embed_src_bwd: %d pairing groups must divide Na=%d and Nb=%d", all_pairs, Na, Nb);
-  SrcCfg src{(const bf16*)a, (const bf16*)b, Na, Wa, Fb == 0 ? 1 : Nb, Fb, Fb > 0 ? all_pairs : 0};
+  SrcCfg src{(const bf16*)a, (const bf16*)b, Na, Wa, Fb == 0 ? 1 : Nb, Fb, Fb > 0 ? all_pairs : 0, nullptr, 0};
   if (Na == 0) return UNIVL_OK;
   const long long rows_a = (long long)Na * Wa, rows_b = (long long)(Fb == 0 ? 0 : Nb) * Fb;
   dim3 grid(emb_bwd_grid(rows_a > rows_b ? rows_a : rows_b), Fb == 0 ? 1 : 2);
@@ -636,4 +641,33 @@ extern "C" int univl_embed_src_bwd(const void* dy, const void* a, const void* b,
       pg, pb, make_emb_drop(p_drop, rng_state, stream_id));
   UNIVL_CHECK_LAUNCH("embed_src_bwd");
   return emb_table_grads(zrows, keys, rows, {nullptr, dpos, dtype}, pg, pb, parts, dgamma, dbeta, st);
+}
+
+extern "C" int univl_embed_text_packed_fwd(const long long* ids, const long long* type_ids, const int* idx, int rows,
+                                           int S, const float* word, const float* pos, const float* type,
+                                           const float* gamma, const float* beta, void* y, int H, int vocab,
+                                           float eps, void* stream) {
+  UNIVL_CHECK_ARG(H == EMB_H, "embed_text_packed_fwd: hidden size must be %d (got %d)", EMB_H, H);
+  UNIVL_CHECK_ARG(ids && idx && word && pos && gamma && beta && y, "embed_text_packed_fwd: null pointer");
+  UNIVL_CHECK_ARG(rows >= 0 && S > 0 && vocab > 0, "embed_text_packed_fwd: bad shape");
+  if (rows == 0) return UNIVL_OK;
+  embed_text_packed_fwd_kernel<<<emb_grid(rows), EMB_WARPS * 32, 0, (cudaStream_t)stream>>>(
+      ids, type_ids, idx, rows, S, word, pos, type, gamma, beta, (bf16*)y, vocab, eps);
+  UNIVL_CHECK_LAUNCH("embed_text_packed_fwd");
+  return UNIVL_OK;
+}
+
+extern "C" int univl_embed_src_packed_fwd(const void* x, const int* idx, int rows, int S, const float* pos,
+                                          const float* gamma, const float* beta, void* y, int H, float eps,
+                                          void* stream) {
+  UNIVL_CHECK_ARG(H == EMB_H, "embed_src_packed_fwd: hidden size must be %d (got %d)", EMB_H, H);
+  UNIVL_CHECK_ARG(x && idx && pos && gamma && beta && y, "embed_src_packed_fwd: null pointer");
+  UNIVL_CHECK_ARG(rows >= 0 && S > 0, "embed_src_packed_fwd: bad shape");
+  if (rows == 0) return UNIVL_OK;
+  // embed_src_fwd_kernel itself, one source row per packed row, so a row gets the padded launch's bits
+  const SrcCfg src{(const bf16*)x, nullptr, rows, 1, 1, 0, 0, idx, S};
+  embed_src_fwd_kernel<<<dim3(emb_grid(rows), 1), EMB_WARPS * 32, 0, (cudaStream_t)stream>>>(
+      src, pos, nullptr, gamma, beta, (bf16*)y, nullptr, nullptr, eps, make_emb_drop(0.f, nullptr, 0));
+  UNIVL_CHECK_LAUNCH("embed_src_packed_fwd");
+  return UNIVL_OK;
 }

@@ -90,11 +90,13 @@ __device__ __forceinline__ uint32_t keep8_mask(const DropCfg& d, uint64_t idx0) 
 // The row loop is software-pipelined: the raw vectors of the warp's NEXT row are requested before the current row's
 // reductions, so every warp always has a full row of loads in flight (the un-pipelined loop spent 67% of its issue
 // slots stalled on the long scoreboard: r01 ncu capture, 2.85 TB/s).
-template <typename TIn, int NVEC>
+// GATHER: row r of y reads row x_rows[r] of x (packed evaluation rows; no residual), otherwise row r.
+template <typename TIn, int NVEC, bool GATHER = false>
 __global__ void __launch_bounds__(LN_WARPS * 32, NVEC <= 3 ? 3 : 2)
 layernorm_fwd_kernel(const TIn* __restrict__ x, const bf16* __restrict__ res, const float* __restrict__ gamma,
                      const float* __restrict__ beta, bf16* __restrict__ y, float* __restrict__ mean_out,
-                     float* __restrict__ rstd_out, int rows, float eps, DropCfg drop_in) {
+                     float* __restrict__ rstd_out, int rows, float eps, DropCfg drop_in,
+                     const int* __restrict__ x_rows) {
   pdl_trigger();
   pdl_wait();
   const DropCfg drop = resolve_drop(drop_in);
@@ -109,7 +111,7 @@ layernorm_fwd_kernel(const TIn* __restrict__ x, const bf16* __restrict__ res, co
 #pragma unroll
     for (int i = 0; i < NVEC; ++i) {
       const long long off = row * cols + (i * 32 + lane) * 8;
-      raw_load(x + off, nx[i]);
+      raw_load(x + (GATHER ? (long long)x_rows[row] * cols + (i * 32 + lane) * 8 : off), nx[i]);
       if (res != nullptr) raw_load(res + off, nr[i]);
     }
   }
@@ -139,7 +141,7 @@ layernorm_fwd_kernel(const TIn* __restrict__ x, const bf16* __restrict__ res, co
 #pragma unroll
       for (int i = 0; i < NVEC; ++i) {
         const long long off = next * cols + (i * 32 + lane) * 8;
-        raw_load(x + off, nx[i]);
+        raw_load(x + (GATHER ? (long long)x_rows[next] * cols + (i * 32 + lane) * 8 : off), nx[i]);
         if (res != nullptr) raw_load(res + off, nr[i]);
       }
     }
@@ -182,10 +184,10 @@ static void launch_ln_fwd(int grid, cudaStream_t st, const TIn* x, const bf16* r
                           DropCfg drop) {
   const dim3 g(grid), b(LN_WARPS * 32);
   switch (cols >> 8) {
-    case 1: launch_kernel(layernorm_fwd_kernel<TIn, 1>, g, b, 0, st, x, res, gamma, beta, y, mean, rstd, rows, eps, drop); break;
-    case 2: launch_kernel(layernorm_fwd_kernel<TIn, 2>, g, b, 0, st, x, res, gamma, beta, y, mean, rstd, rows, eps, drop); break;
-    case 3: launch_kernel(layernorm_fwd_kernel<TIn, 3>, g, b, 0, st, x, res, gamma, beta, y, mean, rstd, rows, eps, drop); break;
-    default: launch_kernel(layernorm_fwd_kernel<TIn, 4>, g, b, 0, st, x, res, gamma, beta, y, mean, rstd, rows, eps, drop); break;
+    case 1: launch_kernel(layernorm_fwd_kernel<TIn, 1>, g, b, 0, st, x, res, gamma, beta, y, mean, rstd, rows, eps, drop, (const int*)nullptr); break;
+    case 2: launch_kernel(layernorm_fwd_kernel<TIn, 2>, g, b, 0, st, x, res, gamma, beta, y, mean, rstd, rows, eps, drop, (const int*)nullptr); break;
+    case 3: launch_kernel(layernorm_fwd_kernel<TIn, 3>, g, b, 0, st, x, res, gamma, beta, y, mean, rstd, rows, eps, drop, (const int*)nullptr); break;
+    default: launch_kernel(layernorm_fwd_kernel<TIn, 4>, g, b, 0, st, x, res, gamma, beta, y, mean, rstd, rows, eps, drop, (const int*)nullptr); break;
   }
 }
 
@@ -413,6 +415,28 @@ extern "C" int univl_layernorm_f32_fwd(const float* x, const float* gamma, const
   launch_ln_fwd<float>(ln_grid(rows), (cudaStream_t)stream, x, (const bf16*)nullptr, gamma, beta, (bf16*)y, mean, rstd,
                        rows, cols, eps, make_drop(0, 0.f, nullptr, 0));
   UNIVL_CHECK_LAUNCH("layernorm_f32_fwd");
+  return UNIVL_OK;
+}
+
+// NormalizeVideo on gathered rows (packed evaluation): y[r] = LN(x[x_rows[r]]), no statistics.  The same kernel body
+// as univl_layernorm_f32_fwd, so a row's bits do not depend on which of the two ran it.
+extern "C" int univl_layernorm_f32_rows_fwd(const float* x, const int* x_rows, const float* gamma, const float* beta,
+                                            void* y, int rows, int cols, float eps, void* stream) {
+  if (int rc = check_ln_shape("layernorm_f32_rows_fwd", rows, cols)) return rc;
+  UNIVL_CHECK_ARG(x && x_rows && gamma && beta && y, "layernorm_f32_rows_fwd: null pointer");
+  if (rows == 0) return UNIVL_OK;
+  const dim3 g(ln_grid(rows)), b(LN_WARPS * 32);
+  const cudaStream_t st = (cudaStream_t)stream;
+  const DropCfg d = make_drop(0, 0.f, nullptr, 0);
+  float* none = nullptr;
+  const bf16* no_res = nullptr;
+  switch (cols >> 8) {
+    case 1: launch_kernel(layernorm_fwd_kernel<float, 1, true>, g, b, 0, st, x, no_res, gamma, beta, (bf16*)y, none, none, rows, eps, d, x_rows); break;
+    case 2: launch_kernel(layernorm_fwd_kernel<float, 2, true>, g, b, 0, st, x, no_res, gamma, beta, (bf16*)y, none, none, rows, eps, d, x_rows); break;
+    case 3: launch_kernel(layernorm_fwd_kernel<float, 3, true>, g, b, 0, st, x, no_res, gamma, beta, (bf16*)y, none, none, rows, eps, d, x_rows); break;
+    default: launch_kernel(layernorm_fwd_kernel<float, 4, true>, g, b, 0, st, x, no_res, gamma, beta, (bf16*)y, none, none, rows, eps, d, x_rows); break;
+  }
+  UNIVL_CHECK_LAUNCH("layernorm_f32_rows_fwd");
   return UNIVL_OK;
 }
 

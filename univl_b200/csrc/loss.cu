@@ -35,23 +35,41 @@ __device__ __forceinline__ float block_max(float v, float* red) {
 // ------------------------------------------------------------------------------------------------------------
 // masked mean pooling
 // ------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-meanpool_fwd_kernel(const bf16* __restrict__ x, const long long* __restrict__ mask, float* __restrict__ out,
-                    float* __restrict__ norm_out, int S, int H, int skip_first, int guard_zero, int l2norm) {
-  __shared__ float red[32];
-  const int n = blockIdx.x;
+// The rows sequence n pools, in the order they are added: row k < count() is x row row(k), pooled when on(k).
+// Padded: the S rows of the [N, S] layout, on where the mask is set.  Packed: the sequence's valid rows alone
+// (cu[n] .. cu[n + 1] - 1, ascending source position), so it adds the same values in the same order as the padded
+// layout, which skips its masked rows.
+struct PaddedPoolRows {
+  const long long* mask;
+  int S, skip_first;
+  long long n;
+  __device__ int count() const { return S; }
+  __device__ bool on(int k) const { return mask[n * S + k] != 0 && !(skip_first && k == 0); }
+  __device__ long long row(int k) const { return n * S + k; }
+};
+struct PackedPoolRows {
+  const int* idx;  // source token of every packed row (i * S + s)
+  int S, skip_first, first, last;
+  __device__ int count() const { return last - first; }
+  __device__ bool on(int k) const { return !(skip_first && idx[first + k] % S == 0); }
+  __device__ long long row(int k) const { return (long long)first + k; }
+};
+
+template <class Rows>
+__device__ __forceinline__ void meanpool_row(const bf16* __restrict__ x, const Rows& rows, float* __restrict__ out,
+                                             float* __restrict__ norm_out, long long n, int H, int guard_zero,
+                                             int l2norm, float* red) {
+  const int count = rows.count();
   float den = 0.f;
-  for (int s = 0; s < S; ++s) den += (mask[(long long)n * S + s] != 0 && !(skip_first && s == 0)) ? 1.f : 0.f;
+  for (int k = 0; k < count; ++k) den += rows.on(k) ? 1.f : 0.f;
   if (guard_zero && den == 0.f) den = 1.f;
   float sq = 0.f;
   float u[4];
   int nc = 0;
   for (int c = threadIdx.x; c < H; c += blockDim.x, ++nc) {
     float acc = 0.f;
-    for (int s = 0; s < S; ++s) {
-      const bool on = mask[(long long)n * S + s] != 0 && !(skip_first && s == 0);
-      if (on) acc += __bfloat162float(x[((long long)n * S + s) * H + c]);
-    }
+    for (int k = 0; k < count; ++k)
+      if (rows.on(k)) acc += __bfloat162float(x[rows.row(k) * H + c]);
     acc = acc / den;
     u[nc] = acc;
     sq += acc * acc;
@@ -62,7 +80,23 @@ meanpool_fwd_kernel(const bf16* __restrict__ x, const long long* __restrict__ ma
   }
   if (threadIdx.x == 0 && norm_out) norm_out[n] = nrm;
   nc = 0;
-  for (int c = threadIdx.x; c < H; c += blockDim.x, ++nc) out[(long long)n * H + c] = u[nc] / nrm;
+  for (int c = threadIdx.x; c < H; c += blockDim.x, ++nc) out[n * H + c] = u[nc] / nrm;
+}
+
+__global__ void __launch_bounds__(256)
+meanpool_fwd_kernel(const bf16* __restrict__ x, const long long* __restrict__ mask, float* __restrict__ out,
+                    float* __restrict__ norm_out, int S, int H, int skip_first, int guard_zero, int l2norm) {
+  __shared__ float red[32];
+  const PaddedPoolRows rows{mask, S, skip_first, (long long)blockIdx.x};
+  meanpool_row(x, rows, out, norm_out, blockIdx.x, H, guard_zero, l2norm, red);
+}
+
+__global__ void __launch_bounds__(256)
+meanpool_packed_fwd_kernel(const bf16* __restrict__ x, const int* __restrict__ cu, const int* __restrict__ idx,
+                           float* __restrict__ out, int S, int H, int skip_first, int guard_zero, int l2norm) {
+  __shared__ float red[32];
+  const PackedPoolRows rows{idx, S, skip_first, cu[blockIdx.x], cu[blockIdx.x + 1]};
+  meanpool_row(x, rows, out, (float*)nullptr, blockIdx.x, H, guard_zero, l2norm, red);
 }
 
 __global__ void __launch_bounds__(256)
@@ -436,6 +470,16 @@ extern "C" int univl_meanpool_fwd(const void* x, const long long* mask, float* o
   meanpool_fwd_kernel<<<N, 256, 0, (cudaStream_t)stream>>>((const bf16*)x, mask, out, norm_out, S, H, skip_first,
                                                            guard_zero, l2norm);
   UNIVL_CHECK_LAUNCH("meanpool_fwd");
+  return UNIVL_OK;
+}
+extern "C" int univl_meanpool_packed_fwd(const void* x, const int* cu, const int* idx, float* out, int N, int S, int H,
+                                         int skip_first, int guard_zero, int l2norm, void* stream) {
+  // x and idx are read only for the rows the sequences hold: both may be null when there are none
+  UNIVL_CHECK_ARG(cu && out && N >= 0 && S > 0 && H > 0 && H <= 1024, "meanpool_packed_fwd: bad arguments");
+  if (N == 0) return UNIVL_OK;
+  meanpool_packed_fwd_kernel<<<N, 256, 0, (cudaStream_t)stream>>>((const bf16*)x, cu, idx, out, S, H, skip_first,
+                                                                  guard_zero, l2norm);
+  UNIVL_CHECK_LAUNCH("meanpool_packed_fwd");
   return UNIVL_OK;
 }
 extern "C" int univl_meanpool_bwd(const float* dy, const float* y, const float* norm, const long long* mask, void* dx,

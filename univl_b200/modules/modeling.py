@@ -31,6 +31,13 @@ logger = logging.getLogger(__name__)
 # path draws no stream-ordered kernel scratch.
 EVAL_PAIR_TOKENS = 1 << 18
 
+# Valid tokens per chunk of the gallery encoders (univl_b200.retrieval.embed_texts / embed_videos).  A chunk's memory
+# grows linearly with it: the packed rows of one encoder layer, the fp32 copy of its valid frames when the video is
+# not contiguous fp32, and index arrays over at most retrieval.RowPacking.ROW_SPAN times as many padded tokens.  A
+# row's vector does not depend on it.  At this value the peak of torch allocations was 2.73 GiB, for the text and the
+# visual encoder alike (measured on an H100 80GB HBM3 at a 700 W power limit, scripts/bench_gallery_index.py).
+EMBED_TOKENS = 1 << 17
+
 EVAL_PRECISIONS = ("bf16", "fp8")
 
 

@@ -505,6 +505,43 @@ class PairPacking:
                           self.start_v[vi], len_a)
 
 
+def embed_text_packed(ids, type_ids, idx, S, word, pos, type_w, gamma, beta):
+    """EmbedTextFn in evaluation on packed rows: row r is token idx[r] (int32, = i * S + s) of the [n, S] ids /
+    type_ids (type_ids None: type 0) -> bf16 [idx.numel(), H]"""
+    y = _empty((idx.numel(), word.shape[1]), BF16, word)
+    call("univl_embed_text_packed_fwd", ids.data_ptr(), ptr(type_ids), idx.data_ptr(), idx.numel(), S,
+         word.data_ptr(), pos.data_ptr(), ptr(type_w), gamma.data_ptr(), beta.data_ptr(), y.data_ptr(),
+         word.shape[1], word.shape[0], LN_EPS)
+    return y
+
+
+def video_norm_rows(video2d, idx, gamma, beta):
+    """VideoNormFn's forward on the fp32 rows idx (int32) of video2d [rows, video_dim] -> bf16 [idx.numel(), video_dim]"""
+    y = _empty((idx.numel(), video2d.shape[1]), BF16, video2d)
+    call("univl_layernorm_f32_rows_fwd", video2d.data_ptr(), idx.data_ptr(), gamma.data_ptr(), beta.data_ptr(),
+         y.data_ptr(), idx.numel(), video2d.shape[1], LN_EPS)
+    return y
+
+
+def embed_src_packed(x, idx, S, pos, gamma, beta):
+    """EmbedSrcFn in evaluation (one aligned source, the visual embeddings) on packed rows: x [T, H] holds token idx[r]
+    (= j * S + s) -> bf16 LN(x[r] + pos[s]) [T, H]"""
+    y = _empty(x.shape, BF16, x)
+    call("univl_embed_src_packed_fwd", x.data_ptr(), idx.data_ptr(), x.shape[0], S, pos.data_ptr(), gamma.data_ptr(),
+         beta.data_ptr(), y.data_ptr(), x.shape[1], LN_EPS)
+    return y
+
+
+def meanpool_packed(x, cu, idx, S, skip_first, guard_zero, l2norm):
+    """MeanPoolFn's forward on packed rows: sequence n is rows [cu[n], cu[n + 1]) of x (int32 cu), row r at position
+    idx[r] mod S -> fp32 [cu.numel() - 1, H], equal bit for bit to MeanPoolFn on the padded layout's rows"""
+    N, H = cu.numel() - 1, x.shape[1]
+    out = _empty((N, H), F32, cu)
+    call("univl_meanpool_packed_fwd", x.data_ptr(), cu.data_ptr(), idx.data_ptr(), out.data_ptr(), N, S, H,
+         int(skip_first), int(guard_zero), int(l2norm))
+    return out
+
+
 def padded_pair_seqs(text_index, video_index, Nt, W, Nv, F):
     """VarlenSeqs (pair addressing) of the listed pairs at all W + F tokens, over the rows of the per-source sources
     [Nt*W, *] (text) and [Nv*F, *] (video): pair p's rows are text rows text_index[p] * W + [0, W) then video rows

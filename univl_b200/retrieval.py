@@ -10,6 +10,13 @@ similarity, re-rank the shortlisted pairs with a cross encoder.
 
 Inputs are what get_sequence_visual_output returns: sequence_output [Nt, W, H], visual_output [Nv, F, H] and the int64
 masks attention_mask [Nt, W], video_mask [Nv, F].
+
+A gallery can also be indexed as one pooled vector per row, encoded once and searched later:
+
+  embed_texts / embed_videos  the text and video vectors _mean_pool_similarity multiplies, fp32 [N, H], from the
+                              text (or visual) encoder alone, run on each row's valid tokens only
+  topk                        the exact top k of stored query vectors against stored gallery vectors, in either
+                              direction (text-to-video or video-to-text)
 """
 import numpy as np
 import torch
@@ -18,6 +25,7 @@ from . import ops
 from . import runtime as rt
 from .modules import modeling
 from .modules.modeling import _flat, eval_layout, eval_precision
+from .modules.transformer import _layer_params
 
 
 def _inputs(model, sequence_output, visual_output, attention_mask, video_mask):
@@ -134,3 +142,173 @@ def search(shortlist_model, rerank_model, sequence_output, visual_output, attent
         scores = score_pairs(rerank_model, seq, vis, attention_mask, video_mask, ti, short.reshape(-1))
     scores, order = torch.sort(scores.view(Nt, k_shortlist), dim=1, descending=True, stable=True)
     return scores[:, :k].contiguous(), short.gather(1, order[:, :k])
+
+
+def _check_eval(model, what):
+    if model.training or torch.is_grad_enabled():
+        raise RuntimeError("%s: call model.eval() and run under torch.no_grad()" % what)
+
+
+def _check_cuda(what, *tensors):
+    for t in tensors:
+        if t is not None and not t.is_cuda:
+            raise RuntimeError("univl_b200: %s needs CUDA tensors (no CPU path)" % what)
+
+
+class RowPacking:
+    """The valid tokens of the N rows of a [N, S] mask (any dtype; nonzero = valid, any pattern), cut into chunks of
+    consecutive rows of at most `budget` valid tokens and at most ROW_SPAN * budget padded tokens each (at least one
+    row per chunk).  The second bound caps the rows of a chunk, which the valid-token budget alone does not: rows
+    without a valid token cost no budget, and chunk() builds per-padded-token index arrays (int32) over its rows.  At
+    a packed fraction of 1 / ROW_SPAN or more, only the valid-token budget cuts.  One device-to-host copy: the per-row
+    counts.
+      counts   host int64 array [N]
+      chunks   list of row ranges (a, b)
+      max_len  the longest row of the whole call: every chunk passes it to the attention, so which attention kernel a
+               row runs on does not depend on the chunking"""
+
+    ROW_SPAN = 8
+
+    def __init__(self, mask, budget):
+        self.valid = mask.reshape(-1, mask.shape[-1]) != 0
+        self.S = self.valid.shape[1]
+        self.counts = self.valid.sum(1).cpu().numpy().astype(np.int64)
+        cap = max(1, self.ROW_SPAN * budget // max(1, self.S))
+        self.chunks = [(x, min(b, x + cap)) for a, b in _pair_chunks(self.counts, budget) for x in range(a, b, cap)]
+        self.max_len = int(self.counts.max(initial=0))
+
+    def chunk(self, a, b):
+        """rows [a, b) -> (idx, cu, seqs): idx int32 the valid tokens (i - a) * S + s in row then position order, cu
+        int32 [b - a + 1] the packed row offsets, seqs their ops.VarlenSeqs (packed addressing)"""
+        valid = self.valid[a:b]
+        idx = ops._valid_rows(valid, int(self.counts[a:b].sum()))
+        cu = ops._exclusive_cumsum(valid.sum(1)).to(ops.I32)
+        return idx, cu, ops.VarlenSeqs(cu, idx.numel(), self.max_len)
+
+
+def _no_rows(like):
+    return torch.empty((0, like.shape[1]), dtype=torch.bfloat16, device=like.device)
+
+
+def _encode_packed(layers, x, seqs):
+    for layer in layers:
+        x = ops.encoder_layer_eval_packed(x, seqs, _layer_params(layer))
+    return x
+
+
+def embed_texts(model, input_ids, attention_mask, token_type_ids=None):
+    """-> fp32 [Nt, H]: the text vectors of UniVL._mean_pool_similarity (reference modeling.py:327-339, :386-388):
+    the text encoder's output mean-pooled over the valid tokens but token 0, L2-normalised unless
+    task_config.use_mil.  The encoder runs on each row's valid tokens alone (attention_mask != 0, any pattern), each
+    at its original position; no visual encoder runs.  A row without a pooled token gives what the padded pooling
+    gives (0 / 0).  input_ids, attention_mask (and token_type_ids) are [Nt, W] (or [..., W], flattened as the model
+    does) CUDA tensors.  Evaluation only: model.eval() under torch.no_grad() (RuntimeError otherwise).  Rows are
+    encoded in chunks of at most modeling.EMBED_TOKENS valid tokens; a row's vector does not depend on the chunking."""
+    _check_eval(model, "embed_texts")
+    ids, am = _flat(input_ids), _flat(attention_mask)
+    if ids.shape != am.shape:
+        raise ValueError("embed_texts: input_ids %s and attention_mask %s differ in shape"
+                         % (tuple(ids.shape), tuple(am.shape)))
+    types = None if token_type_ids is None else _flat(token_type_ids)
+    if types is not None and types.shape != ids.shape:
+        raise ValueError("embed_texts: token_type_ids %s and input_ids %s differ in shape"
+                         % (tuple(types.shape), tuple(ids.shape)))
+    ids, types = ids.long().contiguous(), (None if types is None else types.long().contiguous())
+    emb = model.bert.embeddings
+    W = ids.shape[1]
+    if not 0 < W <= emb.position_embeddings.weight.shape[0]:
+        raise ValueError("embed_texts: %d tokens per row, the position table holds %d"
+                         % (W, emb.position_embeddings.weight.shape[0]))
+    _check_cuda("embed_texts", ids, am, types)
+    l2 = model.task_config.use_mil is False
+    with rt.use_model(model, model._device()):
+        rows = RowPacking(am, modeling.EMBED_TOKENS)
+        out = torch.empty((ids.shape[0], emb.word_embeddings.weight.shape[1]), dtype=torch.float32, device=ids.device)
+        for a, b in rows.chunks:
+            idx, cu, seqs = rows.chunk(a, b)
+            if idx.numel() == 0:  # no valid token in the chunk: the pooling alone gives its rows' vectors
+                out[a:b] = ops.meanpool_packed(_no_rows(out), cu, idx, W, True, False, l2)
+                continue
+            x = ops.embed_text_packed(ids[a:b], None if types is None else types[a:b], idx, W,
+                                      emb.word_embeddings.weight, emb.position_embeddings.weight,
+                                      emb.token_type_embeddings.weight, emb.LayerNorm.weight, emb.LayerNorm.bias)
+            x = _encode_packed(model.bert.encoder.layer, x, seqs)
+            out[a:b] = ops.meanpool_packed(x, cu, idx, W, True, False, l2)
+        return out
+
+
+def embed_videos(model, video, video_mask):
+    """-> fp32 [Nv, H]: the video vectors of UniVL._mean_pool_similarity: NormalizeVideo, the visual encoder and the
+    mean over the valid frames (video_mask != 0, any pattern; a row without one gives the zero vector), L2-normalised
+    unless task_config.use_mil, computed on the valid frames alone, each at its original position; no text encoder
+    runs.  video: fp32 or fp64 [Nv, F, video_dim] (or [..., F, video_dim]), video_mask [Nv, F], CUDA tensors.  A
+    contiguous fp32 video is read in place; of any other only the valid frames of a chunk are copied (to fp32).
+    Evaluation only, chunked, and independent of the chunking as embed_texts."""
+    _check_eval(model, "embed_videos")
+    if video.dtype not in (torch.float32, torch.float64):
+        raise ValueError("embed_videos: video must be float32 or float64, got %s" % video.dtype)
+    if video.dim() < 3:
+        raise ValueError("embed_videos: video must be [N, F, video_dim], got shape %s" % (tuple(video.shape),))
+    D = model.task_config.video_dim
+    v = video.reshape(-1, video.shape[-2], video.shape[-1])
+    vm = _flat(video_mask)
+    if v.shape[-1] != D or tuple(v.shape[:2]) != tuple(vm.shape):
+        raise ValueError("embed_videos: video %s does not match video_mask %s and video_dim %d"
+                         % (tuple(video.shape), tuple(video_mask.shape), D))
+    emb = model.visual.embeddings
+    F = vm.shape[1]
+    if not 0 < F <= emb.position_embeddings.weight.shape[0]:
+        raise ValueError("embed_videos: %d frames per row, the position table holds %d"
+                         % (F, emb.position_embeddings.weight.shape[0]))
+    _check_cuda("embed_videos", video, video_mask)
+    norm = model.normalize_video.visual_norm2d
+    l2 = model.task_config.use_mil is False
+    with rt.use_model(model, model._device()):
+        rows = RowPacking(vm, modeling.EMBED_TOKENS)
+        w16 = rt.current().bf16(emb.word_embeddings.weight)
+        out = torch.empty((v.shape[0], w16.shape[0]), dtype=torch.float32, device=v.device)
+        for a, b in rows.chunks:
+            idx, cu, seqs = rows.chunk(a, b)
+            if idx.numel() == 0:
+                out[a:b] = ops.meanpool_packed(_no_rows(out), cu, idx, F, False, True, l2)
+                continue
+            if v.dtype == torch.float32 and v[a:b].is_contiguous():  # the kernel reads the valid frames in place
+                rows2d, ridx = v[a:b].view(-1, D), idx
+            else:  # copy the valid frames alone to fp32 (an exact conversion): at most EMBED_TOKENS rows
+                li = idx.long()
+                rows2d = v[a + li // F, li % F].float()
+                ridx = torch.arange(idx.numel(), dtype=ops.I32, device=idx.device)
+            x = ops.video_norm_rows(rows2d, ridx, norm.weight, norm.bias)
+            del rows2d, ridx
+            x = ops.linear_fwd(x, w16, emb.word_embeddings.bias)
+            x = ops.embed_src_packed(x, idx, F, emb.position_embeddings.weight, emb.LayerNorm.weight,
+                                     emb.LayerNorm.bias)
+            x = _encode_packed(model.visual.encoder.layer, x, seqs)
+            out[a:b] = ops.meanpool_packed(x, cu, idx, F, False, True, l2)
+        return out
+
+
+def topk(queries, gallery, k):
+    """-> (scores fp32 [Nq, k], index int64 [Nq, k]): for each stored query vector the k gallery rows with the largest
+    dot product, score descending, ties by lower gallery index (univl_sim_topk).  Text-to-video:
+    topk(embed_texts(...), embed_videos(...), k); video-to-text: topk(embed_videos(...), embed_texts(...), k).  Every
+    score has the bits of _mean_pool_similarity(...)[i, j] (text-to-video) or [j, i] (video-to-text) of the same
+    vectors.  queries [Nq, H] and gallery [Ng, H]: fp32 CUDA tensors on one device, H a multiple of 4;
+    1 <= k <= min(256, Ng)."""
+    for t, name in ((queries, "queries"), (gallery, "gallery")):
+        if not isinstance(t, torch.Tensor) or t.dim() != 2 or t.dtype != torch.float32:
+            raise ValueError("topk: %s must be a 2-D float32 tensor" % name)
+    if queries.shape[1] != gallery.shape[1] or queries.shape[1] % 4:
+        raise ValueError("topk: queries %s and gallery %s need the same width, a multiple of 4"
+                         % (tuple(queries.shape), tuple(gallery.shape)))
+    if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= min(256, gallery.shape[0]):
+        raise ValueError("topk: need 1 <= k <= min(256, %d gallery rows), got %r" % (gallery.shape[0], k))
+    if queries.device != gallery.device:
+        raise ValueError("topk: queries on %s and gallery on %s: both must be on one device"
+                         % (queries.device, gallery.device))
+    _check_cuda("topk", queries, gallery)
+    if queries.shape[0] == 0:
+        return (torch.empty((0, k), dtype=torch.float32, device=queries.device),
+                torch.empty((0, k), dtype=torch.int64, device=queries.device))
+    scores, index = ops.sim_topk(queries, gallery, k)
+    return scores, index.long()
