@@ -349,6 +349,20 @@ int univl_beam_advance(const float* key, const int* index, int n_inst, int n_bea
  * Inputs are expected finite (a NaN score has no place in the order). */
 int univl_sim_topk(const float* t, const float* v, float* scores, int* index, int Nt, int Nv, int H, int k,
                    void* stream);
+/* Exact ground-truth ranks of retrieval, the matrix never written.  t [Nt, H] queries and v [Nv, H] gallery rows as
+ * univl_sim_topk takes them; every score has the bits of univl_sim_matmul_fwd's entry, and rows rank in
+ * univl_sim_topk's order (score descending, then gallery index ascending).
+ * univl_sim_best_positive: for each query i, the best of its positives perm[lo[i]], ..., perm[hi[i] - 1] (int32,
+ *   entries in [0, Nv)) in that order -> best_s fp32 [Nt] and best_i int32 [Nt]; (-inf, INT_MAX) when lo[i] == hi[i].
+ * univl_sim_rank: rank int64 [Nt] = the number of gallery rows j that rank above (best_s[i], best_i[i]), i.e. the
+ *   0-based position of query i's best positive (Nv for a query without one).  The counts are exact integers: every
+ *   launch writes the same bytes, for any tiling or split of the gallery.  No scratch and no host synchronisation
+ *   (capturable in a CUDA graph).  H a multiple of 4, t and v 16-byte aligned.
+ * Inputs are expected finite (a NaN score has no place in the order). */
+int univl_sim_best_positive(const float* t, const float* v, const int* perm, const int* lo, const int* hi,
+                            float* best_s, int* best_i, int Nt, int Nv, int H, void* stream);
+int univl_sim_rank(const float* t, const float* v, const float* best_s, const int* best_i, long long* rank, int Nt,
+                   int Nv, int H, void* stream);
 /* cross pooler tanh + similarity_dense (module_cross.py:281-287; modeling.py:371): out[r] = tanh(u[r,:]).w + b */
 int univl_pooler_sim_fwd(const void* u, const float* w, const float* b, float* out, int N, int H, void* stream);
 int univl_pooler_sim_bwd(const void* u, const float* w, const float* dout, void* du, float* dw, float* db, int N,

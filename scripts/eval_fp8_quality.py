@@ -72,35 +72,19 @@ def metrics(sim):
     return out
 
 
-def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--eval", type=int, default=1024, help="held-out pairs")
-    ap.add_argument("--batch", type=int, default=64)
-    ap.add_argument("--vocab", type=int, default=256)
-    ap.add_argument("--noise", type=float, default=0.5)
-    ap.add_argument("--lr", type=float, default=1e-4)
-    ap.add_argument("--max-steps", type=int, default=4000)
-    ap.add_argument("--eval-every", type=int, default=250)
-    ap.add_argument("--target-r1", type=float, default=50.0)
-    ap.add_argument("--seed", type=int, default=0)
-    a = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("eval_fp8_quality: needs a CUDA device")
+def train(a, mode, sample, held_out, evaluate):
+    """Train a reduced model of `mode` (2 text layers, 1 visual layer, 2 cross layers, no dropout) with AdamW on the
+    task until evaluate(model, held_out)["R@1"] reaches a.target_r1 (checked every a.eval_every steps) or a.max_steps.
+    Prints one JSON line per evaluation.  -> (model, steps)"""
     from oracle import synth
     from tests.model_util import build_model
 
-    torch.manual_seed(a.seed)
-    cfg = synth.task_config(mode="ft_align", batch_size=a.batch, text_layers=2, visual_layers=1, cross_layers=2,
+    cfg = synth.task_config(mode=mode, batch_size=a.batch, text_layers=2, visual_layers=1, cross_layers=2,
                             max_words=W, max_frames=F)
     model = build_model(cfg, sd=synth.make_state_dict(cfg, seed=a.seed, init_law=True), dropout=0.0)
     opt = torch.optim.AdamW(model.parameters(), lr=a.lr, weight_decay=0.01)
     warmup = 100
     sched = torch.optim.lr_scheduler.LambdaLR(opt, lambda s: min(1.0, (s + 1) / warmup))
-    sample = make_task(a.vocab, a.noise, a.seed + 1)
-    held_out = sample(a.eval, seed=10 ** 6)
-    print(json.dumps({"gpu": torch.cuda.get_device_name(0), "task": vars(a), "W": W, "F": F,
-                      "chance_R@1": round(100.0 / a.eval, 3)}), flush=True)
-
     step, t0 = 0, time.perf_counter()
     while True:
         model.train()
@@ -112,11 +96,38 @@ def main():
         sched.step()
         step += 1
         if step % a.eval_every == 0 or step == a.max_steps:
-            m = metrics(logits(model, held_out, "bf16"))
-            print(json.dumps({"step": step, "loss": round(float(loss.detach()), 4), "bf16": m,
+            m = evaluate(model, held_out)
+            print(json.dumps({"mode": mode, "step": step, "loss": round(float(loss.detach()), 4), "bf16": m,
                               "train_s": round(time.perf_counter() - t0, 1)}), flush=True)
             if m["R@1"] >= a.target_r1 or step >= a.max_steps:
-                break
+                return model, step
+
+
+def arguments(ap):
+    """the task and training options"""
+    ap.add_argument("--eval", type=int, default=1024, help="held-out pairs")
+    ap.add_argument("--batch", type=int, default=64)
+    ap.add_argument("--vocab", type=int, default=256)
+    ap.add_argument("--noise", type=float, default=0.5)
+    ap.add_argument("--lr", type=float, default=1e-4)
+    ap.add_argument("--max-steps", type=int, default=4000)
+    ap.add_argument("--eval-every", type=int, default=250)
+    ap.add_argument("--target-r1", type=float, default=50.0)
+    ap.add_argument("--seed", type=int, default=0)
+    return ap
+
+
+def main():
+    a = arguments(argparse.ArgumentParser()).parse_args()
+    if not torch.cuda.is_available():
+        sys.exit("eval_fp8_quality: needs a CUDA device")
+
+    torch.manual_seed(a.seed)
+    sample = make_task(a.vocab, a.noise, a.seed + 1)
+    held_out = sample(a.eval, seed=10 ** 6)
+    print(json.dumps({"gpu": torch.cuda.get_device_name(0), "task": vars(a), "W": W, "F": F,
+                      "chance_R@1": round(100.0 / a.eval, 3)}), flush=True)
+    model, step = train(a, "ft_align", sample, held_out, lambda m, d: metrics(logits(m, d, "bf16")))
 
     bf16 = logits(model, held_out, "bf16")
     fp8 = logits(model, held_out, "fp8")

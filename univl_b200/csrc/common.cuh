@@ -117,6 +117,14 @@ __device__ __forceinline__ float warp_sum(float v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
+// One entry of the similarity matrix, t . v over H columns, in the order every similarity kernel reproduces: lane l
+// forms the partial acc_l = fma(t[c], v[c], acc_l) over c = l, l + 32, ... in increasing c, then warp_sum adds the 32
+// partials.  Every lane of the (converged) warp returns the sum.
+__device__ __forceinline__ float sim_dot(const float* __restrict__ t, const float* __restrict__ v, int H, int lane) {
+  float acc = 0.f;
+  for (int c = lane; c < H; c += 32) acc = fmaf(t[c], v[c], acc);
+  return warp_sum(acc);
+}
 __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));

@@ -129,13 +129,14 @@ meanpool_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ y, c
 // ------------------------------------------------------------------------------------------------------------
 __global__ void sim_fwd_kernel(const float* __restrict__ t, const float* __restrict__ v, float* __restrict__ sim,
                                int Bt, int Bv, int H, int groups) {
-  const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (gw >= groups * Bt * Bv) return;
-  const int g = gw / (Bt * Bv), e = gw - g * (Bt * Bv);
-  const int i = g * Bt + e / Bv, j = g * Bv + e % Bv;
-  float acc = 0.f;
-  for (int c = lane; c < H; c += 32) acc += t[(long long)i * H + c] * v[(long long)j * H + c];
-  acc = warp_sum(acc);
+  // 64-bit: a matrix of more than 2^27 entries has more than 2^32 threads
+  const long long gw = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (gw >= (long long)groups * Bt * Bv) return;
+  const int g = (int)(gw / ((long long)Bt * Bv));
+  const long long e = gw - (long long)g * Bt * Bv;
+  const int i = g * Bt + (int)(e / Bv), j = g * Bv + (int)(e % Bv);
+  const float acc = sim_dot(t + (long long)i * H, v + (long long)j * H, H, lane);
   if (lane == 0) sim[gw] = acc;
 }
 // dt[i,:] = sum_j dsim[i,j] v[j,:] ; dv[j,:] = sum_i dsim[i,j] t[i,:]   (within group blockIdx.x / (Bt + Bv))

@@ -1376,6 +1376,32 @@ def sim_topk(t, v, k):
     return scores, index
 
 
+def sim_best_positive(t, v, perm, lo, hi):
+    """For each row i of t [Nt, H], the best of the rows perm[lo[i]:hi[i]] of v [Nv, H] (int32 index tensors on the
+    device) by score descending, then index ascending (csrc/retrieval.cu) -> (best_s fp32 [Nt], best_i int32 [Nt]);
+    each score has SimMatmulFn's bits; (-inf, INT_MAX) for an empty range."""
+    t, v = t.contiguous(), v.contiguous()
+    _check2d(t, "sim_best_positive t"); _check2d(v, "sim_best_positive v")
+    Nt, H = t.shape
+    best_s, best_i = _empty((Nt,), F32, t), _empty((Nt,), I32, t)
+    perm, lo, hi = perm.contiguous(), lo.contiguous(), hi.contiguous()
+    call("univl_sim_best_positive", t.data_ptr(), v.data_ptr(), perm.data_ptr(), lo.data_ptr(), hi.data_ptr(),
+         best_s.data_ptr(), best_i.data_ptr(), Nt, v.shape[0], H)
+    return best_s, best_i
+
+
+def sim_rank(t, v, best_s, best_i):
+    """-> int64 [Nt]: for each row i of t, the number of rows of v that rank above (best_s[i], best_i[i]) in
+    sim_topk's order, scored as sim_topk scores them (csrc/retrieval.cu).  No host synchronisation."""
+    t, v = t.contiguous(), v.contiguous()
+    _check2d(t, "sim_rank t"); _check2d(v, "sim_rank v")
+    Nt, H = t.shape
+    rank = _empty((Nt,), torch.int64, t)
+    call("univl_sim_rank", t.data_ptr(), v.data_ptr(), best_s.contiguous().data_ptr(), best_i.contiguous().data_ptr(),
+         rank.data_ptr(), Nt, v.shape[0], H)
+    return rank
+
+
 class SimLossFn(torch.autograd.Function):
     """scalar loss on a square similarity matrix [B, B], or the mean over groups of the loss of each matrix of a
     [G, B, B] stack; kind: 'maxmargin' | 'crossen' | 'milnce' (reference modules/until_module.py:182-251)."""

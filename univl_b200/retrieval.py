@@ -17,6 +17,12 @@ A gallery can also be indexed as one pooled vector per row, encoded once and sea
                               text (or visual) encoder alone, run on each row's valid tokens only
   topk                        the exact top k of stored query vectors against stored gallery vectors, in either
                               direction (text-to-video or video-to-text)
+
+and scored against ground truth at gallery scale, without the similarity matrix:
+
+  ranks                       each query's exact rank of its first positive (labels: many positives per query)
+  ranks_from_scores           the same rule on a dense score matrix the caller already has (cross encoders)
+  rank_metrics                R@1/5/10, median and mean rank of those ranks
 """
 import numpy as np
 import torch
@@ -288,6 +294,19 @@ def embed_videos(model, video, video_mask):
         return out
 
 
+def _check_vectors(what, queries, gallery):
+    """the stored-vector arguments of topk / ranks, checked on the host"""
+    for t, name in ((queries, "queries"), (gallery, "gallery")):
+        if not isinstance(t, torch.Tensor) or t.dim() != 2 or t.dtype != torch.float32:
+            raise ValueError("%s: %s must be a 2-D float32 tensor" % (what, name))
+    if queries.shape[1] != gallery.shape[1] or queries.shape[1] % 4:
+        raise ValueError("%s: queries %s and gallery %s need the same width, a multiple of 4"
+                         % (what, tuple(queries.shape), tuple(gallery.shape)))
+    if queries.device != gallery.device:
+        raise ValueError("%s: queries on %s and gallery on %s: both must be on one device"
+                         % (what, queries.device, gallery.device))
+
+
 def topk(queries, gallery, k):
     """-> (scores fp32 [Nq, k], index int64 [Nq, k]): for each stored query vector the k gallery rows with the largest
     dot product, score descending, ties by lower gallery index (univl_sim_topk).  Text-to-video:
@@ -295,20 +314,105 @@ def topk(queries, gallery, k):
     score has the bits of _mean_pool_similarity(...)[i, j] (text-to-video) or [j, i] (video-to-text) of the same
     vectors.  queries [Nq, H] and gallery [Ng, H]: fp32 CUDA tensors on one device, H a multiple of 4;
     1 <= k <= min(256, Ng)."""
-    for t, name in ((queries, "queries"), (gallery, "gallery")):
-        if not isinstance(t, torch.Tensor) or t.dim() != 2 or t.dtype != torch.float32:
-            raise ValueError("topk: %s must be a 2-D float32 tensor" % name)
-    if queries.shape[1] != gallery.shape[1] or queries.shape[1] % 4:
-        raise ValueError("topk: queries %s and gallery %s need the same width, a multiple of 4"
-                         % (tuple(queries.shape), tuple(gallery.shape)))
+    _check_vectors("topk", queries, gallery)
     if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= min(256, gallery.shape[0]):
         raise ValueError("topk: need 1 <= k <= min(256, %d gallery rows), got %r" % (gallery.shape[0], k))
-    if queries.device != gallery.device:
-        raise ValueError("topk: queries on %s and gallery on %s: both must be on one device"
-                         % (queries.device, gallery.device))
     _check_cuda("topk", queries, gallery)
     if queries.shape[0] == 0:
         return (torch.empty((0, k), dtype=torch.float32, device=queries.device),
                 torch.empty((0, k), dtype=torch.int64, device=queries.device))
     scores, index = ops.sim_topk(queries, gallery, k)
     return scores, index.long()
+
+
+# Ground-truth ranks.  A query's gallery is ranked in topk's order (score descending, then gallery index ascending); its
+# positives are the gallery rows that share its label, and its rank is the 0-based position of its first positive in
+# that order: the number of gallery rows ranked above its best positive, every one of them a negative.
+
+
+def _labels(what, query_labels, gallery_labels, Nq, Ng, device):
+    """-> (query labels, gallery labels), int64 on `device`: each defaults to arange (query i's positive is gallery row
+    i, which needs Nq <= Ng when neither is given); given labels are 1-D int32 / int64 tensors on `device`"""
+    if query_labels is None and gallery_labels is None and Nq > Ng:
+        raise ValueError("%s: without labels query i's positive is gallery row i, which needs Nq <= Ng (got %d > %d)"
+                         % (what, Nq, Ng))
+    out = []
+    for x, n, name in ((query_labels, Nq, "query_labels"), (gallery_labels, Ng, "gallery_labels")):
+        if x is None:
+            out.append(torch.arange(n, device=device))
+            continue
+        if not isinstance(x, torch.Tensor) or x.dtype not in (torch.int32, torch.int64) or x.dim() != 1:
+            raise ValueError("%s: %s must be a 1-D int32 or int64 tensor" % (what, name))
+        if x.shape[0] != n:
+            raise ValueError("%s: %s holds %d labels for %d rows" % (what, name, x.shape[0], n))
+        if x.device != device:
+            raise ValueError("%s: %s is on %s, the vectors on %s" % (what, name, x.device, device))
+        out.append(x.long())
+    return out
+
+
+def _no_positive(what, missing):
+    """one device-to-host read: the count of queries without a positive"""
+    n = int(missing.sum())
+    if n:
+        raise ValueError("%s: %d queries have no positive (no gallery row shares their label)" % (what, n))
+
+
+def _positive_ranges(what, query_labels, gallery_labels):
+    """-> (perm, lo, hi): query i's positives are the gallery rows perm[lo[i]:hi[i]] (ascending), from a stable sort
+    of the gallery labels and a search of it, on the labels' device; ValueError for a query without a positive"""
+    sorted_labels, perm = torch.sort(gallery_labels, stable=True)
+    lo = torch.searchsorted(sorted_labels, query_labels, side="left")
+    hi = torch.searchsorted(sorted_labels, query_labels, side="right")
+    _no_positive(what, lo == hi)
+    return perm, lo, hi
+
+
+def ranks(queries, gallery, query_labels=None, gallery_labels=None):
+    """-> int64 [Nq]: each stored query's rank, the 0-based position of its best positive in topk's order, computed
+    exactly on the device without the [Nq, Ng] matrix (univl_sim_best_positive, univl_sim_rank): rank < k exactly
+    when a positive is in topk(queries, gallery, k), and the first one sits at position rank.  Every score compared has
+    the bits of _mean_pool_similarity's entry for the same vectors.  Text-to-video: ranks(embed_texts(...),
+    embed_videos(...)); video-to-text: the two swapped.  queries and gallery as topk takes them.  Labels: 1-D int32 /
+    int64 tensors on the vectors' device, [Nq] and [Ng]; a query's positives are the gallery rows with its label, and
+    a missing side defaults to arange (so with neither, query i's positive is gallery row i, which needs Nq <= Ng).  A
+    query without a positive raises ValueError, after one device-to-host read of their count."""
+    _check_vectors("ranks", queries, gallery)
+    Nq, Ng = queries.shape[0], gallery.shape[0]
+    ql, gl = _labels("ranks", query_labels, gallery_labels, Nq, Ng, queries.device)
+    _check_cuda("ranks", queries, gallery)
+    if Nq == 0:
+        return torch.empty((0,), dtype=torch.int64, device=queries.device)
+    perm, lo, hi = _positive_ranges("ranks", ql, gl)
+    best_s, best_i = ops.sim_best_positive(queries, gallery, perm.to(ops.I32), lo.to(ops.I32), hi.to(ops.I32))
+    return ops.sim_rank(queries, gallery, best_s, best_i)
+
+
+def ranks_from_scores(scores, query_labels=None, gallery_labels=None):
+    """-> int64 [Nq]: ranks' rule on a dense fp32 [Nq, Ng] CUDA matrix the caller already has (a cross encoder's
+    get_similarity_logits, or ops.SimMatmulFn of stored vectors), with torch ops on the device.  Labels and errors as
+    ranks."""
+    if not isinstance(scores, torch.Tensor) or scores.dim() != 2 or scores.dtype != torch.float32:
+        raise ValueError("ranks_from_scores: scores must be a 2-D float32 tensor")
+    Nq, Ng = scores.shape
+    ql, gl = _labels("ranks_from_scores", query_labels, gallery_labels, Nq, Ng, scores.device)
+    _check_cuda("ranks_from_scores", scores)
+    pos = ql[:, None] == gl[None, :]
+    _no_positive("ranks_from_scores", ~pos.any(1))
+    best_s = torch.where(pos, scores, float("-inf")).amax(1, keepdim=True)
+    best_i = (pos & (scores == best_s)).int().argmax(1, keepdim=True)  # the first positive with the best score
+    j = torch.arange(Ng, device=scores.device)[None, :]
+    return ((scores > best_s) | ((scores == best_s) & (j < best_i))).sum(1)
+
+
+def rank_metrics(ranks):
+    """-> {"R1", "R5", "R10", "MR", "MeanR"} of 0-based ranks (a 1-D tensor or array-like, not empty), as the
+    reference's compute_metrics defines them: R@K the fraction of ranks below K, MR = median + 1 (numpy's median, the
+    mean of the two middle ranks for an even count) and MeanR = mean + 1."""
+    r = ranks.detach().cpu().numpy() if isinstance(ranks, torch.Tensor) else np.asarray(ranks)
+    if r.ndim != 1 or r.size == 0:
+        raise ValueError("rank_metrics: ranks must be 1-D and not empty, got shape %s" % (r.shape,))
+    out = {"R%d" % k: float(np.mean(r < k)) for k in (1, 5, 10)}
+    out["MR"] = float(np.median(r)) + 1
+    out["MeanR"] = float(np.mean(r)) + 1
+    return out
