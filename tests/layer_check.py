@@ -62,13 +62,16 @@ class Call:
 
 
 class Recorder:
-    """install(monkeypatch): replace every ops primitive by a spy that calls the original and records the call"""
+    """install(monkeypatch): replace every ops primitive in `names` by a spy that calls the original and records the
+    call"""
+
+    names = PRIMITIVES
 
     def __init__(self):
         self.calls = []
 
     def install(self, monkeypatch):
-        for name in PRIMITIVES:
+        for name in self.names:
             monkeypatch.setattr(ops, name, self._spy(name, getattr(ops, name)))
         return self
 
@@ -360,29 +363,53 @@ def layer_blocks(kind, params, x, n_seq, S=None, mask=None, enc=None, L=None, Se
             Block("ffn", ffn(20))]
 
 
-def check_layer(calls, blocks, arena, ph, pa, stream0, dy, out, dx, denc=None, fold_rows=None, perturb=(),
-                label="", fused_bwd=True, want=()):
-    """Check one recorded layer call (forward and backward) stage by stage.
-    calls: the Recorder's calls of this layer; blocks: layer_blocks(); stream0: the arena's stream counter before the
-    forward (the reference layer's dropout sites draw stream0 + 1, + 2, ... in block order: attention core, attention
-    LayerNorm, FFN LayerNorm); dy: the upstream gradient; out / dx / denc: what the layer returned (denc: the decoder's
-    encoder gradient, None when not asked for); fold_rows: the first-token layer's (n_seq, S).
-    perturb: reference perturbations for the negative checks ("stream+1", "tile_layout", "swap_p", "no_dy2",
-    "no_dense_scale", "no_fold", "kv_from_x").
-    Returns (tally, param_refs {(block index, key): (ref, bound)}, refs {name: fp64 tensor} for the names in want)."""
-    t = Tally(label)
-    C = Calls(calls)
-    cache = {}
-    first = next(c for c in calls if c.name in DROPOUT_FWD)
-    seed, epoch = first.rng
-    stream = [stream0]
+def attn_out_fwd(t, C, what, ctx, res, w, arena, p_hid=0.0, keep=None):
+    """the attention block's output stages: ao = ctx Wo^T + bo, then y = LN(ao keep / (1 - p) + res) -> (s dict)"""
+    ao = C.next("linear_fwd", what + " o").out
+    check_linear(t, what + " ao", ao, ctx, arena.bf16(w["o"]), w["bo"].detach())
+    y, mean, rstd = C.next("layernorm_fwd", what + " ln").out
+    ln = LNSite(ao, res, w["gamma"], w["beta"], p_hid, keep)
+    ln.check_fwd(t, what + " ln", y, mean, rstd)
+    return dict(ao=ao, y=y, mean=mean, rstd=rstd, ln=ln)
+
+
+def ffn_fwd(t, C, what, x, w, arena, p_hid=0.0, keep_of=None):
+    """the FFN block: pre = x W1^T + b1, h = gelu(pre), fo = h W2^T + b2, y = LN(fo keep / (1 - p) + x); keep_of():
+    the LayerNorm's dropout mask, drawn after the GEMMs (None: p = 0) -> (s dict)"""
+    w1, w2 = arena.bf16(w["w1"]), arena.bf16(w["w2"])
+    c = C.next("linear_fwd", what + " w1")
+    h, pre = c.out, c.args["aux_out"]
+    check_linear_gelu(t, what + " w1", pre, h, x, w1, w["b1"].detach())
+    fo = C.next("linear_fwd", what + " w2").out
+    check_linear(t, what + " fo", fo, h, w2, w["b2"].detach())
+    y, mean, rstd = C.next("layernorm_fwd", what + " ln").out
+    ln = LNSite(fo, x, w["gamma"], w["beta"], p_hid, keep_of() if keep_of is not None else None)
+    ln.check_fwd(t, what + " ln", y, mean, rstd)
+    return dict(mean=mean, rstd=rstd, x=x, h=h, pre=pre, fo=fo, y=y, ln=ln, w1=w1, w2=w2)
+
+
+def block_key_real(b):
+    """the key mask [n_seq, Sk] of an attention block: given by the walk (key_real), or the block's MaskSpec"""
+    kr = getattr(b, "key_real", None)
+    return kr if kr is not None else key_real_of(b.mask, b.n_seq)
+
+
+def check_layer_fwd(t, C, blocks, arena, ph=0.0, pa=0.0, stream=None, rng=None, cache=None, perturb=(),
+                    core=False):
+    """the forward walk of one layer: every block's stages in the reference's order, teacher-forced, consuming the
+    calls from C (a Calls).  stream: [the arena's stream counter before the forward] (advanced per dropout site);
+    rng: (seed, epoch) of the dropout masks (None at p = 0).  core: check the attention core's context and lse here
+    (a forward-only walk; check_layer checks them with the backward).  Returns the blocks' saved tensors (list of
+    dicts); the layer's output is the last one's "y"."""
+    cache = {} if cache is None else cache
+    stream = [0] if stream is None else stream
+    seed, epoch = rng if rng is not None else (0, 0)
 
     def next_stream():
         stream[0] += 1
         return stream[0]
 
     p_attn, p_hid = (ph, pa) if "swap_p" in perturb else (pa, ph)
-    refs = {}
     prev = None
     st = []
     for bi, b in enumerate(blocks):
@@ -412,6 +439,12 @@ def check_layer(calls, blocks, arena, ph, pa, stream0, dy, out, dx, denc=None, f
                 s.update(q=q, kv=kv)
             if not b.fused:
                 ctx, lse = C.next("attention_fwd", what + " core").out
+            kind = "fused" if b.fused else ("long" if max(b.Sq, b.Sk) > ops.SHORT_ATTN_MAX_S else "short")
+            if core:
+                r = ac.reference(q, k, v, b.n_seq, b.Sq, b.Sk, block_key_real(b), b.mask.causal if b.mask else False,
+                                 kind=kind)
+                t.check(what + " core ctx", ctx, r["o"], r["b_o"])
+                t.check(what + " core lse", lse, r["lse"], r["b_lse"])
             sa, sd = next_stream(), next_stream()
             if "stream+1" in perturb:
                 sa += 1
@@ -419,32 +452,40 @@ def check_layer(calls, blocks, arena, ph, pa, stream0, dy, out, dx, denc=None, f
             if "tile_layout" in perturb:
                 layout = "tile"
             keep = attention_keep(layout, seed, sa, epoch, p_attn, b.n_seq, b.Sq, b.Sk, cache)
-            ao = C.next("linear_fwd", what + " o").out
-            check_linear(t, what + " ao", ao, ctx, arena.bf16(w["o"]), w["bo"].detach())
-            y, mean, rstd = C.next("layernorm_fwd", what + " ln").out
             R = xq.shape[0]
-            ln = LNSite(ao, xq, w["gamma"], w["beta"], p_hid,
-                        keep_elem_cached(cache, seed, sd, epoch, p_hid, R, H) if p_hid > 0 else None)
-            ln.check_fwd(t, what + " ln", y, mean, rstd)
-            s.update(mean=mean, rstd=rstd, xq=xq, xkv=xkv, q=q, k=k, v=v, ctx=ctx, lse=lse, ao=ao, y=y, ln=ln, keep=keep, wqkv=wqkv,
-                     kind="fused" if b.fused else ("long" if max(b.Sq, b.Sk) > ops.SHORT_ATTN_MAX_S else "short"))
+            s.update(attn_out_fwd(t, C, what, ctx, xq, w, arena, p_hid,
+                                  keep_elem_cached(cache, seed, sd, epoch, p_hid, R, H) if p_hid > 0 else None))
+            s.update(xq=xq, xkv=xkv, q=q, k=k, v=v, ctx=ctx, lse=lse, keep=keep, wqkv=wqkv, kind=kind)
         else:
             x = prev
-            w = b.w
-            w1, w2 = arena.bf16(w["w1"]), arena.bf16(w["w2"])
-            c = C.next("linear_fwd", what + " w1")
-            h, pre = c.out, c.args["aux_out"]
-            check_linear_gelu(t, what + " w1", pre, h, x, w1, w["b1"].detach())
-            fo = C.next("linear_fwd", what + " w2").out
-            check_linear(t, what + " fo", fo, h, w2, w["b2"].detach())
-            y, mean, rstd = C.next("layernorm_fwd", what + " ln").out
-            sd = next_stream()
-            ln = LNSite(fo, x, w["gamma"], w["beta"], p_hid,
-                        keep_elem_cached(cache, seed, sd, epoch, p_hid, x.shape[0], H) if p_hid > 0 else None)
-            ln.check_fwd(t, what + " ln", y, mean, rstd)
-            s.update(mean=mean, rstd=rstd, x=x, h=h, pre=pre, fo=fo, y=y, ln=ln, w1=w1, w2=w2)
+            sd = []
+
+            def keep_of():
+                sd.append(next_stream())
+                return keep_elem_cached(cache, seed, sd[0], epoch, p_hid, x.shape[0], H) if p_hid > 0 else None
+            s.update(ffn_fwd(t, C, what, x, b.w, arena, p_hid, keep_of))
         st.append(s)
         prev = s["y"]
+    return st
+
+
+def check_layer(calls, blocks, arena, ph, pa, stream0, dy, out, dx, denc=None, fold_rows=None, perturb=(),
+                label="", fused_bwd=True, want=()):
+    """Check one recorded layer call (forward and backward) stage by stage.
+    calls: the Recorder's calls of this layer; blocks: layer_blocks(); stream0: the arena's stream counter before the
+    forward (the reference layer's dropout sites draw stream0 + 1, + 2, ... in block order: attention core, attention
+    LayerNorm, FFN LayerNorm); dy: the upstream gradient; out / dx / denc: what the layer returned (denc: the decoder's
+    encoder gradient, None when not asked for); fold_rows: the first-token layer's (n_seq, S).
+    perturb: reference perturbations for the negative checks ("stream+1", "tile_layout", "swap_p", "no_dy2",
+    "no_dense_scale", "no_fold", "kv_from_x").
+    Returns (tally, param_refs {(block index, key): (ref, bound)}, refs {name: fp64 tensor} for the names in want)."""
+    t = Tally(label)
+    C = Calls(calls)
+    cache = {}
+    first = next(c for c in calls if c.name in DROPOUT_FWD)
+    p_attn = ph if "swap_p" in perturb else pa
+    refs = {}
+    st = check_layer_fwd(t, C, blocks, arena, ph, pa, [stream0], first.rng, cache, perturb)
     # the layer's output is the last block's LayerNorm output
     y_ref = st[-1]["ln"].check_fwd(t, "out", out, st[-1]["mean"], st[-1]["rstd"], want_ref="out" in want)
     if y_ref is not None:

@@ -237,6 +237,19 @@ def meanpool_ref(x, mask, N, S, skip_first, guard_zero, l2norm, dy=None, count_f
 # ---------------------------------------------------------------------------------------------------------
 # similarity matrix and losses (loss.cu sim_fwd / sim_bwd, maxmargin / crossen / milnce kernels)
 # ---------------------------------------------------------------------------------------------------------
+def pooler_sim_ref(u, w, b):
+    """(ref, bound) of univl_pooler_sim_fwd (PoolerSimFn): logit = tanh(u) . w + b per row, u bf16 [N, H], w [H] (or
+    [1, H]), b [1]; MUFU.TANH per element, then an fp32 dot product in H / 32 lane steps and a warp tree"""
+    H = u.shape[1]
+    th = torch.tanh(u.double())
+    wd = w.double().reshape(-1).to(th.device)
+    bd = float(b.double().reshape(-1)[0])
+    ref = th @ wd + bd
+    terms = (th.abs() * wd.abs()).sum(1)
+    bound = ((TANH_REL * th.abs() + TANH_ABS) * wd.abs()).sum(1) + (H / 32 + 8) * U * (terms + abs(bd))
+    return ref, bound
+
+
 def sim_ref(t, v):
     """sim = t v^T: each lane adds H / 32 products in order, then 5 warp levels"""
     H = t.shape[1]

@@ -10,6 +10,7 @@ import torch
 
 from oracle import synth
 from oracle import univl_oracle as O
+from tests.fp8_check import ACC, bf16_out_ok, deq_blocks, deq_rows, gelu_e4m3_bound, ref_codes, ref_scale  # noqa: F401
 from tests.model_util import build_model, to_device
 from univl_b200 import ops
 from univl_b200.modules import modeling
@@ -27,32 +28,6 @@ def _g(seed):
 
 def _randn(shape, seed, scale=1.0):
     return torch.randn(shape, generator=_g(seed)) * scale
-
-
-# ---------------------------------------------------------------------------------------------------------
-# torch statement of the scaling rule, on the CPU (IEEE fp32 division)
-def ref_scale(amax):
-    """2^ceil(log2(amax / 448)) from the bits of the fp32 quotient, at least 2^-126; 1 for amax == 0"""
-    b = (amax.float() / 448.0).view(torch.int32)
-    e = ((b >> 23) & 0xFF) - 127 + ((b & 0x7FFFFF) != 0).int()
-    s = ((e.clamp(min=-126) + 127) << 23).int().view(torch.float32)
-    return torch.where(amax > 0, s, torch.ones_like(s))
-
-
-def ref_codes(x, s):
-    """x / s rounded to nearest even e4m3, saturated (torch's cast turns values above 448 into NaN: clamp first)"""
-    inv = ((254 << 23) - s.view(torch.int32)).view(torch.float32)  # 1 / s, exact
-    return (x.float() * inv).clamp(-448.0, 448.0).to(E4M3)
-
-
-def deq_rows(q, s):
-    """e4m3 [M, K] with scales [K/128, M] -> fp64"""
-    return q.double() * s.t().double().repeat_interleave(128, dim=1)
-
-
-def deq_blocks(q, s):
-    """e4m3 [N, K] with scales [N/128, K/128] -> fp64"""
-    return q.double() * s.double().repeat_interleave(128, dim=0).repeat_interleave(128, dim=1)
 
 
 def _activations(M, K, seed):
@@ -112,20 +87,7 @@ def test_quantize_blocks_is_bit_exact(N, K):
 
 
 # ---------------------------------------------------------------------------------------------------------
-# FP8 GEMM against fp64 on the dequantized operands
-#
-# Bound per element.  The products of e4m3 values are exact in fp32; what is not exact is the tensor cores' sum of a
-# K block's 128 products, whose precision Hopper does not document for 8-bit inputs, and the fp32 promotion of each
-# block.  We bound both together by ACC * sum_k |a_k b_k| (the absolute product sum, fp64) and measure it.  The bf16
-# output adds at most half an ulp, 2^-8 of the value.  ACC = 2^-9 is what the checker needs to be useful: a dropped K
-# block or a wrong block scale moves an element by a block's signed sum, about sqrt(128) / K of the absolute sum for
-# random operands, several times the bound.  Measured on an H100 (the tests below print both): max |err| /
-# sum_k |a_k b_k| is 2.4e-3 at K = 768 and 1.1e-3 at K = 3072 for 300 rows, 5e-4 for one row, most of it the bf16
-# rounding of the output.  What exceeds that rounding, max(|err| - 2^-8 |ref|, 0) / sum_k |a_k b_k| (the most the
-# accumulation can be blamed for), is 5e-6 to 7e-5, 28 or more times below ACC.
-ACC = 2.0 ** -9
-
-
+# FP8 GEMM against fp64 on the dequantized operands, under tests/fp8_check.py's bound (ACC)
 def _gemm_case(M, N, K, seed):
     x = _randn((M, K), seed) * torch.pow(10.0, torch.empty(M, 1).uniform_(-2, 2, generator=_g(seed + 1)))
     a, sa = ops.quantize_e4m3_rows(x.to(torch.bfloat16).to(DEV))
@@ -135,16 +97,6 @@ def _gemm_case(M, N, K, seed):
     ref = A @ B.t() + bias.double()
     absref = A.abs() @ B.abs().t() + bias.double().abs()
     return a, sa, b, sb, bias, A, B, ref, absref
-
-
-def bf16_out_ok(out, ref, absref):
-    """the written bound for the bf16 epilogue; -> (ok, max of |err| / absolute product sum)"""
-    err = (out.double() - ref).abs()
-    acc = ACC * absref
-    ok = bool((err <= 2.0 ** -8 * (ref.abs() + acc) + acc).all())
-    beyond = float(((err - 2.0 ** -8 * ref.abs()).clamp(min=0) / absref).max())
-    print("  max |err| / sum|a b| beyond the bf16 rounding of the output: %.3g (ACC = %.3g)" % (beyond, ACC))
-    return ok, float((err / absref).max())
 
 
 @pytest.mark.parametrize("N", [768, 1536, 3072])
@@ -173,9 +125,7 @@ def test_gemm_fp8_odd_and_short_k(K):
     assert ok, worst
     h, hs = ops.gemm_fp8(a, sa, b, sb, bias, gelu=True)
     g = torch.nn.functional.gelu(ref)
-    ev = 1.13 * ACC * absref + 1e-6 * g.abs()
-    bound = 2.0 ** -4 * (g.abs() + ev) + ev + 2.0 ** -10 * hs.t().double().repeat_interleave(128, dim=1)
-    assert bool(((deq_rows(h, hs) - g).abs() <= bound).all())
+    assert bool(((deq_rows(h, hs) - g).abs() <= gelu_e4m3_bound(g, absref, hs)).all())
 
 
 def test_gemm_fp8_many_waves_and_the_checker_rejects_wrong_results():
@@ -203,10 +153,7 @@ def test_gemm_fp8_gelu_e4m3_epilogue(M, K):
     assert h.shape == (M, N) and h.dtype == E4M3 and hs.shape == (N // 128, M)
     g = torch.nn.functional.gelu(ref)
     deq = deq_rows(h, hs)
-    # the pre-activation error, through gelu_erf (slope at most 1.13), then the e4m3 rounding of the result: half an
-    # ulp, 2^-4 of the value in e4m3's normal range, and half the subnormal spacing, 2^-10 of the scale, below it
-    ev = 1.13 * ACC * absref + 1e-6 * (g.abs() + 1e-30)
-    bound = 2.0 ** -4 * (g.abs() + ev) + ev + 2.0 ** -10 * hs.t().double().repeat_interleave(128, dim=1)
+    bound = gelu_e4m3_bound(g, absref, hs)
     err = (deq - g).abs()
     print("gelu e4m3 M=%d K=%d: max |err| / bound = %.3g" % (M, K, float((err / bound).max())))
     assert bool((err <= bound).all())

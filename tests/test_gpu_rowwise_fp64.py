@@ -403,11 +403,7 @@ def test_pooler_sim_fwd(N):
     out = torch.empty(N, device=DEV)
     call("univl_pooler_sim_fwd", u.data_ptr(), w.data_ptr(), b.data_ptr(), out.data_ptr(), N, H)
     torch.cuda.synchronize()
-    th = torch.tanh(u.double())
-    wd = w.double()
-    ref = th @ wd + float(b)
-    terms = (th.abs() * wd.abs()).sum(1)
-    bound = ((rc.TANH_REL * th.abs() + rc.TANH_ABS) * wd.abs()).sum(1) + (H / 32 + 8) * U * (terms + abs(float(b)))
+    ref, bound = rc.pooler_sim_ref(u, w, b)
     within(out, ref, bound, "pooler_sim_fwd N=%d" % N)
 
 
